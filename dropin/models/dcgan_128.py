@@ -1,4 +1,4 @@
-"""models.dcgan_128 of the reference, served by the sm_100a implementation."""
+"""models.dcgan_128 of the reference, served by the sm_90a implementation."""
 from p2pvg_b200.models.dcgan_128 import *  # noqa: F401,F403
 from p2pvg_b200.models import dcgan_128 as _impl
 

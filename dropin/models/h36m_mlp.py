@@ -1,4 +1,4 @@
-"""``models.h36m_mlp`` of the reference, served by the sm_100a implementation."""
+"""``models.h36m_mlp`` of the reference, served by the sm_90a implementation."""
 from p2pvg_b200.models.h36m_mlp import *  # noqa: F401,F403
 from p2pvg_b200.models import h36m_mlp as _impl
 

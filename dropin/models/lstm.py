@@ -1,4 +1,4 @@
-"""models.lstm of the reference, served by the sm_100a implementation."""
+"""models.lstm of the reference, served by the sm_90a implementation."""
 from p2pvg_b200.models.lstm import *  # noqa: F401,F403
 from p2pvg_b200.models import lstm as _impl
 

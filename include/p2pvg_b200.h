@@ -1,4 +1,4 @@
-/* p2pvg_b200 — C ABI of the sm_100a kernels behind the p2pvg training hot path.
+/* p2pvg_b200 — C ABI of the sm_90a kernels behind the p2pvg training hot path.
  *
  * The reference (yccyenchicheng/p2pvg) has no FFI of its own: its boundary for this path is the Python
  * module API (models/p2p_model.py, models/lstm.py, models/dcgan_64.py, models/dcgan_128.py,
@@ -39,14 +39,15 @@ struct p2pvg_conv_fusion;
 #define P2PVG_ACT_RELU 4   /* models/h36m_mlp.py:33-41 */
 #define P2PVG_ACT_SIGMOID 3 /* models/dcgan_64.py:77 (stand-alone decoder forward; act_fwd only) */
 
+/* 200: the sm_90a library (wgmma tensor-core kernels); p2pvg_has_tcgen05 of version 100 is now p2pvg_has_tc_gemm. */
 int p2pvg_version(void);
 const char* p2pvg_last_error(void);
-/* 1 when the tcgen05/TMA GEMM can be used on this process' device (driver entry points resolved). */
-int p2pvg_has_tcgen05(void);
-/* 0 = pick automatically (tcgen05 for bf16 operands), 1 = force the CUDA-core GEMM, 2 = force tcgen05 */
+/* 1 when the wgmma/TMA GEMM can be used on this process' device (driver entry points resolved). */
+int p2pvg_has_tc_gemm(void);
+/* 0 = pick automatically (wgmma for bf16 operands), 1 = force the CUDA-core GEMM, 2 = force wgmma */
 int p2pvg_set_gemm_impl(int impl);
 /* p2pvg_gemm `flags` (per call; there is no process-global precision state):
- *   P2PVG_GEMM_TF32          fp32 operands MAY run on tcgen05 kind::tf32 (LSTM GEMMs of the bf16 training mode).  The
+ *   P2PVG_GEMM_TF32          fp32 operands MAY run on wgmma .tf32 (LSTM GEMMs of the bf16 training mode).  The
  *                            tensor-core kernel needs both operands K-major, K >= 32, 16-byte aligned bases and row
  *                            pitches (TMA); any other fp32 GEMM of such a call runs on the exact CUDA-core kernel --
  *                            a documented, precision-INCREASING dispatch between two kernels of this library (never a
@@ -60,7 +61,7 @@ int p2pvg_set_gemm_impl(int impl);
  *   a_mn=0: A[m*lda+k] (K-major), a_mn=1: A[k*lda+m];  b_mn=0: B[n*ldb+k], b_mn=1: B[k*ldb+n].
  * Replaces the library GEMMs behind nn.Conv2d / nn.ConvTranspose2d (models/dcgan_64.py:8,20,43,64,76 after
  * lowering), nn.Linear and nn.LSTMCell (models/lstm.py:13-17,54-57) and their autograd backward.
- * bf16 operands run on tcgen05 tensor cores (fp32 accumulation in TMEM); fp32 operands on CUDA cores (exact) unless
+ * bf16 operands run on the tensor cores (wgmma, fp32 accumulation in registers); fp32 operands on CUDA cores (exact) unless
  * `flags` allows TF32 (see above).  Documented dispatch between two kernels of this library: bf16 operands whose base
  * address or row pitch is not 16-byte aligned (not expressible as a TMA tensor map) run on the CUDA-core kernel with the
  * same arithmetic contract; p2pvg_set_gemm_impl(2) turns that case into P2PVG_ERR_UNSUPPORTED.
@@ -69,7 +70,7 @@ int p2pvg_gemm(const void* A, int in_dtype, int a_mn, int64_t lda, const void* B
                int64_t ldc, int M, int N, int K, int accumulate, const float* bias, const void* addend, int64_t ldd,
                void* workspace, size_t ws_bytes, int flags, void* stream);
 
-/* Implicit-GEMM 4x4 / stride-2 / pad-1 convolution family on NHWC bf16 tensors (TMA 4-D pixel-box loads feeding tcgen05;
+/* Implicit-GEMM 4x4 / stride-2 / pad-1 convolution family on NHWC bf16 tensors (TMA 4-D pixel-box loads feeding wgmma;
  * no im2col / col2im buffers).  H, W = size of the SMALL map (the big map is 2H x 2W).
  *   kind 0: c_small[N,H,W,Cn] = conv_s2(a_big[N,2H,2W,Ck]) . b[Cn,(kh,kw,Ck)] + bias       nn.Conv2d(.,.,4,2,1) forward
  *           (models/dcgan_64.py:8) and the data-gradient of nn.ConvTranspose2d(.,.,4,2,1) (models/dcgan_64.py:20)
@@ -201,9 +202,9 @@ int p2pvg_lstm_pointwise_bwd(const float* dh, const float* dc_next, const float*
                              float* dgates, float* dc_prev, int B, int R, void* stream);
 /* Whole-sequence recurrence of one nn.LSTMCell layer in ONE persistent launch (the W_hh slice of a CTA stays on chip for all
  * timesteps).  tf32 = 1 dispatches by hidden size: R in {64,128,256}: thread-block clusters of 8 CTAs, hardware cluster barrier per
- * timestep; R = 512: clusters of 16 CTAs (non-portable size), slabs of 16 / 32 / 48 batch rows per cluster chosen so that the
- * resident clusters cover the batch in one wave, backward reduction scattered through distributed shared memory, the part of the
- * weight slice that does not fit the registers in shared memory (16-row slabs) or tensor memory (larger slabs).  tf32 = 0 (and
+ * timestep; R = 512: clusters of 16 CTAs (non-portable size), forward slabs of 16 / 32 / 48 batch rows per cluster chosen so that
+ * the resident clusters cover the batch in as few waves as possible, backward in 16-row slabs with the reduction scattered through
+ * distributed shared memory; the part of the weight slice that does not fit the registers lives in shared memory.  tf32 = 0 (and
  * P2PVG_LSTM_CLUSTER=0): cooperative grid with a grid barrier per timestep, exact fp32 FFMA products.
  *   forward : gates_s = pre_s + b_hh + h_{s-1}.W_hh^T -> (i,f,g,o) -> c_s, h_s       pre [S,B,4R] = x-part incl. b_ih
  *             gates [S,B,4R] out (activations), hs / cs [S+1,B,R] with slot 0 = initial state (zeros, models/lstm.py:21-27)

@@ -88,7 +88,7 @@ def kernels_for(device):
 
 
 class CudaKernels:
-    """Launches the sm_100a kernels on the current torch CUDA stream of its device."""
+    """Launches the sm_90a kernels on the current torch CUDA stream of its device."""
 
     name = "cuda"
 
@@ -150,8 +150,8 @@ class CudaKernels:
         (this view only; passed per call as P2PVG_GEMM_TF32)."""
         self.gemm_flags = 1 if mode else 0
 
-    def has_tcgen05(self) -> bool:
-        return bool(self.lib.p2pvg_has_tcgen05())
+    def has_tc_gemm(self) -> bool:
+        return bool(self.lib.p2pvg_has_tc_gemm())
 
     # -- GEMM ------------------------------------------------------------------------------
     def gemm(self, A, B, C, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldc=None, accumulate=False, bias=None,

@@ -1,5 +1,5 @@
 // extern "C" surface of libp2pvg_b200.so (declared in include/p2pvg_b200.h): argument checking,
-// thread-local error state, GEMM dispatch (tcgen05 vs CUDA-core).
+// thread-local error state, GEMM dispatch (wgmma vs CUDA-core).
 #include <stdarg.h>
 #include <string.h>
 
@@ -105,16 +105,16 @@ int p2pvg_convt_c1_loss_impl(const void*, const void*, int, const int*, const fl
 int p2pvg_adam_legacy_impl(float*, const float*, float*, float*, long long, double, double, double, double, const int*, cudaStream_t);
 int p2pvg_scale_impl(float*, long long, float, cudaStream_t);
 
-static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 tcgen05
+static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
 
 #define ST ((cudaStream_t)stream)
 
 extern "C" {
 
-int p2pvg_version(void) { return 100; }
+int p2pvg_version(void) { return 200; }
 const char* p2pvg_last_error(void) { return g_err; }
-int p2pvg_has_tcgen05(void) { return p2pvg_gemm_tc_available(); }
+int p2pvg_has_tc_gemm(void) { return p2pvg_gemm_tc_available(); }
 int p2pvg_set_gemm_impl(int impl) {
   if (impl < 0 || impl > 2) return P2PVG_ERR_BAD_ARG;
   g_gemm_impl = impl;
@@ -127,7 +127,7 @@ int p2pvg_gemm(const void* A, int in_dtype, int a_mn, int64_t lda, const void* B
   P2PVG_REQUIRE(A && B && C, P2PVG_ERR_BAD_ARG, "gemm: null operand");
   P2PVG_REQUIRE(M >= 0 && N >= 0 && K >= 0, P2PVG_ERR_BAD_ARG, "gemm: negative size");
   bool want_tc = (in_dtype == P2PVG_BF16) && g_gemm_impl != 1;
-  // fp32 operands (LSTM / parity mode) always run on the CUDA cores; "forced tcgen05" only makes the bf16 path
+  // fp32 operands (LSTM / parity mode) always run on the CUDA cores; "forced wgmma" only makes the bf16 path
   // refuse to fall back when an operand is not TMA-compatible.
   if (want_tc)
     return p2pvg_gemm_tc(A, a_mn, lda, B, b_mn, ldb, C, c_dtype, ldc, M, N, K, accumulate, bias, addend, ldd, workspace, ws_bytes, ST);

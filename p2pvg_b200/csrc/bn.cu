@@ -336,7 +336,7 @@ __global__ void bn_ema_kernel(float* __restrict__ rmean, float* __restrict__ rva
 
 __attribute__((unused)) inline int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 64;
+  const long long cap = 132LL * 64;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

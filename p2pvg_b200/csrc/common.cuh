@@ -1,4 +1,4 @@
-// Shared helpers for the p2pvg_b200 sm_100a kernels.
+// Shared helpers for the p2pvg_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

@@ -1,6 +1,6 @@
 // Implicit-GEMM 4x4 / stride-2 / pad-1 convolution family on NHWC bf16 tensors (no im2col / col2im buffers).
-// Same persistent tcgen05 skeleton as gemm_tc.cu (TMA -> 128B-swizzled smem -> tcgen05.mma kind::f16 -> TMEM ->
-// tcgen05.ld epilogue, double-buffered accumulator); what changes is how an operand tile is fetched:
+// Same persistent wgmma skeleton as gemm_tc.cu (TMA -> 128B-swizzled smem -> wgmma.mma_async in one MMA warpgroup ->
+// shared-memory staging buffer -> epilogue warps); what changes is how an operand tile is fetched:
 //
 //   "pixel box" tiles: P consecutive NHW pixels of the SMALL map (H x W per image) are a rectangular box
 //   {bw = W, bh, bn}; the operand rows for filter tap (kh,kw) are the BIG-map pixels (2y+kh-1, 2x+kw-1), i.e. one
@@ -25,15 +25,17 @@ namespace {
 using namespace tc;
 
 constexpr int BLOCK_M = 128;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;   // warps 0..3 epilogue, 4..7 MMA warpgroup, 8 TMA producer (as in gemm_tc.cu)
 constexpr int A_STAGE_BYTES = BLOCK_M * 128;
 
+// 128 x 64 / 128 x 128 tiles: one warpgroup holds the whole fp32 accumulator in registers (64 / 128 per thread)
 template <int BN> struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128) ? 6 : 8;  // 128x256 tiles: 87 FLOP per smem-fill byte (L2 -> SM
-                                                                        // bandwidth bounds the 128x128 tiles at ~1100 TFLOP/s)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512;
+  static constexpr int STAGES = (BN == 128) ? 4 : 7;
+  static constexpr int ACC_LD = BN + 4;
+  static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 + 512;
 };
 
 struct Geom {
@@ -109,19 +111,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                  float2* __restrict__ stat_partial) {
   using C_ = Cfg<BN>;
   constexpr bool A_MN = (KIND == 1), B_MN = (KIND != 0);
-  constexpr int UMMA_K = 16;
-  constexpr uint32_t TMEM_COLS = 2 * BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES);
+  float* accs = reinterpret_cast<float*>(smem + C_::STAGES * C_::STAGE_BYTES);   // [BLOCK_M][ACC_LD] staging buffer
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES + C_::ACC_BYTES);
   uint64_t* empty_bar = full_bar + C_::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + C_::STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint64_t* bres_bar = tmem_empty_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bres_bar + 1);
-  // resident-weight mode (kind 0, BN = 64): weights at [0, 9 * 8 KB), A ring of 7 x 16 KB behind them
+  uint64_t* acc_full_bar = empty_bar + C_::STAGES;
+  uint64_t* acc_empty_bar = acc_full_bar + 1;
+  uint64_t* bres_bar = acc_empty_bar + 1;
+  // resident-weight mode (kind 0, BN = 64): weights at [0, 9 * 8 KB), A ring of 6 x 16 KB behind them
   const bool bres = (KIND == 0) && (BN == 64) && g.bres != 0;
-  constexpr int BRES_B_BYTES = 9 * 64 * 128, BRES_STAGES = 7;
+  constexpr int BRES_B_BYTES = 9 * 64 * 128, BRES_STAGES = 6;
+  static_assert(BN != 64 || BRES_B_BYTES + BRES_STAGES * A_STAGE_BYTES <= C_::STAGES * C_::STAGE_BYTES, "resident weights + A ring");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M, tiles_n = (g.Ntot + BN - 1) / BN;
@@ -135,28 +136,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     for (int s = 0; s < C_::STAGES; s++) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 128);   // every thread of the MMA warpgroup
     }
-    for (int a = 0; a < 2; a++) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 4);
-    }
+    mbar_init(acc_full_bar, 128);
+    mbar_init(acc_empty_bar, 4);       // one arrival per epilogue warp
     mbar_init(bres_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    regs_producer();
+    if (warp == 8 && lane == 0) {
       uint32_t it = 0;
       if (bres) {   // all weight taps once: [tap][64 output channels][64 input channels]
         mbar_expect_tx(bres_bar, (uint32_t)(g.ks * g.ks) * 64 * 128);
@@ -165,8 +157,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         // tile decode with as few integer divisions as possible: the producer thread is the latency-critical one
         // kind 2: the output-parity phase is the FASTEST tile index, so that the four phases of one pixel tile run on four
-        // CTAs at the same time and share the A tile through L2 (phase-major order re-read A from DRAM once per phase:
-        // ncu r01 measured 4.0x the algorithmic A bytes).  Kinds 0 / 2 never split K.
+        // CTAs at the same time and share the A tile through L2 (in phase-major order every phase would re-read A from
+        // DRAM).  Kinds 0 / 2 never split K.
         const int ph = (KIND == 2) ? (t & 3) : 0;
         const int t2 = (KIND == 2) ? (t >> 2) : t;
         const int z = (splits == 1) ? 0 : t2 / tiles_mn, r = t2 - z * tiles_mn;
@@ -266,56 +258,58 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                             ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-      const uint32_t smem0 = smem_u32(smem);
-      const uint64_t da0 = A_MN ? make_desc(smem0, 64 * 128, 1024) : make_desc(smem0, 0, 1024);
-      const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, 64 * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
-      uint32_t it = 0, lt = 0;
-      if (bres) {
-        mbar_wait(bres_bar, 0);   // the resident weights have landed
-        tcgen05_fence_after();
+  } else if (warp >= 4) {
+    // ===================== MMA warpgroup =====================
+    regs_worker();
+    const int wt = threadIdx.x - 128;
+    const uint32_t smem0 = smem_u32(smem);
+    const uint64_t da0 = A_MN ? make_desc(smem0, 64 * 128, 1024) : make_desc(smem0, 0, 1024);
+    const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, 64 * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
+    uint32_t it = 0, lt = 0;
+    if (bres) mbar_wait(bres_bar, 0);   // the resident weights have landed
+    const uint64_t da0r = make_desc(smem0 + BRES_B_BYTES, 0, 1024), db0r = make_desc(smem0, 0, 1024);
+    float acc[2][BN / 2];
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
+      int z = 0;
+      if (splits > 1) z = t / tiles_mn;   // only kind 1 splits K (one phase)
+      const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
+      int prev = -1;   // stage of the previous K block: released once its MMAs have completed
+      for (int kb = kb0; kb < kb1; kb++, it++) {
+        // (both divisors are compile-time constants: no runtime division in the per-K-block path)
+        const int s = bres ? (int)(it % BRES_STAGES) : (int)(it % C_::STAGES);
+        const uint32_t par = (bres ? (it / BRES_STAGES) : (it / C_::STAGES)) & 1;
+        mbar_wait(&full_bar[s], par);
+        // descriptors of stage 0 / k 0 are built once; the start-address field (bits 0-13, address >> 4) is advanced by
+        // plain additions
+        const uint64_t stage_off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
+        const uint64_t a_off = bres ? (uint64_t)((uint32_t)s * (uint32_t)(A_STAGE_BYTES >> 4)) : stage_off;
+        const uint64_t b_off = bres ? (uint64_t)((uint32_t)kb * (uint32_t)((64 * 128) >> 4)) : stage_off;   // resident: tap kb
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        wgmma_fence();
+        wgmma_kblock<false, BN, A_MN, B_MN>(acc, (bres ? da0r : da0) + a_off, (bres ? db0r : db0) + b_off, kb == kb0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
       }
-      const uint64_t da0r = make_desc(smem0 + BRES_B_BYTES, 0, 1024), db0r = make_desc(smem0, 0, 1024);
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
-        int z = 0;
-        if (splits > 1) z = t / tiles_mn;   // only kind 1 splits K (one phase)
-        const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
-        const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
-        mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1);
-        tcgen05_fence_after();
-        const uint32_t tmem_c = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; kb++, it++) {
-          // (both divisors are compile-time constants: no runtime division in the single producer / issuer threads)
-          const int s = bres ? (int)(it % BRES_STAGES) : (int)(it % C_::STAGES);
-          const uint32_t par = (bres ? (it / BRES_STAGES) : (it / C_::STAGES)) & 1;
-          mbar_wait(&full_bar[s], par);
-          tcgen05_fence_after();
-          // descriptors of stage 0 / k 0 are built once; the start-address field (bits 0-13, address >> 4) is advanced by
-          // plain additions -- the single issuing thread has ~32 clk per 128x64x16 MMA to spend
-          const uint64_t stage_off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
-          const uint64_t a_off = bres ? (uint64_t)((uint32_t)s * (uint32_t)(A_STAGE_BYTES >> 4)) : stage_off;
-          const uint64_t b_off = bres ? (uint64_t)((uint32_t)kb * (uint32_t)((64 * 128) >> 4)) : stage_off;   // resident: tap kb
-#pragma unroll
-          for (int k = 0; k < 64 / UMMA_K; k++) {
-            const uint64_t da = (bres ? da0r : da0) + a_off + (uint64_t)(k * ((A_MN ? UMMA_K * 128 : 32) >> 4));
-            const uint64_t db = (bres ? db0r : db0) + b_off + (uint64_t)(k * ((B_MN ? UMMA_K * 128 : 32) >> 4));
-            umma_bf16(tmem_c, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full_bar[acc]);
-      }
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+      mbar_wait(acc_empty_bar, (lt & 1) ^ 1);   // the epilogue has drained the previous tile
+      acc_to_smem<BN>(acc, accs, C_::ACC_LD, wt);
+      mbar_arrive(acc_full_bar);
     }
   } else {
     // ===================== epilogue =====================
-    const int q = warp & 3;
+    regs_worker();
+    const int q = warp;
     __shared__ float bias_s[2 * BN];
     // BatchNorm forward statistics fused into the epilogue: per-warp column sums (sum y, sum y^2) of the tile, double-
-    // buffered by accumulator so that tile t+1 may write while the sums of tile t are still being combined
+    // buffered by tile parity so that tile t+1 may write while the sums of tile t are still being combined
     __shared__ float2 stat_s[STAT ? 2 * 4 * BN : 1];
     constexpr bool do_stat = STAT;   // a separate instantiation: the statistics cost ~50 registers in this epilogue
     uint32_t lt = 0;
@@ -325,7 +319,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int z = (splits == 1) ? 0 : t2 / tiles_mn, r = t2 - z * tiles_mn;
       const int mt = (tiles_n == 1) ? r : r / tiles_n, nt = (tiles_n == 1) ? 0 : r - mt * tiles_n;
       const int n0 = nt * BN;
-      const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
+      const uint32_t acc = lt & 1;   // bias_s / stat_s half of this tile
       const int rt = q * 32 + lane;  // row within the tile
       long long out_row = (long long)mt * BLOCK_M + rt;
       long long add_row = 0;
@@ -363,28 +357,21 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const bool abf = g.add_bf16 != 0;
       float4 a4[16];  // addend of the next 64 columns, requested before the accumulator is waited for
       if (use_add) addend_load64(a4, addend, aoff0, abf);
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tcgen05_fence_after();
+      mbar_wait(acc_full_bar, lt & 1);
 #pragma unroll 1
       for (int pr = 0; pr < BN / 64; pr++) {
-        // two 32-column chunks per round: both tcgen05.ld in flight before the wait; after the last round the
-        // accumulator goes back to the MMA warp *before* the global stores
-        uint32_t v2[64];
-        const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(pr * 64);
-        tmem_ld32(taddr, v2);
-        tmem_ld32(taddr + 32, v2 + 32);
         if (pr > 0 && use_add) addend_load64(a4, addend, aoff0 + pr * 64, abf);
-        tmem_ld_wait_dep(v2);
-        tmem_ld_wait_dep(v2 + 32);
-        if (pr == BN / 64 - 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-        }
 #pragma unroll
         for (int h = 0; h < 2; h++) {
+          // 32 columns at a time; after the last chunk is read the staging buffer goes back to the MMA warpgroup *before*
+          // the global stores
           const int c = pr * 2 + h;
-          const uint32_t* v = v2 + 32 * h;
+          uint32_t v[32];
+          acc_row32(accs + rt * C_::ACC_LD + c * 32, v);
+          if (c == BN / 32 - 1) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(acc_empty_bar);
+          }
           const int nbase = n0 + c * 32;
           if (nbase >= g.Ntot) continue;             // warp-uniform
           if (!row_ok && !do_stat) continue;         // rows past the end only matter as zeros of the column sums
@@ -474,270 +461,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// kind 2 with the FOUR output-parity phases fused into one tile (ConvTranspose2d 4x4 / s2 / p1 forward, Conv2d data gradient).
-// A tile = 128 small-map pixels x (4 phases x 64 output channels) = 128 x 256 accumulator columns; column block p = 2a + b
-// is output parity (a, b).  out[2y+a, 2x+b] = sum over the 2x2 taps of phase (a, b) of x[y+dy, x+dx] . W[ky, kx]:
-// the nine shifted pixel boxes (dy, dx) in {-1,0,1}^2 are each fetched ONCE per channel chunk and multiplied (N = 64
-// tcgen05.mma) against the weight taps of every phase that uses the shift: (0,0) serves 4 phases, an edge shift 2, a corner
-// shift 1 -- 16 (shift, phase) products per chunk like the phase-by-phase kernel, but 9 A tiles instead of 16: 123 FLOP per
-// shared-memory fill byte instead of 43 (64 output channels) / 65 (128), i.e. off the L2 -> SM operand-fill limit that held
-// those layers at 520 - 660 TFLOP/s (DESIGN.md).  Output channels beyond 64 are further tiles (n-tile nt = channels
-// [64 nt, 64 nt + 64)).  Epilogue as in conv_gemm_kernel (bias, fp32 skip addend, bf16 / fp32 store, optional BatchNorm
-// statistics), one 64-column round per phase.
-__device__ __forceinline__ bool phase_uses(int a, int d) { return d == 0 || (d < 0 ? a == 0 : a == 1); }
-__device__ __forceinline__ int phase_tap(int a, int d) { return d == 0 ? a + 1 : (a ? 0 : 3); }
-// The accumulator holds the phases in the column-block order [p0, p1, p3, p2]: then the phases served by one shift are
-// NEIGHBOURS for the centre shift (all four) and three of the four edge shifts, so one 256- / 128-wide tcgen05.mma covers them
-// instead of four / two 64-wide ones (10 instead of 16 MMAs per 16-wide K slice and channel chunk: the single issuing thread
-// was the limit of the 64-wide version).  The centre shift comes FIRST in every tile so that all four column blocks start
-// accumulating together.
-__device__ __forceinline__ int cb_phase(int cb) { return cb == 2 ? 3 : cb == 3 ? 2 : cb; }   // involution: block <-> phase
-__device__ __forceinline__ void shift_of(int so, int& dy, int& dx) {
-  // 0 centre; 1..4 edges (-1,0) (+1,0) (0,+1) (0,-1); 5..8 corners
-  dy = (so == 1 || so == 5 || so == 6) ? -1 : (so == 2 || so == 7 || so == 8) ? 1 : 0;
-  dx = (so == 4 || so == 5 || so == 7) ? -1 : (so == 3 || so == 6 || so == 8) ? 1 : 0;
-}
-__device__ __forceinline__ bool cb_used(int cb, int dy, int dx) {
-  const int p = cb_phase(cb);
-  return phase_uses(p >> 1, dy) && phase_uses(p & 1, dx);
-}
-
-template <bool STAT>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-convt4_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* __restrict__ Cv, int c_bf16,
-              long long ldc, Geom g, const float* __restrict__ bias, const float* __restrict__ addend, const int* __restrict__ grp_src,
-              float2* __restrict__ stat_partial) {
-  constexpr int BN = 256;
-  using C_ = Cfg<BN>;
-  constexpr int UMMA_K = 16;
-  constexpr int B_TILE_BYTES = 64 * 128;   // 64 reduction channels x 64 output channels (MN-major)
-  constexpr uint32_t TMEM_COLS = 2 * BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C_::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + C_::STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M, tiles_n = g.Cn / 64;
-  const int num_tiles = tiles_m * tiles_n;
-  const int cchunks = g.Ck / 64;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C_::STAGES; s++) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; a++) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 4);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    // ===================== TMA producer: one stage = one shifted pixel box + the weight taps of the phases using it
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int mt = (tiles_n == 1) ? t : t / tiles_n, nt = (tiles_n == 1) ? 0 : t - mt * tiles_n;
-        int pn0, py0;
-        pix_block(mt, 128, g.H, g.W, g.bh128, g.bn128, pn0, py0);
-        for (int cc = 0; cc < cchunks; cc++) {
-          const int c0 = cc * 64;
-#pragma unroll
-          for (int so = 0; so < 9; so++, it++) {
-            int dy, dx;
-            shift_of(so, dy, dx);
-            const int nb = (dy == 0 ? 2 : 1) * (dx == 0 ? 2 : 1);
-            const int s = it % C_::STAGES;
-            const uint32_t par = (it / C_::STAGES) & 1;
-            mbar_wait(&empty_bar[s], par ^ 1);
-            uint8_t* sa = smem + s * C_::STAGE_BYTES;
-            uint8_t* sb = sa + A_STAGE_BYTES;
-            mbar_expect_tx(&full_bar[s], A_STAGE_BYTES + nb * B_TILE_BYTES);
-            tma_load_4d(&tmA, &full_bar[s], sa, c0, dx, py0 + dy, pn0);
-            int j = 0;
-#pragma unroll
-            for (int cb = 0; cb < 4; cb++) {   // weight taps in accumulator column-block order
-              if (!cb_used(cb, dy, dx)) continue;
-              const int p = cb_phase(cb);
-              const int ky = phase_tap(p >> 1, dy), kx = phase_tap(p & 1, dx);
-              tma_load_2d(&tmB, &full_bar[s], sb + j * B_TILE_BYTES, (ky * 4 + kx) * g.Cn + nt * 64, c0);
-              j++;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | (0u << 15) | (1u << 16) | ((uint32_t)(BLOCK_M >> 4) << 24);
-      const uint32_t smem0 = smem_u32(smem);
-      const uint64_t da0 = make_desc(smem0, 0, 1024);
-      const uint64_t db0 = make_desc(smem0 + A_STAGE_BYTES, 64 * 128, 1024);
-      uint32_t it = 0, lt = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
-        const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
-        mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1);
-        tcgen05_fence_after();
-        for (int cc = 0; cc < cchunks; cc++) {
-#pragma unroll
-          for (int so = 0; so < 9; so++, it++) {
-            int dy, dx;
-            shift_of(so, dy, dx);
-            const int s = it % C_::STAGES;
-            const uint32_t par = (it / C_::STAGES) & 1;
-            mbar_wait(&full_bar[s], par);
-            tcgen05_fence_after();
-            const uint64_t stage_off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
-            int j = 0;
-#pragma unroll
-            for (int cb = 0; cb < 4;) {
-              if (!cb_used(cb, dy, dx)) { cb++; continue; }
-              int len = 1;
-              while (cb + len < 4 && cb_used(cb + len, dy, dx)) len++;   // neighbouring column blocks: one wide MMA
-              const uint32_t idesc = idesc0 | ((uint32_t)((64 * len) >> 3) << 17);
-              const uint32_t tmem_c = tmem_base + acc * BN + cb * 64;
-#pragma unroll
-              for (int k = 0; k < 64 / UMMA_K; k++) {
-                const uint64_t da = da0 + stage_off + (uint64_t)(k * (32 >> 4));
-                const uint64_t db = db0 + stage_off + (uint64_t)(j * (B_TILE_BYTES >> 4)) + (uint64_t)(k * ((UMMA_K * 128) >> 4));
-                // the centre shift of channel chunk 0 is the first product of every column block of the tile
-                umma_bf16(tmem_c, da, db, idesc, (cc > 0 || so > 0 || k > 0) ? 1u : 0u);
-              }
-              j += len;
-              cb += len;
-            }
-            umma_commit(&empty_bar[s]);
-          }
-        }
-        umma_commit(&tmem_full_bar[acc]);
-      }
-    }
-  } else {
-    // ===================== epilogue: one 64-column round per output-parity phase =====================
-    const int q = warp & 3;
-    __shared__ float bias_s[64];
-    __shared__ float2 stat_s[STAT ? 2 * 4 * BN : 1];
-    uint32_t lt = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
-      const int mt = (tiles_n == 1) ? t : t / tiles_n, nt = (tiles_n == 1) ? 0 : t - mt * tiles_n;
-      const int n0 = nt * 64;
-      const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
-      const int rt = q * 32 + lane;
-      int pn0, py0;
-      pix_block(mt, 128, g.H, g.W, g.bh128, g.bn128, pn0, py0);
-      const int HW = g.H * g.W;
-      int nn, yy, xx;
-      if (HW >= 128) { nn = 0; yy = rt / g.W; xx = rt - yy * g.W; }
-      else { nn = rt / HW; const int rem = rt - nn * HW; yy = rem / g.W; xx = rem - yy * g.W; }
-      const int n = pn0 + nn, y = py0 + yy;
-      const bool row_ok = (n < g.N) && (y < g.H);
-      int n2 = n;
-      if (addend != nullptr && row_ok) n2 = grp_src[n / g.imgs_per_group] * g.imgs_per_group + (n % g.imgs_per_group);
-      const bool use_add = addend != nullptr && row_ok;
-      epi_bar_sync();   // every warp is done with bias_s of the previous tile
-      if (rt < 64) bias_s[rt] = (bias != nullptr) ? bias[n0 + rt] : 0.f;
-      epi_bar_sync();
-      const bool abf = g.add_bf16 != 0;
-      float4 a4[16];
-      if (use_add)   // skip addend of the first column block's phase (p0), requested before the accumulator is waited for
-        addend_load64(a4, addend, (((long long)n2 * (2 * g.H) + 2 * y) * (2 * g.W) + 2 * xx) * g.Cn + n0, abf);
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int cbi = 0; cbi < 4; cbi++) {
-        const int p = cb_phase(cbi);   // accumulator column block cbi holds output parity p
-        const int oy = 2 * y + (p >> 1), ox = 2 * xx + (p & 1);
-        const long long out_row = ((long long)n * (2 * g.H) + oy) * (2 * g.W) + ox;
-        uint32_t v2[64];
-        const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(cbi * 64);
-        tmem_ld32(taddr, v2);
-        tmem_ld32(taddr + 32, v2 + 32);
-        if (cbi > 0 && use_add) addend_load64(a4, addend, (((long long)n2 * (2 * g.H) + oy) * (2 * g.W) + ox) * g.Cn + n0, abf);
-        tmem_ld_wait_dep(v2);
-        tmem_ld_wait_dep(v2 + 32);
-        if (cbi == 3) {   // the accumulator goes back to the MMA warp before the last stores
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const uint32_t* v = v2 + 32 * h;
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(bias_s + 32 * h + j);
-            f[j] = __uint_as_float(v[j]) + b4.x; f[j + 1] = __uint_as_float(v[j + 1]) + b4.y;
-            f[j + 2] = __uint_as_float(v[j + 2]) + b4.z; f[j + 3] = __uint_as_float(v[j + 3]) + b4.w;
-          }
-          if (use_add) addend_add32(f, a4, h, abf);
-          if (STAT) {
-            float s1[32], s2[32];
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const float r = row_ok ? (c_bf16 ? bf16_round(f[j]) : f[j]) : 0.f;
-              s1[j] = r;
-              s2[j] = r * r;
-            }
-            const float cs = warp_colsum32(s1, lane), cq = warp_colsum32(s2, lane);
-            stat_s[(acc * 4 + q) * BN + p * 64 + h * 32 + lane] = make_float2(cs, cq);
-          }
-          if (!row_ok) continue;
-          if (c_bf16) {
-            bf16* crow = reinterpret_cast<bf16*>(Cv) + out_row * ldc + n0 + 32 * h;
-#pragma unroll
-            for (int j = 0; j < 32; j += 16)
-              st_global_256(crow + j, pack_bf16x2(f[j], f[j + 1]), pack_bf16x2(f[j + 2], f[j + 3]), pack_bf16x2(f[j + 4], f[j + 5]),
-                            pack_bf16x2(f[j + 6], f[j + 7]), pack_bf16x2(f[j + 8], f[j + 9]), pack_bf16x2(f[j + 10], f[j + 11]),
-                            pack_bf16x2(f[j + 12], f[j + 13]), pack_bf16x2(f[j + 14], f[j + 15]));
-          } else {
-            float* crow = reinterpret_cast<float*>(Cv) + out_row * ldc + n0 + 32 * h;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8)
-              st_global_256(crow + j, __float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
-                            __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7]));
-          }
-        }
-      }
-      if (STAT) {
-        epi_bar_sync();
-        for (int i = q * 32 + lane; i < BN; i += 128) {
-          const int p = i >> 6, ch = i & 63;
-          const float2 a = stat_s[(acc * 4 + 0) * BN + i], b = stat_s[(acc * 4 + 1) * BN + i];
-          const float2 c2 = stat_s[(acc * 4 + 2) * BN + i], d = stat_s[(acc * 4 + 3) * BN + i];
-          stat_partial[((long long)mt * 4 + p) * g.Cn + n0 + ch] = make_float2((a.x + b.x) + (c2.x + d.x), (a.y + b.y) + (c2.y + d.y));
-        }
-      }
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 // C[M, N] = sum_z partial[z]; transposed != 0: the partials are [z][N][M] (kind 1 with swapped operand roles)
@@ -760,14 +483,8 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_enc = nullptr;
 std::once_flag g_once2;
-int g_sms = 148;
-int g_k1_wide_max = 1 << 30;  // kind 1: 256-wide tiles while there are at most this many 128-wide output tiles (P2PVG_K1_WIDE_MAX)
-int g_bn256 = 1;  // P2PVG_CONV_BN256=0 keeps the 128-wide tiles (A/B comparison)
-int g_attr[2][3][3] = {};
-int g_convt4_max_cn = 64;   // kind 2 with at most this many output channels: the four parity phases fused into one tile (P2PVG_CONVT4_MAX_CN;
-                            // 0 = off).  Measured (C2 step, B200): 64 -> -0.36 ms; 128 -> +0.1 ms (the N = 64 MMAs of the fused tile issue twice as
-                            // many instructions as the 128-wide phase tiles, which outweighs the saved operand fills)
-int g_convt4_attr[2] = {};
+int g_sms = 132;
+int g_attr[2][3][2] = {};
 int g_bres = 1;      // 64 -> 64 channel 3x3 layers: weights resident in shared memory (P2PVG_CONV_BRES=0 disables)
 int g_k1_swap = 1;   // kind 1 / 4 with 64 output channels: swapped operand roles (P2PVG_K1_SWAP=0 disables)
 
@@ -779,16 +496,10 @@ void resolve2() {
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
     g_enc = reinterpret_cast<EncodeTiledFn>(fn);
   (void)cudaGetLastError();
-  const char* e = getenv("P2PVG_CONV_BN256");
-  if (e != nullptr && e[0] == '0') g_bn256 = 0;
   const char* br = getenv("P2PVG_CONV_BRES");
   if (br != nullptr && br[0] == '0') g_bres = 0;
   const char* sw = getenv("P2PVG_K1_SWAP");
   if (sw != nullptr && sw[0] == '0') g_k1_swap = 0;
-  const char* f4 = getenv("P2PVG_CONVT4_MAX_CN");
-  if (f4 != nullptr) g_convt4_max_cn = atoi(f4);
-  const char* w = getenv("P2PVG_K1_WIDE_MAX");
-  if (w != nullptr) g_k1_wide_max = atoi(w);
 }
 
 int map2d(CUtensorMap* m, const void* base, long long dim0, long long dim1, long long ld, int box1) {
@@ -852,7 +563,7 @@ int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype,
              const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
              float2* stat_partial) {
   auto kern = conv_gemm_kernel<KIND, BN, STAT>;
-  int& done = g_attr[STAT][KIND][BN == 256 ? 2 : BN == 128];
+  int& done = g_attr[STAT][KIND][BN == 128];
   if (!done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
     if (e != cudaSuccess) {
@@ -866,28 +577,6 @@ int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype,
   kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, st>>>(ta, tb, C, c_dtype == P2PVG_BF16, ldc, g, accumulate, bias, addend, grp_src, partial,
                                                       kb_per_split, splits, stat_partial);
   return p2pvg_check_launch("conv_gemm");
-}
-
-int launch_convt4(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, const float* bias,
-                  const float* addend, const int* grp_src, float2* stat_partial, cudaStream_t st) {
-  const bool stat = stat_partial != nullptr;
-  int& done = g_convt4_attr[stat];
-  if (!done) {
-    cudaError_t e = stat ? cudaFuncSetAttribute(convt4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<256>::SMEM_BYTES)
-                         : cudaFuncSetAttribute(convt4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<256>::SMEM_BYTES);
-    if (e != cudaSuccess) {
-      p2pvg_set_error("conv_gemm (fused phases): cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return P2PVG_ERR_CUDA;
-    }
-    done = 1;
-  }
-  const long long tiles = (long long)cdiv(g.M, BLOCK_M) * (g.Cn / 64);
-  const int grid = (int)(tiles < g_sms ? tiles : g_sms);
-  if (stat)
-    convt4_kernel<true><<<grid, NUM_THREADS, Cfg<256>::SMEM_BYTES, st>>>(ta, tb, C, c_dtype == P2PVG_BF16, ldc, g, bias, addend, grp_src, stat_partial);
-  else
-    convt4_kernel<false><<<grid, NUM_THREADS, Cfg<256>::SMEM_BYTES, st>>>(ta, tb, C, c_dtype == P2PVG_BF16, ldc, g, bias, addend, grp_src, nullptr);
-  return p2pvg_check_launch("conv_gemm (fused phases)");
 }
 
 }  // namespace
@@ -936,12 +625,11 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     g.M = (int)pix; g.Ntot = Cn;
     rc = map4d(&ta, a, N, g.st * H, g.st * W, Ck, W, g.bh128, g.bn128, g.st);
     if (rc) return rc;
-    const int BN = (Cn % 256 == 0 && g_bn256) ? 256 : Cn > 64 ? 128 : 64;
+    const int BN = Cn > 64 ? 128 : 64;
     rc = map2d(&tb, b, (long long)taps * Ck, Cn, ldb, BN);
     if (rc) return rc;
     const int nkb = taps * (Ck / 64);
     g.bres = (BN == 64 && Cn == 64 && Ck == 64 && taps <= 9 && g_bres) ? 1 : 0;
-    if (BN == 256) return launch<0, 256>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
     if (BN == 128) return launch<0, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
     return launch<0, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
   }
@@ -952,11 +640,7 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     rc = map2d(&tb, b, 16LL * Cn, Ck, ldb, 64);  // MN-major weight [Ck rows][16*Cn]
     if (rc) return rc;
     const int nkb = 4 * (Ck / 64);
-    if (Cn % 64 == 0 && Cn <= g_convt4_max_cn && !accumulate && (ldc % 16 == 0) && (c_dtype == P2PVG_F32 || ldc % 32 == 0) &&
-        ((uintptr_t)c & 31) == 0 && (addend == nullptr || ((uintptr_t)addend & 15) == 0))
-      return launch_convt4(ta, tb, c, c_dtype, ldc, g, bias, addend, grp_src, stat_partial, st);
-    const int BN = (Cn % 256 == 0 && g_bn256) ? 256 : Cn > 64 ? 128 : 64;
-    if (BN == 256) return launch<2, 256>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
+    const int BN = Cn > 64 ? 128 : 64;
     if (BN == 128) return launch<2, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
     return launch<2, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
   }
@@ -981,9 +665,7 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     rc = map4d(&tb, b, N, g.st * H, g.st * W, Cn, g.bw64, g.bh64, g.bn64, g.st);
     if (rc) return rc;
   }
-  // a wide tile spans several filter taps when Cn == 64; 256-wide tiles pay off while there are few output tiles (measured)
-  const bool wide = !g.swap && g.Ntot % 256 == 0 && g_bn256 && (long long)cdiv(Cm, BLOCK_M) * (g.Ntot / 128) <= g_k1_wide_max;
-  const int BN = wide ? 256 : (g.Ntot % 128 == 0) ? 128 : 64;
+  const int BN = (g.Ntot % 128 == 0) ? 128 : 64;
   const long long tiles = (long long)cdiv(g.M, BLOCK_M) * cdiv(g.Ntot, BN);
   // split-K chosen by a small cost model (units: time of one 128x128x64 k-block on one SM, ~0.22 us): the persistent grid
   // processes ceil(items / SMs) rounds of (k-blocks per item + fixed per-item cost); partial sums cost a write + read
@@ -1004,13 +686,12 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   int kbps = cdiv(nkb, splits);
   splits = cdiv(nkb, kbps);
   float* partial = splits > 1 ? reinterpret_cast<float*>(ws) : nullptr;
-  if (BN == 256) rc = launch<1, 256>(ta, tb, c, c_dtype, ldc, g, accumulate, nullptr, nullptr, nullptr, partial, splits, kbps, st);
-  else if (BN == 128) rc = launch<1, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, nullptr, nullptr, nullptr, partial, splits, kbps, st);
+  if (BN == 128) rc = launch<1, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, nullptr, nullptr, nullptr, partial, splits, kbps, st);
   else rc = launch<1, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, nullptr, nullptr, nullptr, partial, splits, kbps, st);
   if (rc) return rc;
   if (splits > 1) {
     long long total = (long long)Cm * taps * Cn;
-    int blocks = (int)((total + 255) / 256 > 1184 ? 1184 : (total + 255) / 256);
+    int blocks = (int)((total + 255) / 256 > g_sms * 8 ? g_sms * 8 : (total + 255) / 256);
     conv_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(partial, splits, (float*)c, ldc, Cm, taps * Cn, accumulate, g.swap);
     return p2pvg_check_launch("conv_splitk_reduce");
   }

@@ -324,7 +324,7 @@ __global__ void __launch_bounds__(256) transpose_batched_kernel(const TS* __rest
 
 inline int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 64;
+  const long long cap = 132LL * 64;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

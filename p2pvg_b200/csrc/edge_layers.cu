@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(256) convT_thin_out_kernel(const T* __restrict
 
 inline int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -160,7 +160,7 @@ int p2pvg_conv_thin_in_impl(const void* x, int dtype, const float* w, const floa
   const long long npix = (long long)N * (H / 2) * (W / 2);
   const int planes = 256 / (Co / vec);
   long long blocks = (npix + planes - 1) / planes;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (Ci == 1) {
     DISPATCH_DTYPE(dtype, T, (conv_thin_in_kernel<T, 1><<<(int)blocks, 256, smem, st>>>((const T*)x, w, bias, (T*)y, N, H, W, Co)));
   } else {

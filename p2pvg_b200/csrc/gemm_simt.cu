@@ -1,5 +1,5 @@
 // CUDA-core GEMM (fp32 accumulate) used by the fp32 parity mode, by the LSTM path, and as the
-// bisecting fallback for the tcgen05 GEMM (P2PVG_GEMM=simt).  Handles every shape / leading
+// bisecting fallback for the wgmma GEMM (P2PVG_GEMM=simt).  Handles every shape / leading
 // dimension / operand major-ness without alignment requirements.
 //
 //   C[M,N] = (accumulate ? C : 0) + opA(A) * opB(B) + bias[n] + addend[m,n]

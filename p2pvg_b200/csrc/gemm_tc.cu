@@ -1,6 +1,6 @@
-// bf16 GEMM on the 5th-generation tensor cores (sm_100a): TMA (cp.async.bulk.tensor) stages 128B-swizzled
-// operand tiles in shared memory, one elected thread issues tcgen05.mma (cta_group::1, kind::f16) with the
-// fp32 accumulator in TMEM, four epilogue warps read it back with tcgen05.ld and store.
+// bf16 GEMM on the Hopper tensor cores (sm_90a): TMA (cp.async.bulk.tensor) stages 128B-swizzled operand tiles in
+// shared memory, one warpgroup issues wgmma.mma_async (fp32 accumulator in registers) and hands each finished tile to
+// four epilogue warps through a shared-memory staging buffer; they add bias / addend and store.
 //
 //   C[M,N] = (accumulate ? C : 0) + opA(A)*opB(B) + bias[n] + addend[m,n]          (same contract as gemm_simt)
 //
@@ -9,8 +9,8 @@
 // transposed copies of activations are ever materialised.  Split-K (grid.z) with a deterministic second
 // pass covers the weight gradients, whose output is tiny and whose reduction dimension is huge.
 //
-// Warp roles (192 threads): warp 0 = TMA producer + TMEM allocator, warp 1 = MMA issuer,
-// warps 2..5 = epilogue (TMEM lane quarter = warp_idx % 4).
+// Warp roles (384 threads): warps 0..3 = epilogue (one tile row per thread), warps 4..7 = the MMA warpgroup,
+// warp 8 = TMA producer (warps 9..11 only complete its warpgroup).
 #include <cuda.h>
 
 #include <mutex>
@@ -22,23 +22,25 @@ namespace {
 constexpr int BLOCK_M = 128;
 constexpr int ROW_BYTES = 128;  // one SWIZZLE_128B row: 64 bf16 or 32 fp32 (tf32) along the contiguous dimension
 constexpr int A_STAGE_BYTES = BLOCK_M * ROW_BYTES;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;
 
 template <int BN> struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * ROW_BYTES;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN == 128) ? 6 : 8;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
+  static constexpr int STAGES = (BN == 128) ? 4 : 7;
+  static constexpr int ACC_LD = BN + 4;   // staging row pitch in floats: the row-per-thread float4 reads are conflict-free
+  static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
 };
 
-// PTX wrappers (mbarrier / TMA / tcgen05 / TMEM): tc_common.cuh, shared with conv_gemm.cu
+// PTX wrappers (mbarrier / TMA / wgmma): tc_common.cuh, shared with conv_gemm.cu
 using namespace tc;
 
 // ------------------------------------------------------------------ the kernel
 
 // Persistent: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...  A tile is
 // (split z, m-tile, n-tile) with the n-tile fastest, so CTAs running at the same time share the A rows in L2.
-// The accumulator is double-buffered in TMEM (2 x BN columns): the epilogue of tile i overlaps the MMAs of tile i+1.
+// The MMA warpgroup accumulates tile i+1 in registers while the epilogue drains tile i from the staging buffer.
 template <typename TIn, int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* __restrict__ Cv,
@@ -47,17 +49,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   using C_ = Cfg<BN>;
   constexpr int ELEM = sizeof(TIn);
   constexpr int BLOCK_K = ROW_BYTES / ELEM;  // elements of K per pipeline stage (K-major) / rows per stage (MN-major)
-  constexpr int UMMA_K = 32 / ELEM;          // K per tcgen05.mma: 16 for bf16, 8 for tf32
   constexpr bool TF32 = (ELEM == 4);
-  constexpr uint32_t TMEM_COLS = 2 * BN;
   static_assert(!(TF32 && (A_MN || B_MN)), "tf32 path supports K-major operands only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES);
+  float* accs = reinterpret_cast<float*>(smem + C_::STAGES * C_::STAGE_BYTES);   // [BLOCK_M][ACC_LD] staging buffer
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES + C_::ACC_BYTES);
   uint64_t* empty_bar = full_bar + C_::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + C_::STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
+  uint64_t* acc_full_bar = empty_bar + C_::STAGES;
+  uint64_t* acc_empty_bar = acc_full_bar + 1;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + BLOCK_M - 1) / BLOCK_M, tiles_n = (N + BN - 1) / BN;
@@ -68,27 +68,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C_::STAGES; s++) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 128);   // every thread of the MMA warpgroup
     }
-    for (int a = 0; a < 2; a++) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 4);  // one arrival per epilogue warp
-    }
+    mbar_init(acc_full_bar, 128);
+    mbar_init(acc_empty_bar, 4);  // one arrival per epilogue warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    regs_producer();
+    if (warp == 8 && lane == 0) {
       uint32_t it = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const int z = (splits == 1) ? 0 : t / tiles_mn, r = t - z * tiles_mn;   // fast path: no integer division without split-K
@@ -118,48 +109,47 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (single thread) =====================
-    if (lane == 0) {
-      // instruction descriptor: D=f32, operand format, majors, N>>3, M>>4
-      const uint32_t fmt = TF32 ? 2u : 1u;  // 1 = bf16, 2 = tf32
-      const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                             ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-      const uint32_t smem0 = smem_u32(smem);
-      const uint64_t da0 = A_MN ? make_desc(smem0, BLOCK_K * 128, 1024) : make_desc(smem0, 0, 1024);
-      const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, BLOCK_K * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
-      uint32_t it = 0, lt = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
-        const int z = (splits == 1) ? 0 : t / tiles_mn;
-        const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
-        const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
-        mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1);  // epilogue has drained this accumulator
-        tcgen05_fence_after();
-        const uint32_t tmem_c = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; kb++, it++) {
-          const int s = it % C_::STAGES;
-          const uint32_t ph = (it / C_::STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tcgen05_fence_after();
-          const uint32_t sa = smem_u32(smem + s * C_::STAGE_BYTES);
-          const uint32_t sb = sa + A_STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; k++) {
-            // K-major: 32 B further inside the 128 B swizzle row; MN-major: UMMA_K rows of 128 B further
-            const uint64_t da = A_MN ? make_desc(sa + k * UMMA_K * 128, BLOCK_K * 128, 1024) : make_desc(sa + k * 32, 0, 1024);
-            const uint64_t db = B_MN ? make_desc(sb + k * UMMA_K * 128, BLOCK_K * 128, 1024) : make_desc(sb + k * 32, 0, 1024);
-            const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
-            if (TF32) umma_tf32(tmem_c, da, db, idesc, accum);
-            else umma_bf16(tmem_c, da, db, idesc, accum);
-          }
-          umma_commit(&empty_bar[s]);  // frees the smem stage once these MMAs have read it
-        }
-        umma_commit(&tmem_full_bar[acc]);  // accumulator of this tile complete
+  } else if (warp >= 4) {
+    // ===================== MMA warpgroup =====================
+    regs_worker();
+    const int wt = threadIdx.x - 128;
+    const uint32_t smem0 = smem_u32(smem);
+    const uint64_t da0 = A_MN ? make_desc(smem0, BLOCK_K * 128, 1024) : make_desc(smem0, 0, 1024);
+    const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, BLOCK_K * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
+    float acc[2][BN / 2];
+    uint32_t it = 0, lt = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
+      const int z = (splits == 1) ? 0 : t / tiles_mn;
+      const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
+      int prev = -1;   // stage of the previous K block: released once its MMAs have completed
+      for (int kb = kb0; kb < kb1; kb++, it++) {
+        const int s = it % C_::STAGES;
+        const uint32_t ph = (it / C_::STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint64_t off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        wgmma_fence();
+        wgmma_kblock<TF32, BN, A_MN, B_MN>(acc, da0 + off, db0 + off, kb == kb0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
       }
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+      mbar_wait(acc_empty_bar, (lt & 1) ^ 1);   // the epilogue has drained the previous tile
+      acc_to_smem<BN>(acc, accs, C_::ACC_LD, wt);
+      mbar_arrive(acc_full_bar);
     }
   } else {
-    // ===================== epilogue: TMEM -> registers -> global =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
+    // ===================== epilogue: staging buffer -> registers -> global =====================
+    regs_worker();
+    const int q = warp;  // rows [32 q, 32 q + 32) of the tile
     const bool split = (partial != nullptr);
     __shared__ float bias_s[2 * BN];
     uint32_t lt = 0;
@@ -167,35 +157,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int z = (splits == 1) ? 0 : t / tiles_mn, r = t - z * tiles_mn;   // fast path: no integer division without split-K
       const int mt_ = (tiles_n == 1) ? r : r / tiles_n;
         const int m0 = mt_ * BLOCK_M, n0 = (r - mt_ * tiles_n) * BN;
-      const uint32_t acc = lt & 1, acc_ph = (lt >> 1) & 1;
+      const uint32_t bsel = lt & 1;   // bias_s half of this tile
       const long long m = (long long)m0 + q * 32 + lane;
       const bool row_ok = m < M;
       // stage the bias slice of this tile in shared memory while the MMAs are still running
       if (bias != nullptr && !split) {
-        for (int i = q * 32 + lane; i < BN; i += 128) bias_s[acc * BN + i] = (n0 + i < N) ? bias[n0 + i] : 0.f;
+        for (int i = q * 32 + lane; i < BN; i += 128) bias_s[bsel * BN + i] = (n0 + i < N) ? bias[n0 + i] : 0.f;
         epi_bar_sync();
       }
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tcgen05_fence_after();
+      mbar_wait(acc_full_bar, lt & 1);
 #pragma unroll 1
       for (int pr = 0; pr < BN / 64; pr++) {
-        // two 32-column chunks per round: both tcgen05.ld in flight before one wait; after the last round the
-        // accumulator is handed back to the MMA warp *before* the global stores
-        uint32_t v2[64];
-        const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(pr * 64);
-        tmem_ld32(taddr, v2);
-        tmem_ld32(taddr + 32, v2 + 32);
-        tmem_ld_wait_dep(v2);
-        tmem_ld_wait_dep(v2 + 32);
-        if (pr == BN / 64 - 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-        }
 #pragma unroll
         for (int h = 0; h < 2; h++) {
+          // 32 columns at a time; after the last chunk is read the staging buffer goes back to the MMA warpgroup *before*
+          // the global stores
           const int c = pr * 2 + h;
-          const uint32_t* v = v2 + 32 * h;
+          uint32_t v[32];
+          acc_row32(accs + (q * 32 + lane) * C_::ACC_LD + c * 32, v);
+          if (c == BN / 32 - 1) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(acc_empty_bar);
+          }
           const int nbase = n0 + c * 32;
           if (!row_ok || nbase >= N) continue;
           if (split) {
@@ -215,7 +198,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
           for (int j = 0; j < 32; j++) f[j] = __uint_as_float(v[j]);
           if (bias) {
-            const float* bs = bias_s + acc * BN + c * 32;
+            const float* bs = bias_s + bsel * BN + c * 32;
 #pragma unroll
             for (int j = 0; j < 32; j += 4) {
               const float4 b4 = *reinterpret_cast<const float4*>(bs + j);
@@ -289,11 +272,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 // second pass of split-K: C = sum_z partial[z] + bias + addend + (accumulate ? C : 0)
@@ -321,7 +299,7 @@ EncodeTiledFn g_encode = nullptr;
 std::once_flag g_once;
 int g_attr_done[2][2][2][2] = {};
 
-int g_num_sms = 148;
+int g_num_sms = 132;
 
 void resolve_driver() {
   int dev = 0, sms = 0;
@@ -425,12 +403,12 @@ int p2pvg_gemm_tc(const void* A, int a_mn, long long lda, const void* B, int b_m
   else rc = make_map(&tb, B, K, N, ldb, BN);
   if (rc) return rc;
 
-  // split-K when the output has too few tiles to fill the 148 SMs and the reduction is long
+  // split-K when the output has too few tiles to fill the SMs and the reduction is long
   const int nkb = cdiv(K, BLOCK_K);
   const long long tiles = (long long)cdiv(M, BLOCK_M) * cdiv(N, BN);
   int splits = 1;
   if (tiles < 120 && nkb >= 16) {
-    long long want = (2 * 148 + tiles - 1) / tiles;
+    long long want = (2 * g_num_sms + tiles - 1) / tiles;
     long long maxs = nkb / 8;
     splits = (int)(want < maxs ? want : maxs);
     if (splits < 1) splits = 1;
@@ -461,7 +439,7 @@ int p2pvg_gemm_tc(const void* A, int a_mn, long long lda, const void* B, int b_m
   if (rc) return rc;
   if (splits > 1) {
     long long total = (long long)M * N;
-    int blocks = (int)((total + 255) / 256 > 148 * 8 ? 148 * 8 : (total + 255) / 256);
+    int blocks = (int)((total + 255) / 256 > g_num_sms * 8 ? g_num_sms * 8 : (total + 255) / 256);
     if (c_dtype == P2PVG_BF16)
       splitk_reduce_kernel<bf16><<<blocks, 256, 0, st>>>(partial, splits, (bf16*)C, ldc, M, N, accumulate, bias, (const bf16*)addend, ldd);
     else

@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(256) sigmoid_mse_kernel(const T* __restrict__ 
 
 // K5 of SURVEY.md §2.2: the last decoder layer -- ConvTranspose2d(2*64 -> 1, 4, 2, 1) + Sigmoid (models/dcgan_64.py:75-79) --
 // fused with the reconstruction / CPC loss (nn.MSELoss, models/p2p_model.py:254,256).  The 16-tap products of every input
-// pixel come from the tcgen05 GEMMs (col [N*Hi*Wi, 16] for the decoder path, col2 for the shared skip path); this kernel
+// pixel come from the tensor-core GEMMs (col [N*Hi*Wi, 16] for the decoder path, col2 for the shared skip path); this kernel
 // gathers the four taps of an output pixel from both, adds the bias, applies the sigmoid, accumulates the squared error
 // against the target frame and writes d(loss)/d(raw) -- one pass, no raw-output tensor, 32-bit index arithmetic.
 template <typename T, int C>
@@ -210,7 +210,7 @@ int p2pvg_adam_legacy_impl(float* p, const float* g, float* m, float* v, long lo
   if (n == 0) return P2PVG_OK;
   P2PVG_REQUIRE(step_ptr != nullptr, P2PVG_ERR_BAD_ARG, "adam: step counter pointer is null");
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   adam_legacy_kernel<<<(int)blocks, 256, 0, st>>>(p, g, m, v, n, beta1, beta2, eps, lr, step_ptr);
   return p2pvg_check_launch("adam_legacy");
 }
@@ -218,7 +218,7 @@ int p2pvg_adam_legacy_impl(float* p, const float* g, float* m, float* v, long lo
 int p2pvg_scale_impl(float* x, long long n, float a, cudaStream_t st) {
   if (n == 0) return P2PVG_OK;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   scale_kernel<<<(int)blocks, 256, 0, st>>>(x, n, a);
   return p2pvg_check_launch("scale");
 }

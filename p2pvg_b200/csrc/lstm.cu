@@ -249,7 +249,7 @@ __global__ void act_bwd_kernel(const float* __restrict__ dy, const float* __rest
 
 inline int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -312,8 +312,8 @@ int p2pvg_colsum_impl(const void* x, int dtype, long long rows, int cols, long l
     if (rc) return rc;
     return p2pvg_colsum_impl(tmp, P2PVG_F32, FOLD, cols, cols, out, accumulate, ws, (size_t)1024 * FOLD * cols * sizeof(float), st);
   }
-  // enough chunks to fill the machine (148 SMs x a few blocks), at least 64 rows per chunk
-  long long want = (148LL * 8) / cdiv(cols, 32) + 1;
+  // enough chunks to fill the machine (132 SMs x a few blocks), at least 64 rows per chunk
+  long long want = (132LL * 8) / cdiv(cols, 32) + 1;
   long long maxc = (rows + 63) / 64;
   long long nchunk = want < maxc ? want : maxc;
   if (nchunk < 1) nchunk = 1;

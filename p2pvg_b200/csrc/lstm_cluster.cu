@@ -8,7 +8,7 @@
 //     through shared memory instead of the 128 KB weight slice;
 //   * steps are separated by the hardware cluster barrier (arrive.release / wait.acquire, ~0.2 us) instead of a grid-wide
 //     barrier; the exchanged state (h_s forward, dG_s backward) is exactly what the kernel has to write to global memory
-//     anyway -- the other 7 CTAs read it back from L2 (measured: DSMEM scatter is limited to ~20 B/clk per SM, slower);
+//     anyway -- the other 7 CTAs read it back from L2 instead of receiving a distributed-shared-memory scatter;
 //   * everything that does not depend on the recurrence (input-side pre-activations, saved gates) is requested before
 //     the barrier.
 // The recurrent product runs as mma.sync m16n8k8 TF32 with fp32 accumulation; activations use MUFU approximations whose
@@ -399,7 +399,7 @@ static int mt2_above() {
   return v;
 }
 
-// 8 clusters of 8 CTAs are co-resident on a B200 (measured): slabs of 32 rows keep up to 256 rows in one wave
+// slabs of 32 rows above mt2_above() rows: fewer clusters of 8 CTAs, so that large batches need fewer waves
 int p2pvg_lstm_cluster_fwd_impl(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
                                 int R, cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;

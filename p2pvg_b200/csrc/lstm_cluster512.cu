@@ -63,30 +63,6 @@ __device__ __forceinline__ void st_cluster_v2(uint32_t addr, float a, float b) {
   asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 
-// 16 consecutive 32-bit columns of this thread's tensor-memory lane (lane = 32 * (warp % 4) + lane id): what a thread stores it
-// reads back in the same registers
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-               "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-               "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                 "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr)
-               : "memory");
-}
-// tcgen05.wait::ld naming the destination registers of the outstanding load, so that no use of them is scheduled above the wait
-__device__ __forceinline__ void tmem_wait_ld16(uint32_t* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]),
-                 "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-               :
-               : "memory");
-}
-
 // ------------------------------------------------------------------------------------------------ forward
 // Warp w = (kh, ng): K half kh = w >> 2 (256 wide = 32 k8 steps), n-tile group ng = w & 3 (4 tiles of 8 gate columns).
 // k8 steps [0, KR) of a warp are register-resident, [KR, 32) shared-memory-resident.
@@ -420,196 +396,6 @@ lstm_cl16_bwd_kernel(const float* __restrict__ dhtop, const float* __restrict__ 
   }
 }
 
-// ------------------------------------------------------------------------------------------------ backward, 32 / 48-row slabs
-// Same algorithm as lstm_cl16_bwd_kernel for slabs of MT m16 tiles.  The receive slots grow with the slab (64 KB per 16 rows,
-// double-buffered) and leave no shared memory for a weight half, so the half that does not fit the registers lives in TENSOR
-// MEMORY (256 KB per SM, otherwise unused by this kernel): 256 columns, written once with tcgen05.st in the fragment-major order
-// the mma.sync B operands need and read back 16 columns per k8 step with tcgen05.ld, double-buffered against the MMAs.  The
-// m16 tiles run one after the other (32 accumulator registers).  Why: only 7 clusters of 16 CTAs are resident at a time
-// (cudaOccupancyMaxActiveClusters), so 256 rows in 16-row slabs need three passes over the sequence; 48-row slabs need one.
-template <int MT>
-__global__ void __launch_bounds__(NT, 1)
-lstm_cl16_bwd_tm_kernel(const float* __restrict__ dhtop, const float* __restrict__ whh, const float* __restrict__ gates,
-                        const float* __restrict__ cs, float* __restrict__ dG, int S, int B) {
-  constexpr int MB = 16 * MT, K4 = 4 * R, KL = 4 * UBc;
-  constexpr int NTL = 8, KS = KL / 8, KR = 8, KTM = KS - KR;
-  constexpr int LDA = KL + PAD;
-  constexpr int CPT = (MB * UBc) / NT;                  // 2 MT cells per thread
-  constexpr uint32_t TCOLS = 2 * KTM * NTL * 2;          // 256 columns: [warp >> 2][k][tile][2]
-  static_assert(KTM % 2 == 0 && TCOLS == 256, "tensor-memory layout");
-  extern __shared__ __align__(16) float sm[];
-  float* recv = sm;                                     // [2][CS src][MB][UBc]
-  float* As = recv + 2 * CS * MB * UBc;                 // [MB][LDA]
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(As + MB * LDA);
-  const int tid = threadIdx.x;
-  const uint32_t rank = cluster_rank();
-  const int r0 = (blockIdx.x / CS) * MB, u0 = (int)rank * UBc;
-  const int warp = tid >> 5, lane = tid & 31, gq = lane >> 2, tq = lane & 3;
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(tslot)), "r"(TCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tbase = *reinterpret_cast<volatile uint32_t*>(tslot);
-  // this warp's lane quarter and column block
-  const uint32_t tw = tbase + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * (KTM * NTL * 2));
-
-  // B fragments: B[k = kk][n] = W_hh[q(kk)][n], n = 64 warp + 8 t + gq
-  uint32_t wreg[NTL][KR][2];
-#pragma unroll
-  for (int t = 0; t < NTL; t++) {
-    const int n = warp * 64 + t * 8 + gq;
-#pragma unroll
-    for (int k = 0; k < KR; k++) {
-      const int kk0 = k * 8 + tq, kk1 = kk0 + 4;
-      wreg[t][k][0] = to_tf32(whh[(long long)((kk0 / UBc) * R + u0 + kk0 % UBc) * R + n]);
-      wreg[t][k][1] = to_tf32(whh[(long long)((kk1 / UBc) * R + u0 + kk1 % UBc) * R + n]);
-    }
-  }
-  for (int k = KR; k < KS; k++) {
-    uint32_t v[2 * NTL];
-    const int kk0 = k * 8 + tq, kk1 = kk0 + 4;
-    const float* w0 = whh + (long long)((kk0 / UBc) * R + u0 + kk0 % UBc) * R + warp * 64 + gq;
-    const float* w1 = whh + (long long)((kk1 / UBc) * R + u0 + kk1 % UBc) * R + warp * 64 + gq;
-#pragma unroll
-    for (int t = 0; t < NTL; t++) {
-      v[2 * t] = to_tf32(w0[t * 8]);
-      v[2 * t + 1] = to_tf32(w1[t * 8]);
-    }
-    tmem_st16(tw + (uint32_t)((k - KR) * 2 * NTL), v);
-  }
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-
-  int crow[CPT], cuu[CPT];
-  bool cok[CPT];
-  float dc_reg[CPT];
-#pragma unroll
-  for (int h = 0; h < CPT; h++) {
-    const int ci = tid + NT * h;
-    crow[h] = ci / UBc;
-    cuu[h] = ci - crow[h] * UBc;
-    cok[h] = (r0 + crow[h]) < B;
-    dc_reg[h] = 0.f;
-  }
-  uint32_t raddr[2];   // base of recv in CTA 2*warp and 2*warp+1
-  raddr[0] = map_to_cta(recv, 2 * warp);
-  raddr[1] = map_to_cta(recv, 2 * warp + 1);
-  __syncthreads();
-  cluster_arrive();   // every CTA of the cluster has started (distributed shared memory may be written from here on)
-  cluster_wait();
-
-  for (int it = 0; it < S; it++) {
-    const int s = S - 1 - it;
-    float ig[CPT], fg[CPT], gg[CPT], og[CPT], cprev[CPT], cnow[CPT], dht[CPT];
-#pragma unroll
-    for (int h = 0; h < CPT; h++) {
-      ig[h] = fg[h] = gg[h] = og[h] = cprev[h] = cnow[h] = dht[h] = 0.f;
-      if (cok[h]) {
-        const long long gbase = ((long long)s * B + r0 + crow[h]) * K4 + u0 + cuu[h];
-        ig[h] = __ldcs(gates + gbase); fg[h] = __ldcs(gates + gbase + R);
-        gg[h] = __ldcs(gates + gbase + 2LL * R); og[h] = __ldcs(gates + gbase + 3LL * R);
-        const long long o = ((long long)s * B + r0 + crow[h]) * R + u0 + cuu[h];   // cs[s] = c_{s-1}, cs[s+1] = c_s
-        cprev[h] = __ldcs(cs + o);
-        cnow[h] = __ldcs(cs + o + (long long)B * R);
-        dht[h] = __ldcs(dhtop + o);
-      }
-    }
-    float rec[CPT];
-#pragma unroll
-    for (int h = 0; h < CPT; h++) rec[h] = 0.f;
-    if (it > 0) {
-      cluster_wait();   // the 16 partial products for my units have arrived in recv[it & 1]
-      const float* rb = recv + (it & 1) * CS * MB * UBc;
-#pragma unroll
-      for (int h = 0; h < CPT; h++) {
-        float r = 0.f;
-#pragma unroll
-        for (int src = 0; src < CS; src++) r += rb[(src * MB + crow[h]) * UBc + cuu[h]];   // fixed order: deterministic
-        rec[h] = r;
-      }
-    }
-#pragma unroll
-    for (int h = 0; h < CPT; h++) {
-      float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;
-      if (cok[h]) {
-        const float dh = dht[h] + rec[h];
-        const float tc = fast_tanh(cnow[h]);
-        const float dc = dh * og[h] * (1.f - tc * tc) + dc_reg[h];
-        dc_reg[h] = dc * fg[h];
-        d0 = dc * gg[h] * ig[h] * (1.f - ig[h]);
-        d1 = dc * cprev[h] * fg[h] * (1.f - fg[h]);
-        d2 = dc * ig[h] * (1.f - gg[h] * gg[h]);
-        d3 = dh * tc * og[h] * (1.f - og[h]);
-        const long long gbase = ((long long)s * B + r0 + crow[h]) * K4 + u0 + cuu[h];
-        dG[gbase] = d0;
-        dG[gbase + R] = d1;
-        dG[gbase + 2LL * R] = d2;
-        dG[gbase + 3LL * R] = d3;
-      }
-      float* a = As + crow[h] * LDA + cuu[h];
-      a[0] = round_tf32(d0); a[UBc] = round_tf32(d1); a[2 * UBc] = round_tf32(d2); a[3 * UBc] = round_tf32(d3);
-    }
-    if (it < S - 1) {
-      __syncthreads();   // As complete
-      const uint32_t slot = (uint32_t)((((it + 1) & 1) * CS + (int)rank) * MB * UBc) * 4u;
-      uint32_t b0[2 * NTL], b1[2 * NTL];
-      tmem_ld16(tw, b0);   // first tensor-memory step: in flight during the register-resident half
-#pragma unroll
-      for (int m = 0; m < MT; m++) {
-        float acc[NTL][4];
-#pragma unroll
-        for (int t = 0; t < NTL; t++)
-#pragma unroll
-          for (int q = 0; q < 4; q++) acc[t][q] = 0.f;
-        const float* ga = As + (m * 16 + gq) * LDA + tq;
-#pragma unroll
-        for (int k = 0; k < KR; k++) {
-          uint32_t a[4];
-          a[0] = __float_as_uint(ga[k * 8]); a[1] = __float_as_uint(ga[8 * LDA + k * 8]);
-          a[2] = __float_as_uint(ga[k * 8 + 4]); a[3] = __float_as_uint(ga[8 * LDA + k * 8 + 4]);
-#pragma unroll
-          for (int t = 0; t < NTL; t++) mma_tf32(acc[t], a, wreg[t][k]);
-        }
-#pragma unroll
-        for (int k = 0; k < KTM; k += 2) {
-          uint32_t a[4];
-          tmem_wait_ld16(b0);
-          tmem_ld16(tw + (uint32_t)((k + 1) * 2 * NTL), b1);
-          a[0] = __float_as_uint(ga[(KR + k) * 8]); a[1] = __float_as_uint(ga[8 * LDA + (KR + k) * 8]);
-          a[2] = __float_as_uint(ga[(KR + k) * 8 + 4]); a[3] = __float_as_uint(ga[8 * LDA + (KR + k) * 8 + 4]);
-#pragma unroll
-          for (int t = 0; t < NTL; t++) mma_tf32(acc[t], a, &b0[2 * t]);
-          tmem_wait_ld16(b1);
-          if (k + 2 < KTM) tmem_ld16(tw + (uint32_t)((k + 2) * 2 * NTL), b0);
-          else if (m + 1 < MT) tmem_ld16(tw, b0);   // first step of the next m16 tile
-          a[0] = __float_as_uint(ga[(KR + k + 1) * 8]); a[1] = __float_as_uint(ga[8 * LDA + (KR + k + 1) * 8]);
-          a[2] = __float_as_uint(ga[(KR + k + 1) * 8 + 4]); a[3] = __float_as_uint(ga[8 * LDA + (KR + k + 1) * 8 + 4]);
-#pragma unroll
-          for (int t = 0; t < NTL; t++) mma_tf32(acc[t], a, &b1[2 * t]);
-        }
-        // scatter: tile t of warp w holds columns n = 64 w + 8 t + 2 tq (+1), rows m*16 + gq (+8) -> owner 2w + (t >> 2), unit
-        // (8 t + 2 tq) & 31, slot [next parity][src = my rank]
-#pragma unroll
-        for (int t = 0; t < NTL; t++) {
-          const uint32_t base = raddr[t >> 2] + slot + (uint32_t)(((t & 3) * 8 + 2 * tq) * 4);
-          st_cluster_v2(base + (uint32_t)((m * 16 + gq) * UBc * 4), acc[t][0], acc[t][1]);
-          st_cluster_v2(base + (uint32_t)((m * 16 + gq + 8) * UBc * 4), acc[t][2], acc[t][3]);
-        }
-      }
-      cluster_arrive();   // release: my partial products are visible to their owners
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(TCOLS) : "memory");
-}
-constexpr size_t bwd_tm_smem(int MT) { return (size_t)(2 * CS * 16 * MT * UBc + 16 * MT * (4 * UBc + PAD)) * sizeof(float) + 16; }
-static_assert(bwd_tm_smem(3) <= 232448, "backward scan shared memory");
-
 constexpr size_t fwd_smem(int MT) {
   return (size_t)(8 * 16 * 4 * 2 * 32 + 16 * MT * (R + PAD) + (MT > 2 ? 0 : 2 * 16 * MT * (4 * UBc + 1)) + 4 * UBc) * sizeof(float);
 }
@@ -647,7 +433,7 @@ int launch_cluster16(Kern kern, const char* what, int grid, size_t smem, cudaStr
 
 }  // namespace
 
-// cudaOccupancyMaxActiveClusters of the cluster-16 scans (which = 0: forward 16-row slabs, 1: 32 rows, 3: 48 rows, 2: backward 16 rows, 4 / 5: backward 32 / 48 rows)
+// cudaOccupancyMaxActiveClusters of the cluster-16 scans (which = 0: forward 16-row slabs, 1: 32 rows, 3: 48 rows, 2: backward 16 rows)
 int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CS * 64);
@@ -676,18 +462,6 @@ int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
     cudaFuncSetAttribute(lstm_cl16_fwd_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem(3));
     cudaFuncSetAttribute(lstm_cl16_fwd_kernel<3>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     e = cudaOccupancyMaxActiveClusters(&n, lstm_cl16_fwd_kernel<3>, &cfg);
-  } else if (which == 4 || which == 5) {
-    const int mt = which - 2;   // 2 or 3 m16 tiles per slab
-    cfg.dynamicSmemBytes = bwd_tm_smem(mt);
-    if (mt == 2) {
-      cudaFuncSetAttribute(lstm_cl16_bwd_tm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_tm_smem(2));
-      cudaFuncSetAttribute(lstm_cl16_bwd_tm_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-      e = cudaOccupancyMaxActiveClusters(&n, lstm_cl16_bwd_tm_kernel<2>, &cfg);
-    } else {
-      cudaFuncSetAttribute(lstm_cl16_bwd_tm_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_tm_smem(3));
-      cudaFuncSetAttribute(lstm_cl16_bwd_tm_kernel<3>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-      e = cudaOccupancyMaxActiveClusters(&n, lstm_cl16_bwd_tm_kernel<3>, &cfg);
-    }
   } else {
     cfg.dynamicSmemBytes = bwd_smem();
     cudaFuncSetAttribute(lstm_cl16_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem());
@@ -698,10 +472,10 @@ int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
   return n;
 }
 
-// Rows per slab of the forward scan.  Only `maxc` clusters of 16 CTAs are resident at a time (7 on a B200: one per 20-SM GPC),
+// Rows per slab of the forward scan.  Only `maxc` clusters of 16 CTAs are resident at a time (one per GPC with 16 free SMs),
 // a launch with more clusters runs in waves, each wave a complete pass over the S timesteps.  One timestep of a 16*MT-row slab
-// costs about 1.5 + 2.8*MT us (measured: 4.3 / 7.1 us for MT = 1 / 2; barrier + L2 round trip, then MMA + pointwise per m16
-// tile): pick the MT with the smallest waves * step time.  B = 256: 6 clusters of 48 rows, one wave.
+// is modelled as 1.5 + 2.8*MT (barrier + L2 round trip, then MMA + pointwise per m16 tile): pick the MT with the smallest
+// waves * step time.
 static int fwd_slab_tiles(int B) {
   static int maxc = 0, forced = -1;
   if (forced < 0) {
@@ -732,36 +506,10 @@ int p2pvg_lstm_cluster512_fwd_impl(const float* pre, const float* whh, const flo
   return launch_cluster16(lstm_cl16_fwd_kernel<1>, "lstm_cl16_fwd", CS * cdiv(B, 16), fwd_smem(1), st, a1, pre, whh, bhh, gates, hs, cs, S, B);
 }
 
-// Rows per slab of the backward scan, same wave model as the forward one.  Measured per timestep: 16-row slabs (weight half in
-// shared memory) 5.7 us, 32 / 48-row slabs (weight half in tensor memory) 8.0 / 11.1 us, i.e. about 3.0 + 2.7 us per m16 tile;
-// B = 256: one wave of 6 clusters (11.2 us) instead of three waves of 16-row slabs (15.9 us).  Env override
-// P2PVG_LSTM512_BWD_MT = 1 | 2 | 3.
-static int bwd_slab_tiles(int B) {
-  static int maxc = 0, forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("P2PVG_LSTM512_BWD_MT");
-    forced = e ? atoi(e) : 0;
-    if (forced < 0 || forced > 3) forced = 0;
-    maxc = p2pvg_lstm_cluster512_max_clusters_impl(2);
-    if (maxc <= 0) maxc = 7;
-  }
-  if (forced) return forced;
-  int best = 1;
-  float best_cost = 0.f;
-  for (int mt = 1; mt <= 3; mt++) {
-    const int clusters = cdiv(B, 16 * mt), waves = cdiv(clusters, maxc);
-    const float cost = waves * (3.0f + 2.7f * mt);
-    if (mt == 1 || cost < best_cost) best = mt, best_cost = cost;
-  }
-  return best;
-}
-
 int p2pvg_lstm_cluster512_bwd_impl(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B,
                                    cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
-  static bool a = false, a2 = false, a3 = false;
-  const int mt = bwd_slab_tiles(B);
-  if (mt == 3) return launch_cluster16(lstm_cl16_bwd_tm_kernel<3>, "lstm_cl16_bwd", CS * cdiv(B, 48), bwd_tm_smem(3), st, a3, dhtop, whh, gates, cs, dG, S, B);
-  if (mt == 2) return launch_cluster16(lstm_cl16_bwd_tm_kernel<2>, "lstm_cl16_bwd", CS * cdiv(B, 32), bwd_tm_smem(2), st, a2, dhtop, whh, gates, cs, dG, S, B);
+  // 16-row slabs: the receive slots of larger slabs leave no shared memory for the weight half that does not fit the registers
+  static bool a = false;
   return launch_cluster16(lstm_cl16_bwd_kernel, "lstm_cl16_bwd", CS * cdiv(B, 16), bwd_smem(), st, a, dhtop, whh, gates, cs, dG, S, B);
 }

@@ -1,4 +1,4 @@
-"""Host-side schedule of one p2pvg training step on the sm_100a kernels.
+"""Host-side schedule of one p2pvg training step on the sm_90a kernels.
 
 Restructures ``P2PModel.forward`` (reference models/p2p_model.py:185-271) into time-batched phases
 (SURVEY.md §3.3) without changing its results:
@@ -177,19 +177,19 @@ class TrainEngine:
         # pixel-box gathers), without im2col / col2im buffers; P2PVG_IMPLICIT=0 keeps the explicit lowering
         import os
         # one persistent cooperative launch per LSTM layer and direction instead of two launches per timestep
-        # direct CUDA-core kernels for the 1/3-channel ends: measured slower than im2col + tcgen05 GEMM, so opt-in only
+        # direct CUDA-core kernels for the 1/3-channel ends: slower than im2col + tensor-core GEMM, so opt-in only
         self.thin = hasattr(kernels, "conv_thin_in") and os.environ.get("P2PVG_THIN", "0") == "1"
         # (R = 512: clusters of 16 CTAs, tensor-core mode only -- the exact-fp32 cooperative grid cannot keep a 4 MB W_hh resident)
         r512 = self.R == 512 and tc_lstm and os.environ.get("P2PVG_LSTM_CLUSTER", "1") != "0"
         self.fused_scan = hasattr(kernels, "lstm_scan_fwd") and self.R % 64 == 0 and (self.R <= 256 or r512) and os.environ.get("P2PVG_FUSED_SCAN", "1") != "0"
         self.implicit = (act_dtype == torch.bfloat16) and hasattr(kernels, "conv_gemm") and os.environ.get("P2PVG_IMPLICIT", "1") != "0"
         # 1/3-channel ends (K = 16 nc or N = 16 nc < 64): four pixel rows are multiplied as one row against a block-diagonal
-        # copy of the weight, so that no TMA box is out of bounds (measured 3x faster than the partially-OOB boxes)
+        # copy of the weight, so that no TMA box is out of bounds
         self.bd = (act_dtype == torch.bfloat16) and hasattr(kernels, "blockdiag") and os.environ.get("P2PVG_BLOCKDIAG", "1") != "0"
         # weight gradients and the skip-path of the backward pass are off the critical path: they are enqueued on a side
         # stream (captured into the same CUDA graph) so that the TMA-bound wgrad GEMMs overlap the HBM-bound BatchNorm kernels
-        # and the latency-bound LSTM scans of the main stream.  Measured gain on one B200: 1.3 % (24.57 -> 24.26 ms) -- the
-        # persistent GEMMs leave little room for a co-resident kernel -- so it is opt-in: P2PVG_OVERLAP=1.
+        # and the latency-bound LSTM scans of the main stream.  The persistent GEMMs leave little room for a co-resident kernel,
+        # so it is opt-in: P2PVG_OVERLAP=1.
         # BatchNorm forward statistics come out of the producing implicit GEMM's epilogue (per-tile column sums) instead of a
         # separate pass over the stored tensor; P2PVG_BN_FUSE=0 keeps the stand-alone statistics kernel (A/B comparison)
         # 1-channel stacks: tap gather + sigmoid + MSE of the last decoder layer as one kernel (no raw-output tensor)
@@ -198,8 +198,8 @@ class TrainEngine:
         self.addend_dtype = act_dtype if os.environ.get("P2PVG_ADDEND_BF16", "1") != "0" else torch.float32
         self.fuse_last = hasattr(kernels, "convt_c1_loss") and act_dtype == torch.bfloat16 and os.environ.get("P2PVG_FUSE_LAST", "1") != "0"
         self.fuse_stats = self.implicit and os.environ.get("P2PVG_BN_FUSE", "1") != "0"
-        # ... but only where the tile's MMA time hides the extra epilogue work: reduction length x tile width of the GEMM must
-        # reach this many MACs per output row (measured: low-K tiles are epilogue-bound and get slower, DESIGN.md)
+        # ... but only where the tile's MMA time can hide the extra epilogue work: reduction length x tile width of the GEMM must
+        # reach this many MACs per output row (a low-K tile does little MMA work per epilogue row)
         self.fuse_stats_min = int(os.environ.get("P2PVG_BN_FUSE_MIN", str(2048 * 128)))
         self.overlap = getattr(kernels, "name", "") == "cuda" and os.environ.get("P2PVG_OVERLAP", "0") == "1"
         # independent chains of small kernels (the three LSTMs, backward #2) run on side streams inside the captured graph

@@ -4,7 +4,7 @@ decoder around the same recurrent phase, losses, two-phase update and optimiser 
 There is no BatchNorm, so every encoder / decoder call is row-wise independent: all T frames (and all S+1 decoder
 calls) are plain row batches.  ``torch.cat([d, skip], 1)`` before a Linear is never materialised: the Linear is
 evaluated as two GEMMs over the two column blocks of its weight.  All tensors are fp32; in the tensor-core mode the
-K-major GEMMs with TMA-compatible operands run as tcgen05 kind::tf32 (p2pvg_gemm), the rest on the CUDA cores.
+K-major GEMMs with TMA-compatible operands run as wgmma .tf32 (p2pvg_gemm), the rest on the CUDA cores.
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ As in the dcgan schedule the encoder runs once over all T frames and the decoder
 BatchNorm statistics grouped per reference call; torch.cat is never materialised: the first layer of every decoder
 stage is evaluated as two convolutions over the two halves of its weight, the skip half once per distinct source frame
 (fp32 addend), the upsampled half with the addend folded into the GEMM epilogue.  In bf16 mode every layer with >= 64
-channels on both sides is an implicit GEMM (p2pvg_conv_gemm kinds 3-5: 4-D TMA pixel boxes -> tcgen05); the 3-channel
+channels on both sides is an implicit GEMM (p2pvg_conv_gemm kinds 3-5: 4-D TMA pixel boxes -> wgmma); the 3-channel
 ends and the fp32 mode use the explicit im2col3 lowering.
 """
 from __future__ import annotations

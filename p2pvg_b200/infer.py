@@ -1,4 +1,4 @@
-"""Stand-alone (no-autograd) forward passes of the drop-in modules on the sm_100a kernels: what
+"""Stand-alone (no-autograd) forward passes of the drop-in modules on the sm_90a kernels: what
 ``p2p_generate`` / ``generate.py`` / ``misc/visualize.py`` of the reference call (SURVEY.md §3.4).
 
 Same call signatures and return values as the reference modules:

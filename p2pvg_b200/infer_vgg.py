@@ -1,4 +1,4 @@
-"""Stand-alone (no-autograd) forward passes of the vgg_64 drop-in modules on the sm_100a kernels
+"""Stand-alone (no-autograd) forward passes of the vgg_64 drop-in modules on the sm_90a kernels
 (reference models/vgg_64.py:50-56, 94-105): what ``p2p_generate`` calls outside the train step.  Same conventions as
 p2pvg_b200/infer.py: NCHW fp32 in / out, BatchNorm honours ``module.training``."""
 import torch

@@ -1,5 +1,5 @@
 """``KLCriterion`` — same constructor / call signature as the reference's misc/criterion.py:5-15, computed by
-the fused sm_100a reparameterise+KL kernel (p2pvg_reparam_kl_fwd)."""
+the fused sm_90a reparameterise+KL kernel (p2pvg_reparam_kl_fwd)."""
 import torch
 import torch.nn as nn
 

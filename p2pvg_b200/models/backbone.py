@@ -3,7 +3,7 @@
 
 The torch.nn layers below are *holders* of parameters and BatchNorm buffers only: they are created in the
 reference's order so that the torch RNG is consumed identically, but their ``forward`` is never used — all
-arithmetic goes through the sm_100a kernels (p2pvg_b200/engine.py for the train step, p2pvg_b200/infer.py for
+arithmetic goes through the sm_90a kernels (p2pvg_b200/engine.py for the train step, p2pvg_b200/infer.py for
 stand-alone calls).
 """
 import torch.nn as nn

@@ -1,6 +1,6 @@
 """``models.h36m_mlp`` drop-in (reference models/h36m_mlp.py:28-95): residual-MLP pose encoder / decoder with the
 reference's constructor keywords and ``state_dict`` keys.  The nn layers hold parameters only; arithmetic runs in the
-sm_100a kernels (p2pvg_b200/engine_mlp.py for training, p2pvg_b200/infer.py for stand-alone calls)."""
+sm_90a kernels (p2pvg_b200/engine_mlp.py for training, p2pvg_b200/infer.py for stand-alone calls)."""
 import torch.nn as nn
 
 

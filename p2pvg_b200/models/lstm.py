@@ -1,7 +1,7 @@
 """``models.lstm`` drop-in: ``lstm`` (frame predictor) and ``gaussian_lstm`` (posterior / prior) with the
 reference's constructor signatures, ``state_dict`` keys and mutable ``.hidden`` list
 (reference models/lstm.py:5-44 and :46-94).  The nn layers only hold parameters; arithmetic runs in the
-sm_100a kernels.  ``init_hidden`` allocates on the parameters' device instead of hard-coding ``.cuda()``."""
+sm_90a kernels.  ``init_hidden`` allocates on the parameters' device instead of hard-coding ``.cuda()``."""
 import torch
 import torch.nn as nn
 

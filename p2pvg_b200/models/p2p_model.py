@@ -1,7 +1,7 @@
 """``models.p2p_model.P2PModel`` drop-in (reference models/p2p_model.py:12-330): same constructor, attributes
 (``encoder``, ``decoder``, ``frame_predictor``, ``posterior``, ``prior``, ``*_optimizer``), ``forward`` return
 value, ``save`` / ``load`` checkpoint format — with ``forward`` executed by p2pvg_b200.engine.TrainEngine on
-hand-written sm_100a kernels.  ``train.py`` / ``generate.py`` of the reference run against it unchanged.
+hand-written sm_90a kernels.  ``train.py`` / ``generate.py`` of the reference run against it unchanged.
 
 Differences that are visible and documented (DESIGN.md): after ``forward`` the ``.grad`` of the four non-prior
 modules holds the gradient that was *applied* (backward #1); the reference additionally accumulates the

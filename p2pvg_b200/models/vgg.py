@@ -5,7 +5,7 @@ models/vgg_128.py:4-120) with the reference's ``state_dict`` layout: ``c<stage>.
 
 The stages are generated from the channel tables of p2pvg_b200/engine_vgg.py in the reference's construction order, so
 the torch RNG stream (and with it ``init_weights``) is consumed identically.  The layers only *hold* parameters and
-BatchNorm buffers: arithmetic runs in the sm_100a kernels (engine_vgg.py for training, infer_vgg.py for stand-alone calls).
+BatchNorm buffers: arithmetic runs in the sm_90a kernels (engine_vgg.py for training, infer_vgg.py for stand-alone calls).
 """
 import torch.nn as nn
 

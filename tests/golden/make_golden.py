@@ -161,7 +161,12 @@ def run_case(name, spec, p2p_model, backbones):
             tape.append(rec)
         hooks.append(mods[mname].register_forward_hook(hook))
 
-    gen = torch.Generator().manual_seed(1234 + len(name))
+    # image inputs are not stored (files would exceed 1 MB): the fixture keeps the seed and the shapes, and
+    # tests/test_oracle_golden.py:load_fixture draws them again, one torch.rand per step
+    x_seed = 1234 + len(name)
+    gen = torch.Generator().manual_seed(x_seed)
+    if spec["width"] != "mlp":
+        fix["x_seed"] = x_seed
     for step in range(spec["steps"]):
         T, B, C, W = spec["T"], spec["B"], spec["channels"], spec["width"]
         if W == "mlp":
@@ -202,7 +207,7 @@ def run_case(name, spec, p2p_model, backbones):
                 z = e * (r["logvar"] * 0.5).exp() + r["mu"]
                 assert torch.allclose(z, r["z"], atol=1e-6), "eps replay failed"
         gprior = {k: p.grad.detach().clone() for k, p in model.prior.named_parameters()}
-        rec = dict(x=x, probs=torch.from_numpy(probs), np_seed=spec["np_seed"] + step, eps=eps,
+        rec = dict(probs=torch.from_numpy(probs), np_seed=spec["np_seed"] + step, eps=eps,
                    losses=[float(l) for l in losses], n_exec=n_exec,
                    tape=[dict(r) for r in tape],
                    grad_digest={m: {k: tensor_digest(v) for k, v in g.items()} for m, g in {**grads1, "prior": gprior}.items()},
@@ -210,6 +215,10 @@ def run_case(name, spec, p2p_model, backbones):
                                 for m, mod in mods.items()},
                    bn_buffers={m: {k: v.detach().clone() for k, v in mods[m].state_dict().items()
                                    if "running_" in k or "num_batches" in k} for m in ("encoder", "decoder")})
+        if spec["width"] == "mlp":
+            rec["x"] = x
+        else:
+            rec["x_shape"] = tuple(x.shape)
         fix["steps"].append(rec)
         print(f"[{name}] step {step}: exec={n_exec} losses={rec['losses']}")
     for h in hooks:

@@ -1,4 +1,4 @@
-"""Implicit-GEMM convolution family (p2pvg_conv_gemm: 4-D TMA pixel-box loads + tcgen05) against torch's
+"""Implicit-GEMM convolution family (p2pvg_conv_gemm: 4-D TMA pixel-box loads + wgmma) against torch's
 conv2d / conv_transpose2d on the same bf16 operands (fp32 reference arithmetic)."""
 import pytest
 import torch

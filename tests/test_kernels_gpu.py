@@ -72,8 +72,9 @@ TC_SHAPES = [
 
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn", TC_SHAPES)
 def test_gemm_tcgen05(KS, M, N, K, a_mn, b_mn):
+    """The tensor-core GEMM (the name predates its port from tcgen05 to wgmma) against the emulation, every operand major."""
     Kc, Ke = KS
-    assert Kc.has_tcgen05(), "driver entry point cuTensorMapEncodeTiled not available"
+    assert Kc.has_tc_gemm(), "driver entry point cuTensorMapEncodeTiled not available"
     Kc.set_gemm_impl("tc")
     try:
         dt = torch.bfloat16

@@ -93,10 +93,9 @@ def test_scan512_slab_size_invariance(K):
 
 
 def test_scan512_backward_slab_size_invariance(K):
-    """The R=512 backward scan has two implementations: 16-row slabs with the non-register weight half in shared memory, and
-    32 / 48-row slabs with that half in tensor memory (tcgen05.st / tcgen05.ld).  Per batch row the arithmetic is the same
-    (same k order, the 16 partial products summed in rank order), so the gradients of rows taken from a 256-row launch
-    (48-row slabs) and from a 128-row launch (32-row slabs) must be bit-identical to those rows launched alone (16-row slabs)."""
+    """The R=512 backward scan runs in 16-row slabs, with the 16 partial products of every row summed in rank order, so the
+    gradients of rows taken from a 256-row launch and from a 128-row launch must be bit-identical to those rows launched alone:
+    a row's result must not depend on which slab or cluster it lands in."""
     S, R = 5, 512
     torch.manual_seed(4)
     dev = "cuda"

@@ -22,11 +22,9 @@ from tests.test_engine_emu import CFG64, bn_cancelled_bias
 
 pytestmark = pytest.mark.gpu
 LR = 1e-3
-# vgg_64 is 23 bf16 conv+BatchNorm layers deep: per-tensor floor measured on the B200 (r2), median must hold 0.99
-# (every tensor / median over tensors).  Gradients arrive through ~20 bf16 BatchNorm backward projections (decoder + skip paths
-# + encoder), each of which removes the common mode of a bf16-rounded tensor: measured on the B200 at batch 32, T = 6:
-# min 0.919 (first encoder layer), 10 % quantile 0.943, median 0.982, 90 % quantile 0.9999.  The exact-fp32 mode holds
-# 1 - 1e-4 (tests/test_vgg_gpu.py).
+# vgg_64 is 23 bf16 conv+BatchNorm layers deep: a per-tensor floor and a floor for the median over tensors.  Gradients arrive
+# through ~20 bf16 BatchNorm backward projections (decoder + skip paths + encoder), each of which removes the common mode of a
+# bf16-rounded tensor, so the first encoder layer sits lowest.  The exact-fp32 mode holds 1 - 1e-4 (tests/test_vgg_gpu.py).
 VGG_MIN_COS = 0.90
 VGG_MEDIAN_COS = 0.975
 
@@ -132,9 +130,8 @@ def test_c1_shape_bf16_graph_cluster_vs_oracle(optkw, np_seed):
     adam = {m: O.new_adam_state(state[m]) for m in O.MODULES}
     ref = O.train_step(state, adam, x, opt, 64, eps, probs, mode="A")
     # the first layer's weight gradient is the deepest point of the backward chain (5 bf16 BatchNorm layers below the
-    # decoder): measured 0.9943 with frame skipping; everything else holds 0.995
-    # BatchNorm shift gradients (sums of dz with heavy cancellation) of the encoder: measured 0.9927 .. 0.995 on the B200;
-    # everything else holds 0.995
+    # decoder) and sits just below 0.995 with frame skipping, as do the BatchNorm shift gradients (sums of dz with heavy
+    # cancellation) of the encoder; everything else holds 0.995
     relaxed = {"encoder.c1.main.0.weight": 0.99}
     relaxed.update({f"encoder.c{i}.main.1.bias": 0.99 for i in range(1, 5)})
     check_step(ref, state0, got, eng, 1e-2, 0.995, f"C1/{optkw}", relaxed=relaxed)

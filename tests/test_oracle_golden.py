@@ -13,8 +13,19 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 CASES = sorted(os.path.basename(p)[5:-3] for p in glob.glob(os.path.join(GOLD, "step_*.pt")))
 
 
+def load_fixture(path):
+    """A step fixture of make_golden.py.  Fixtures with image inputs too large to store keep `x_seed` instead: the inputs were
+    drawn as one torch.rand per step from torch.Generator().manual_seed(x_seed), and are drawn again here."""
+    fix = torch.load(path, weights_only=False)
+    if "x_seed" in fix:
+        gen = torch.Generator().manual_seed(fix["x_seed"])
+        for rec in fix["steps"]:
+            rec["x"] = torch.rand(*rec["x_shape"], generator=gen)
+    return fix
+
+
 def load(case):
-    return torch.load(os.path.join(GOLD, f"step_{case}.pt"), weights_only=False)
+    return load_fixture(os.path.join(GOLD, f"step_{case}.pt"))
 
 
 def check_digest(t, d, rtol, atol, what):
@@ -35,7 +46,10 @@ def test_initial_weights_bit_exact(case):
         for k, d in digs.items():
             f = state[m][k].double().reshape(-1)
             assert torch.equal(f[d["idx"]], d["samples"]), f"{m}.{k}"
-            assert float(f.sum()) == d["sum"], f"{m}.{k}"
+            # the float64 sum of the digest depends on the order torch reduces in (thread count of the host): allow the
+            # worst-case reordering error of n float64 additions, nothing more
+            bound = f.numel() * 2.0 ** -53 * float(f.abs().sum())
+            assert abs(float(f.sum()) - d["sum"]) <= bound, f"{m}.{k}"
 
 
 @pytest.mark.parametrize("case", CASES)

@@ -12,6 +12,7 @@ import torch
 from oracle import p2p_oracle as O
 from p2pvg_b200.engine import StepPlan, TrainEngine
 from tests.test_engine_emu import CFG64, bn_cancelled_bias
+from tests.test_oracle_golden import load_fixture
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -87,7 +88,7 @@ CASES_BF16 = [(n, c, o, t, max(b, 4)) for n, c, o, t, b in CASES]
 @pytest.mark.parametrize("name,cfg,optkw,T,B", CASES_BF16)
 @pytest.mark.parametrize("gemm", ["simt", "tc"])
 def test_step_bf16_vs_emulation(name, cfg, optkw, T, B, gemm):
-    """bf16 path (CUDA-core GEMM and tcgen05 GEMM) against the torch emulation run with the same bf16
+    """bf16 path (CUDA-core GEMM and tensor-core wgmma GEMM) against the torch emulation run with the same bf16
     rounding points: isolates kernel errors from bf16 storage noise."""
     from tests.emu_backend import EmuKernels
     state = O.build_state(cfg, seed=1)
@@ -95,7 +96,7 @@ def test_step_bf16_vs_emulation(name, cfg, optkw, T, B, gemm):
     opt["batch_size"] = opt["batch_size"] or B
     eng = make_engine(state, cfg, opt, torch.bfloat16, gemm)
     if gemm == "tc":
-        assert eng.K.has_tcgen05(), "tcgen05 GEMM unavailable on this device"
+        assert eng.K.has_tc_gemm(), "tensor-core GEMM unavailable on this device"
     emu = TrainEngine(O.clone_state(state), cfg, opt, EmuKernels("cuda"), act_dtype=torch.bfloat16)
     x, probs, eps = inputs(name, cfg, opt, T, B)
     try:
@@ -138,7 +139,7 @@ def digest_close(t, d, rtol, what):
 @pytest.mark.parametrize("path", sorted(glob.glob(os.path.join(GOLD, "step_d*.pt"))), ids=lambda p: os.path.basename(p)[5:-3])
 def test_step_vs_reference_golden(path):
     """fp32 CUDA path against numbers produced by the reference's own P2PModel.forward."""
-    fix = torch.load(path, weights_only=False)
+    fix = load_fixture(path)
     cfg, opt = fix["cfg"], dict(fix["opt"])
     state = O.build_state(cfg, seed=fix["init_seed"])
     eng = make_engine(state, cfg, opt, torch.float32)

@@ -10,6 +10,7 @@ import torch.nn.functional as F
 
 from oracle import p2p_oracle as O
 from p2pvg_b200.engine import StepPlan
+from tests.test_oracle_golden import load_fixture
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "step_vgg64_rgb.pt")
@@ -182,7 +183,7 @@ def test_vgg_step_bf16_vs_emulation_and_oracle():
 def test_vgg_step_vs_reference_golden():
     from p2pvg_b200._lib import CudaKernels
     from p2pvg_b200.engine_vgg import TrainEngineVGG
-    fix = torch.load(GOLD, weights_only=False)
+    fix = load_fixture(GOLD)
     state = O.build_state(fix["cfg"], seed=fix["init_seed"])
     cfg = dict(fix["cfg"], image_width=64)
     eng = TrainEngineVGG(state, cfg, dict(fix["opt"]), CudaKernels("cuda"), act_dtype=torch.float32)
@@ -207,7 +208,7 @@ def test_vgg128_step_vs_reference_golden():
     """models/vgg_128.py (5 stages, 128x128): fp32 CUDA path against the unmodified reference's numbers."""
     from p2pvg_b200._lib import CudaKernels
     from p2pvg_b200.engine_vgg import TrainEngineVGG
-    fix = torch.load(os.path.join(os.path.dirname(__file__), "golden", "step_vgg128_gray.pt"), weights_only=False)
+    fix = load_fixture(os.path.join(os.path.dirname(__file__), "golden", "step_vgg128_gray.pt"))
     state = O.build_state(fix["cfg"], seed=fix["init_seed"])
     cfg = dict(fix["cfg"], image_width=128)
     eng = TrainEngineVGG(state, cfg, dict(fix["opt"]), CudaKernels("cuda"), act_dtype=torch.float32)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Representative launches of the implicit-GEMM convolution kernel (shapes of the dcgan_64 batch-256 step) for
-`ncu --set full -k regex:conv_gemm_kernel`: conv forward c3, ConvT forward upc3, weight gradient c3, fused-phase ConvT upc4 (with the skip addend), c3 forward with fused BatchNorm statistics."""
+`ncu --set full -k regex:conv_gemm_kernel`: conv forward c3, ConvT forward upc3, weight gradient c3, ConvT upc4 (with the skip addend), c3 forward with fused BatchNorm statistics."""
 import os
 import sys
 
@@ -23,7 +23,7 @@ for rep in range(2):
     K.conv_gemm(2, xs, wt, yb, N, 8, 8, 256, 128)                     # kind 2: ConvT forward
     gw = torch.empty(256, 16 * 128, device="cuda")
     K.conv_gemm(1, xs, x, gw, N, 8, 8, 0, 128, Cm=256)                # kind 1: weight gradient
-    # upc4 shape (128 -> 64 channels, 16x16 -> 32x32): the four output-parity phases fused into one 128x256 tile (convt4_kernel)
+    # upc4 shape (128 -> 64 channels, 16x16 -> 32x32): one 128x64 tile per output-parity phase
     x4 = torch.randn(N, 16, 16, 128, device="cuda", dtype=bf)
     w4 = torch.randn(128, 16 * 64, device="cuda", dtype=bf) * 0.02
     add = torch.randn(256, 32, 32, 64, device="cuda")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Representative launches of the tcgen05 GEMM (shapes of the dcgan_64 batch-256 train step) for
+"""Representative launches of the wgmma GEMM (shapes of the dcgan_64 batch-256 train step) for
 `ncu --set full -k regex:gemm_tc_kernel`:  conv forward (K-major), ConvT forward (MN-major B, output-bound),
 weight gradient (MN-major A and B, split-K).  `--shape M,N,K,a_mn,b_mn,f32out` (repeatable) overrides the list;
 `--time` prints the CUDA-event time of each launch (second repetition)."""

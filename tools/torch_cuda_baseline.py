@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Library baseline (BASELINE.md §3 (ii)): the reference's train step -- restated by oracle/p2p_oracle.py, i.e. plain PyTorch
-ops + autograd + the legacy Adam -- run on the same B200 through stock torch-CUDA (cuDNN / cuBLAS), on the bench workload
+ops + autograd + the legacy Adam -- run on the same GPU through stock torch-CUDA (cuDNN / cuBLAS), on the bench workload
 (mnist dcgan_64, T=30, B=256, skip_prob 0).  Test / measurement infrastructure only; nothing in the product path imports it."""
 import argparse
 import os
