@@ -173,18 +173,22 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* desc, uint64_t* b
 
 // Thread-per-row epilogues hold one tile row per lane: column sums over the 32 rows of a warp by a transpose-reduce
 // butterfly (16 + 8 + 4 + 2 + 1 = 31 shuffles for 32 columns instead of 5 per column).  Lane L returns the sum over the
-// warp's lanes of v[L]; v is destroyed.
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// warp's lanes of v[L]; v is destroyed.  One template instance per stage: with a run-time stage loop the compiler did not
+// unroll the inner loop fully, `v[j + off]` became a dynamic index and the arrays of the statistics epilogues lived in local
+// memory (256-byte stack frame, 384 local loads / stores per 32-column chunk of a tile row).
+template <int OFF>
+__device__ __forceinline__ void colsum_stage(float (&v)[32], int lane) {
+  const bool upper = (lane & OFF) != 0;
 #pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int j = 0; j < off; j++) {
-      const float send = upper ? v[j] : v[j + off];
-      const float keep = upper ? v[j + off] : v[j];
-      v[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
+  for (int j = 0; j < OFF; j++) {
+    const float send = upper ? v[j] : v[j + OFF];
+    const float keep = upper ? v[j + OFF] : v[j];
+    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
   }
+  if constexpr (OFF > 1) colsum_stage<OFF / 2>(v, lane);
+}
+__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+  colsum_stage<16>(v, lane);
   return v[0];
 }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
