@@ -98,7 +98,12 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
  *                     row block mt and phase ph is row mt*phases + ph; reduce per group with p2pvg_bn_fwd_finalize_tiles
  *                     (rows of one BatchNorm group must be a multiple of 128).
  *   bwd_*             reserved for the BatchNorm-backward reduction of a data-gradient GEMM (sum dz, sum dz*xhat).
- *   addend_dtype      the skip-half addend may be stored in bf16 (it is the output of another p2pvg_conv_gemm call). */
+ *   addend_dtype      the skip-half addend may be stored in bf16 (it is the output of another p2pvg_conv_gemm call).
+ *   eval_scale/shift  kinds 0 and 2: nn.BatchNorm2d in eval mode + activation applied in the epilogue (generation,
+ *                     models/p2p_model.py:80-183 with running statistics): the stored output is
+ *                     y = act(eval_scale[c] * (acc + bias[c] + addend) + eval_shift[c]), act = P2PVG_ACT_LRELU | P2PVG_ACT_TANH,
+ *                     coefficients as p2pvg_bn_eval_coeffs writes them.  NULL: no such epilogue.  Not combinable with
+ *                     fwd_stat_partial or accumulate (P2PVG_ERR_BAD_ARG). */
 typedef struct p2pvg_conv_fusion {
   void* fwd_stat_partial;
   const void* bwd_raw;
@@ -109,6 +114,9 @@ typedef struct p2pvg_conv_fusion {
   void* bwd_stat_partial;
   int64_t rows_per_group;
   int addend_dtype; /* dtype of `addend`: P2PVG_F32 (default, also without a fusion struct) or P2PVG_BF16 (half the epilogue read traffic) */
+  const float* eval_scale;
+  const float* eval_shift;
+  int act;
 } p2pvg_conv_fusion_t;
 
 /* vgg_64 data movement (models/vgg_64.py), NHWC, dtype f32 | bf16.
@@ -221,6 +229,47 @@ int p2pvg_lstm_scan_bwd(const float* dhtop, const float* whh, const float* gates
 int p2pvg_lstm_cluster512_max_clusters(int which);
 /* the same for the hidden-size-256 scans (clusters of 8 CTAs): which = 0 / 1 forward with 16- / 32-row slabs, 2 / 3 backward */
 int p2pvg_lstm_cluster_max_clusters(int which);
+/* One timestep of one or two stand-alone LSTM modules in ONE launch (models/lstm.py:29-44 `lstm`, :83-94 `gaussian_lstm`):
+ * embed Linear -> `layers` x nn.LSTMCell -> head.  Generation runs posterior + prior as one launch and the frame predictor as a
+ * second.  Clusters of 8 CTAs, each CTA owning R/8 hidden units of every layer, one cluster per slab of 8 batch rows; stage
+ * outputs are exchanged through distributed shared memory; weights stream from L2; exact fp32 FFMA.  R in 64..512 (multiple
+ * of 8), any layer count, any row count.
+ *   input row b  = [ seg_a[idx_a[0]*rows + b, 0:ga] | seg_b[idx_b[0]*rows + b, 0:gb] | tuc[0] | dt[0] ]  (the torch.cat of
+ *                  models/p2p_model.py:150-179, never materialised; idx_a / idx_b / tuc / dt are device pointers read at run time)
+ *   layer_w      device array [layers][4] of device pointers: weight_ih [4R][R], bias_ih [4R], weight_hh [4R][R], bias_hh [4R]
+ *   state        device array [layers][4] of device pointers: h_in, c_in, h_out, c_out, each [rows][R] fp32 (h_out == h_in and
+ *                c_out == c_in is allowed: the state may be updated in place)
+ *   head         P2PVG_LSTM_HEAD_LINEAR_TANH: out[rows][out_dim] = tanh(h W_out^T + b_out)
+ *                P2PVG_LSTM_HEAD_GAUSSIAN:    mu = h W_out^T + b_out, logvar = h W_out2^T + b_out2, out = eps * exp(logvar / 2) + mu
+ *                                             (mu / logvar written when non-NULL)  */
+#define P2PVG_LSTM_HEAD_LINEAR_TANH 0
+#define P2PVG_LSTM_HEAD_GAUSSIAN 1
+typedef struct p2pvg_lstm_step_module {
+  const float* seg_a;
+  const int* idx_a;
+  int ga;
+  const float* seg_b;
+  const int* idx_b;
+  int gb;
+  const float* tuc;
+  const float* dt;
+  const float* w_embed;
+  const float* b_embed;
+  int layers;
+  const float* const* layer_w;
+  float* const* state;
+  int head;
+  int out_dim;
+  const float* w_out;
+  const float* b_out;
+  const float* w_out2;
+  const float* b_out2;
+  const float* eps;
+  float* out;
+  float* mu;
+  float* logvar;
+} p2pvg_lstm_step_module;
+int p2pvg_lstm_step(const p2pvg_lstm_step_module* modules /*host array*/, int n_modules, int rows, int R, void* stream);
 /* gaussian_lstm.reparameterize (models/lstm.py:76-81) for posterior and prior + KLCriterion.forward
  * (misc/criterion.py:10-15) summed over all elements (division by opt.batch_size happens in finalize_losses). */
 int p2pvg_reparam_kl_fwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,

@@ -62,7 +62,21 @@ class ConvFusion(ctypes.Structure):
     """p2pvg_conv_fusion_t (include/p2pvg_b200.h)."""
     _fields_ = [("fwd_stat_partial", ctypes.c_void_p), ("bwd_raw", ctypes.c_void_p), ("bwd_mean", ctypes.c_void_p),
                 ("bwd_invstd", ctypes.c_void_p), ("bwd_scale", ctypes.c_void_p), ("bwd_shift", ctypes.c_void_p),
-                ("bwd_stat_partial", ctypes.c_void_p), ("rows_per_group", ctypes.c_int64), ("addend_dtype", ctypes.c_int)]
+                ("bwd_stat_partial", ctypes.c_void_p), ("rows_per_group", ctypes.c_int64), ("addend_dtype", ctypes.c_int),
+                ("eval_scale", ctypes.c_void_p), ("eval_shift", ctypes.c_void_p), ("act", ctypes.c_int)]
+
+
+class LstmStepModule(ctypes.Structure):
+    """p2pvg_lstm_step_module (include/p2pvg_b200.h)."""
+    _fields_ = [("seg_a", ctypes.c_void_p), ("idx_a", ctypes.c_void_p), ("ga", ctypes.c_int), ("seg_b", ctypes.c_void_p),
+                ("idx_b", ctypes.c_void_p), ("gb", ctypes.c_int), ("tuc", ctypes.c_void_p), ("dt", ctypes.c_void_p),
+                ("w_embed", ctypes.c_void_p), ("b_embed", ctypes.c_void_p), ("layers", ctypes.c_int), ("layer_w", ctypes.c_void_p),
+                ("state", ctypes.c_void_p), ("head", ctypes.c_int), ("out_dim", ctypes.c_int), ("w_out", ctypes.c_void_p),
+                ("b_out", ctypes.c_void_p), ("w_out2", ctypes.c_void_p), ("b_out2", ctypes.c_void_p), ("eps", ctypes.c_void_p),
+                ("out", ctypes.c_void_p), ("mu", ctypes.c_void_p), ("logvar", ctypes.c_void_p)]
+
+
+LSTM_HEAD_LINEAR_TANH, LSTM_HEAD_GAUSSIAN = 0, 1
 
 
 class _Workspaces:
@@ -168,9 +182,10 @@ class CudaKernels:
 
     # -- implicit-GEMM convolutions ---------------------------------------------------------
     def conv_gemm(self, kind, a, b, c, N, H, W, Ck, Cn, Cm=0, ldb=None, ldc=None, bias=None, addend=None, grp_src=None,
-                  imgs_per_group=0, accumulate=False, stat_partial=None):
+                  imgs_per_group=0, accumulate=False, stat_partial=None, eval_scale=None, eval_shift=None, act=ACT_NONE):
         """kind 0..5 of p2pvg_conv_gemm (see include/p2pvg_b200.h).  H, W: small-map size.  stat_partial: fp32 buffer of
-        [tiles * phases, Cn, 2] receiving the BatchNorm forward statistics of the output (epilogue fusion)."""
+        [tiles * phases, Cn, 2] receiving the BatchNorm forward statistics of the output (epilogue fusion).  eval_scale /
+        eval_shift (kinds 0, 2): eval-mode BatchNorm + `act` applied in the epilogue."""
         taps = 9 if kind >= 3 else 16
         if ldb is None:
             ldb = taps * Ck if kind in (0, 3, 5) else taps * Cn
@@ -178,9 +193,11 @@ class CudaKernels:
             ldc = taps * Cn if kind in (1, 4) else Cn
         ws = self.gemm_workspace()
         fusion = None
-        if stat_partial is not None or (addend is not None and addend.dtype == torch.bfloat16):
+        if stat_partial is not None or eval_scale is not None or (addend is not None and addend.dtype == torch.bfloat16):
             fusion = ctypes.byref(ConvFusion(fwd_stat_partial=stat_partial.data_ptr() if stat_partial is not None else None,
-                                             addend_dtype=_dt(addend) if addend is not None else F32))
+                                             addend_dtype=_dt(addend) if addend is not None else F32,
+                                             eval_scale=eval_scale.data_ptr() if eval_scale is not None else None,
+                                             eval_shift=eval_shift.data_ptr() if eval_shift is not None else None, act=int(act)))
         self._ck(self.lib.p2pvg_conv_gemm(_i(kind), _p(a), _p(b), _i64(ldb), _p(c), _i(_dt(c)), _i64(ldc), _i(N), _i(H), _i(W), _i(Ck),
                                           _i(Cn), _i(Cm), _p(bias), _p(addend), _p(grp_src), _i(imgs_per_group), _i(int(accumulate)),
                                           _p(ws), _sz(ws.numel()), fusion, self._stream()))
@@ -301,6 +318,14 @@ class CudaKernels:
     def lstm_scan_bwd(self, dhtop, whh, gates, cs, dG, S, B, R, counter, tf32=False):
         self._ck(self.lib.p2pvg_lstm_scan_bwd(_p(dhtop), _p(whh), _p(gates), _p(cs), _p(dG), _i(S), _i(B), _i(R), _i(int(tf32)),
                                               _p(counter), self._stream()))
+
+    def lstm_step(self, modules, rows, R):
+        """p2pvg_lstm_step: modules = list of one or two dicts of LstmStepModule fields (tensors or None; ints as ints)."""
+        arr = (LstmStepModule * len(modules))()
+        for i, m in enumerate(modules):
+            for k, v in m.items():
+                setattr(arr[i], k, v if isinstance(v, int) else (v.data_ptr() if v is not None else None))
+        self._ck(self.lib.p2pvg_lstm_step(arr, _i(len(modules)), _i(rows), _i(R), self._stream()))
 
     def reparam_kl_fwd(self, mu, lv, mu_p, lv_p, eps, eps_p, z, z_p, n, kl_sum):
         self._ck(self.lib.p2pvg_reparam_kl_fwd(_p(mu), _p(lv), _p(mu_p), _p(lv_p), _p(eps), _p(eps_p), _p(z), _p(z_p), _i(n),

@@ -43,7 +43,7 @@ int p2pvg_conv_thin_in_impl(const void*, int, const float*, const float*, void*,
 int p2pvg_convT_thin_out_impl(const void*, int, const float*, const float*, const float*, const int*, int, void*, int, int, int, int, int,
                               int, cudaStream_t);
 int p2pvg_conv_gemm_impl(int, const void*, const void*, long long, void*, int, long long, int, int, int, int, int, int, const float*,
-                         const float*, const int*, int, int, void*, size_t, void*, int, cudaStream_t);
+                         const float*, const int*, int, int, void*, size_t, void*, int, const float*, const float*, int, cudaStream_t);
 int p2pvg_bn_fwd_finalize_tiles_impl(const void*, int, int, int, int, long long, int, const float*, const float*, float, float*, float*, float*,
                                      float*, float*, cudaStream_t);
 int p2pvg_bn_bwd_finalize_tiles_impl(const void*, int, int, int, int, int, float*, float*, cudaStream_t);
@@ -85,6 +85,7 @@ int p2pvg_lstm_cluster512_fwd_impl(const float*, const float*, const float*, flo
 int p2pvg_lstm_cluster512_bwd_impl(const float*, const float*, const float*, const float*, float*, int, int, cudaStream_t);
 int p2pvg_lstm_cluster512_max_clusters_impl(int);
 int p2pvg_lstm_cluster_max_clusters_impl(int);
+int p2pvg_lstm_step_impl(const p2pvg_lstm_step_module*, int, int, int, cudaStream_t);
 int p2pvg_reparam_kl_fwd_impl(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, int,
                               float*, cudaStream_t);
 int p2pvg_reparam_kl_bwd_impl(const float*, const float*, const float*, const float*, const float*, const float*, const float*,
@@ -157,7 +158,8 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
   const int add_dt = fusion ? fusion->addend_dtype : P2PVG_F32;
   P2PVG_REQUIRE(add_dt == P2PVG_F32 || add_dt == P2PVG_BF16, P2PVG_ERR_BAD_ARG, "conv_gemm: bad addend dtype %d", add_dt);
   return p2pvg_conv_gemm_impl(kind, a, b, ldb, c, c_dtype, ldc, N, H, W, Ck, Cn, Cm, bias, reinterpret_cast<const float*>(addend), grp_src,
-                              imgs_per_group, accumulate, workspace, ws_bytes, fwd_stat, add_dt, ST);
+                              imgs_per_group, accumulate, workspace, ws_bytes, fwd_stat, add_dt, fusion ? fusion->eval_scale : nullptr,
+                              fusion ? fusion->eval_shift : nullptr, fusion ? fusion->act : 0, ST);
 }
 
 int p2pvg_conv_thin_in(const void* x, int dtype, const float* w, const float* bias, void* y, int N, int H, int W, int Ci, int Co,
@@ -286,6 +288,9 @@ int p2pvg_lstm_scan_bwd(const float* dhtop, const float* whh, const float* gates
 }
 int p2pvg_lstm_cluster512_max_clusters(int which) { return p2pvg_lstm_cluster512_max_clusters_impl(which); }
 int p2pvg_lstm_cluster_max_clusters(int which) { return p2pvg_lstm_cluster_max_clusters_impl(which); }
+int p2pvg_lstm_step(const p2pvg_lstm_step_module* modules, int n_modules, int rows, int R, void* stream) {
+  return p2pvg_lstm_step_impl(modules, n_modules, rows, R, ST);
+}
 int p2pvg_reparam_kl_fwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
                          const float* eps_p, float* z, float* z_p, int n, float* kl_sum, void* stream) {
   return p2pvg_reparam_kl_fwd_impl(mu, lv, mu_p, lv_p, eps, eps_p, z, z_p, n, kl_sum, ST);

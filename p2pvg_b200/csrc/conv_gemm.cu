@@ -103,12 +103,13 @@ __device__ __forceinline__ void addend_add32(float (&f)[32], const float4 (&a4)[
   }
 }
 
-template <int KIND, int BN, bool STAT>
+// EVAL: eval-mode BatchNorm + activation in the epilogue, y = act(eval_scale[c] * (acc + bias + addend) + eval_shift[c]) (kinds 0 / 2)
+template <int KIND, int BN, bool STAT, bool EVAL = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* __restrict__ Cv, int c_bf16,
                  long long ldc, Geom g, int accumulate, const float* __restrict__ bias, const float* __restrict__ addend,
                  const int* __restrict__ grp_src, float* __restrict__ partial, int kb_per_split, int splits,
-                 float2* __restrict__ stat_partial) {
+                 float2* __restrict__ stat_partial, const float* __restrict__ eval_scale, const float* __restrict__ eval_shift, int act) {
   using C_ = Cfg<BN>;
   constexpr bool A_MN = (KIND == 1), B_MN = (KIND != 0);
   extern __shared__ uint8_t smem_raw[];
@@ -312,6 +313,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // buffered by tile parity so that tile t+1 may write while the sums of tile t are still being combined
     __shared__ float2 stat_s[STAT ? 2 * 4 * BN : 1];
     constexpr bool do_stat = STAT;   // a separate instantiation: the statistics cost ~50 registers in this epilogue
+    // eval-mode BatchNorm coefficients of the tile's columns, double-buffered by tile parity like bias_s: [parity][scale | shift][BN]
+    __shared__ float ev_s[EVAL ? 2 * 2 * BN : 1];
     uint32_t lt = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
       const int ph = (KIND == 2) ? (t & 3) : 0;
@@ -348,6 +351,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         add_row = (long long)n2 * HW + (out_row - (long long)n * HW);
       }
       // stage the bias slice of this tile in shared memory while the MMAs are still running
+      if (EVAL) {
+        for (int i = q * 32 + lane; i < BN; i += 128) {
+          const bool in = n0 + i < g.Ntot;
+          ev_s[acc * 2 * BN + i] = in ? eval_scale[n0 + i] : 0.f;
+          ev_s[acc * 2 * BN + BN + i] = in ? eval_shift[n0 + i] : 0.f;
+        }
+        if (bias == nullptr) epi_bar_sync();
+      }
       if (bias != nullptr) {
         for (int i = q * 32 + lane; i < BN; i += 128) bias_s[acc * BN + i] = (n0 + i < g.Ntot) ? bias[n0 + i] : 0.f;
         epi_bar_sync();
@@ -394,6 +405,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
           }
           if (use_add) addend_add32(f, a4, h, abf);
+          if (EVAL) {
+            const float* sc = ev_s + acc * 2 * BN + c * 32;
+#pragma unroll
+            for (int j = 0; j < 32; j++) {
+              float y = fmaf(f[j], sc[j], sc[BN + j]);
+              if (act == P2PVG_ACT_LRELU) y = y > 0.f ? y : 0.2f * y;
+              else if (act == P2PVG_ACT_TANH) y = tanhf(y);
+              f[j] = y;
+            }
+          }
           if (STAT) {
             // statistics of the tensor AS STORED (bf16-rounded when the output is bf16); all 32 lanes take part
             float s1[32], s2[32];
@@ -484,7 +505,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn g_enc = nullptr;
 std::once_flag g_once2;
 int g_sms = 132;
-int g_attr[2][3][2] = {};
+int g_attr[3][3][2] = {};   // [plain | statistics | eval epilogue][kind][BN == 128]
 int g_bres = 1;      // 64 -> 64 channel 3x3 layers: weights resident in shared memory (P2PVG_CONV_BRES=0 disables)
 int g_k1_swap = 1;   // kind 1 / 4 with 64 output channels: swapped operand roles (P2PVG_K1_SWAP=0 disables)
 
@@ -545,25 +566,33 @@ bool box_for(int P, int H, int W, int& bh, int& bn) {
   return bh * 2 <= 256 && W * 2 <= 256 && bn <= 256;
 }
 
-template <int KIND, int BN, bool STAT>
+// eval-mode BatchNorm epilogue operands (all NULL / 0: no such epilogue)
+struct EvalEpi {
+  const float* scale = nullptr;
+  const float* shift = nullptr;
+  int act = 0;
+};
+
+template <int KIND, int BN, bool STAT, bool EVAL>
 int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, int accumulate,
              const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
-             float2* stat_partial);
+             float2* stat_partial, const EvalEpi& ev);
 
 template <int KIND, int BN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, int accumulate,
            const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
-           float2* stat_partial = nullptr) {
-  if (KIND != 1 && stat_partial != nullptr) return launch_t<KIND, BN, (KIND != 1)>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, stat_partial);
-  return launch_t<KIND, BN, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr);
+           float2* stat_partial = nullptr, const EvalEpi& ev = EvalEpi()) {
+  if (KIND != 1 && ev.scale != nullptr) return launch_t<KIND, BN, false, (KIND != 1)>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
+  if (KIND != 1 && stat_partial != nullptr) return launch_t<KIND, BN, (KIND != 1), false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, stat_partial, ev);
+  return launch_t<KIND, BN, false, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
 }
 
-template <int KIND, int BN, bool STAT>
+template <int KIND, int BN, bool STAT, bool EVAL>
 int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, int accumulate,
              const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
-             float2* stat_partial) {
-  auto kern = conv_gemm_kernel<KIND, BN, STAT>;
-  int& done = g_attr[STAT][KIND][BN == 128];
+             float2* stat_partial, const EvalEpi& ev) {
+  auto kern = conv_gemm_kernel<KIND, BN, STAT, EVAL>;
+  int& done = g_attr[EVAL ? 2 : STAT][KIND][BN == 128];
   if (!done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
     if (e != cudaSuccess) {
@@ -575,7 +604,7 @@ int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype,
   long long tiles = (long long)cdiv(g.M, BLOCK_M) * cdiv(g.Ntot, BN) * splits * (KIND == 2 ? 4 : 1);
   int grid = (int)(tiles < g_sms ? tiles : g_sms);
   kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, st>>>(ta, tb, C, c_dtype == P2PVG_BF16, ldc, g, accumulate, bias, addend, grp_src, partial,
-                                                      kb_per_split, splits, stat_partial);
+                                                      kb_per_split, splits, stat_partial, ev.scale, ev.shift, ev.act);
   return p2pvg_check_launch("conv_gemm");
 }
 
@@ -585,11 +614,21 @@ int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype,
 // fit the pixel-box tiling (the caller then uses the explicit im2col / col2im path).
 int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, void* c, int c_dtype, long long ldc, int N, int H, int W,
                          int Ck, int Cn, int Cm, const float* bias, const float* addend, const int* grp_src, int imgs_per_group,
-                         int accumulate, void* ws, size_t ws_bytes, void* stat_partial_v, int addend_dtype, cudaStream_t st) {
+                         int accumulate, void* ws, size_t ws_bytes, void* stat_partial_v, int addend_dtype, const float* eval_scale,
+                         const float* eval_shift, int act, cudaStream_t st) {
   float2* stat_partial = reinterpret_cast<float2*>(stat_partial_v);
+  EvalEpi ev;
+  ev.scale = eval_scale; ev.shift = eval_shift; ev.act = act;
   std::call_once(g_once2, resolve2);
   P2PVG_REQUIRE(g_enc != nullptr, P2PVG_ERR_UNSUPPORTED, "conv_gemm: cuTensorMapEncodeTiled unavailable");
   P2PVG_REQUIRE(kind >= 0 && kind <= 5, P2PVG_ERR_BAD_ARG, "conv_gemm: bad kind %d", kind);
+  if (eval_scale != nullptr) {
+    P2PVG_REQUIRE(kind == 0 || kind == 2, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue belongs to kinds 0 and 2");
+    P2PVG_REQUIRE(eval_shift != nullptr, P2PVG_ERR_BAD_ARG, "conv_gemm: eval_scale without eval_shift");
+    P2PVG_REQUIRE(stat_partial == nullptr, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue excludes fwd_stat_partial");
+    P2PVG_REQUIRE(!accumulate, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue does not accumulate");
+    P2PVG_REQUIRE(act == P2PVG_ACT_LRELU || act == P2PVG_ACT_TANH, P2PVG_ERR_BAD_ARG, "conv_gemm: eval epilogue act %d", act);
+  }
   if (N <= 0) return P2PVG_OK;
   Geom g;
   g.N = N; g.H = H; g.W = W; g.Ck = Ck; g.Cn = Cn; g.imgs_per_group = imgs_per_group > 0 ? imgs_per_group : 1;
@@ -630,8 +669,8 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     if (rc) return rc;
     const int nkb = taps * (Ck / 64);
     g.bres = (BN == 64 && Cn == 64 && Ck == 64 && taps <= 9 && g_bres) ? 1 : 0;
-    if (BN == 128) return launch<0, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
-    return launch<0, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
+    if (BN == 128) return launch<0, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
+    return launch<0, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
   }
   if (kind == 2) {
     g.M = (int)pix; g.Ntot = Cn;
@@ -641,8 +680,8 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     if (rc) return rc;
     const int nkb = 4 * (Ck / 64);
     const int BN = Cn > 64 ? 128 : 64;
-    if (BN == 128) return launch<2, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
-    return launch<2, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial);
+    if (BN == 128) return launch<2, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
+    return launch<2, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
   }
   // kind 1: weight gradient
   P2PVG_REQUIRE(c_dtype == P2PVG_F32, P2PVG_ERR_BAD_ARG, "conv_gemm kind 1 writes fp32");

@@ -1,0 +1,470 @@
+"""Graph-captured point-to-point generation for the dcgan backbones (reference models/p2p_model.py:80-183).
+
+``GenerateEngine`` computes what ``infer.p2p_generate`` / ``infer.p2p_generate_samples`` compute, with every call one
+replay of a CUDA graph captured per signature (rows, sequence lengths, executed steps, model_mode, n_past,
+last_frame_skip, precision and the device addresses of every parameter and BatchNorm buffer read).
+
+Host work per call: the reference's NumPy skip draw, the slot planner below, the per-slot tables (time_until_cp,
+delta_time, posterior target), the eps buffer, the replay, and copying the generated frames out of graph memory.
+Inside the graph:
+  * the bf16 weight packs and the eval-BatchNorm coefficients are recomputed from the live parameters, so a training
+    step between two calls is picked up without any host bookkeeping;
+  * the ground-truth frames are encoded once, time-batched at B rows (not nsample * B; eval-mode rows are independent);
+    that one encode gives global_z, the posterior targets, the teacher-forced inputs and the skip maps;
+  * the skip half of every decoder torch.cat([d, skip]) is computed once per call (per decode when last_frame_skip);
+  * every executed slot runs the encoder on the previous decoded frame (only after the teacher-forced steps), the
+    posterior, prior and frame predictor, and the decoder.
+
+Recurrent part: per executed step ONE p2pvg_lstm_step launch for posterior + prior and one for the frame predictor (embed,
+LSTM cells with the state updated in place, heads and reparameterisation in one kernel; exact fp32 in both precisions, as
+the eager path's LSTMs).  The module inputs torch.cat([h, global_z | z, tuc, dt]) are read through per-slot index tables.
+
+Layer dispatch (bf16 mode): the 4x4/s2 convolutions with >= 64 channels on both sides are implicit GEMMs
+(p2pvg_conv_gemm kinds 0 / 2) with eval-BatchNorm + activation in their epilogue; the thin 1- / 3-channel ends
+(im2col / col2im + GEMM), the 4x4-valid GEMMs (encoder final, decoder first) and all of the fp32 mode use the explicit
+lowering followed by p2pvg_bn_act, as infer.py does (the training engine's default for the thin ends is the same
+im2col + tensor-core GEMM lowering; its direct thin kernels are opt-in there because they are slower).
+
+Memory: every cached signature (at most MAX_GRAPHS, least recently used evicted) owns its buffers; the ground-truth encode
+covers all len(x) frames of the call.  ``GenerateEngine.memory_bytes()`` reports the total, ``clear()`` frees it.
+
+Noise: eps comes from ONE torch.randn of shape [slots, 2, rows, z] per call, so for a given torch seed the values
+differ from the eager path's per-step draws (the distribution is the same).  Inside ``infer.eps_stream`` the injected
+draws are consumed in the reference's order (posterior, then prior, per executed step).
+"""
+from __future__ import annotations
+
+from collections import OrderedDict
+
+import numpy as np
+import torch
+
+from ._lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH
+
+MAX_GRAPHS = 4
+
+
+def plan_slots(len_output, len_x, probs, skip_prob, n_past, skip_frame, eval_cp_ix):
+    """Executed steps of p2p_generate (reference models/p2p_model.py:126-138): a list of (i, time_until_cp, delta_time,
+    target) per executed step i, in Python doubles exactly as the reference computes them; target = i while a
+    ground-truth frame x[i] exists, else -1 (the posterior then reads h_cpaw, :167-171)."""
+    prev_i, skip_count, out = 0, 0, []
+    max_skip_count = len_x * skip_prob
+    for i in range(1, len_output):
+        if (probs[i - 1] <= skip_prob and i >= n_past and skip_count < max_skip_count and i != 1
+                and i != (len_output - 1) and skip_frame):
+            skip_count += 1
+            continue
+        out.append((i, (eval_cp_ix - i + 1) / eval_cp_ix, (i - prev_i) / eval_cp_ix, i if i < len_x else -1))
+        prev_i = i
+    return out
+
+
+def check_supported(model):
+    """ValueError unless the model is a dcgan_64 / dcgan_128 P2PModel with every module in eval mode."""
+    from .models.backbone import DcganDecoder, DcganEncoder
+    if getattr(model, "is_pose", False) or not isinstance(model.encoder, DcganEncoder) or not isinstance(model.decoder, DcganDecoder):
+        raise ValueError("p2p_generate_graphed supports the dcgan_64 / dcgan_128 backbones only; use p2p_generate for this model")
+    for m in ("encoder", "decoder", "frame_predictor", "posterior", "prior"):
+        if any(mod.training for mod in getattr(model, m).modules()):
+            raise ValueError(f"p2p_generate_graphed needs every module in eval mode ({m} is in training mode); "
+                             "call model.eval() or use p2p_generate")
+
+
+class _Graph:
+    def __init__(self):
+        self.bufs = {}
+        self.graph = None
+        self.ws_gen = None
+
+
+class GenerateEngine:
+    def __init__(self, model):
+        self.model = model
+        self._graphs = OrderedDict()
+
+    # ------------------------------------------------------------------ public entry
+    @torch.no_grad()
+    def generate(self, x, len_output, eval_cp_ix, model_mode="full", skip_frame=False, init_hidden=True, nsample=1):
+        from . import infer
+        model = self.model
+        check_supported(model)
+        if isinstance(x, tuple):
+            x = x[1]
+        if model_mode not in ("full", "posterior", "prior"):
+            raise ValueError(f"unknown model_mode {model_mode!r}")
+        if nsample < 1:
+            raise ValueError("nsample must be >= 1")
+        opt = model.opt
+        T = len(x)
+        B, C, H, W = (int(v) for v in x[0].shape)
+        if H != model.encoder.image_width or W != H or C != model.encoder.nc:
+            raise ValueError(f"frames of shape {tuple(x[0].shape)} do not fit the {model.encoder.image_width}-pixel, "
+                             f"{model.encoder.nc}-channel backbone")
+        n_past = int(opt.n_past)
+        if n_past < 1 or T < min(n_past, len_output):
+            raise ValueError("p2p_generate_graphed needs n_past >= 1 and at least min(n_past, len_output) input frames")
+        rows = nsample * B
+        dev = x[0].device
+        # (1) the reference's NumPy draw, made even when skip_frame is False (models/p2p_model.py:128)
+        probs = np.random.uniform(0, 1, len_output - 1)
+        slots = plan_slots(len_output, T, probs, float(opt.skip_prob), n_past, skip_frame, eval_cp_ix)
+        S = len(slots)
+        lfs = bool(opt.last_frame_skip)
+        adt = infer._act_dtype()
+        K = infer.kernels_for(dev)
+        ptrs = tuple(p.data_ptr() for p in model.parameters()) + tuple(b.data_ptr() for b in model.buffers())
+        sig = (rows, B, T, C, H, len_output, S, model_mode, n_past, lfs, str(adt), ptrs)
+        G = self._graphs.get(sig)
+        if G is not None and G.ws_gen != K.ws_gen:
+            del self._graphs[sig]
+            G = None
+        n_tf = min(n_past - 1, len_output - 1)
+        cfg = dict(rows=rows, B=B, T=T, C=C, W=H, S=S, n_tf=n_tf, mode=model_mode, n_past=n_past, lfs=lfs, adt=adt,
+                   ns=nsample, dev=dev)
+        if not init_hidden:
+            for m in ("posterior", "prior", "frame_predictor"):
+                mod = getattr(model, m)
+                if mod.hidden is None or len(mod.hidden) != mod.n_layers or tuple(mod.hidden[0][0].shape) != (rows, mod.hidden_size):
+                    raise ValueError(f"init_hidden=False needs {m}.hidden of shape [{rows}, {mod.hidden_size}] per layer")
+        # capture on first use of a signature, after one eager warm-up run of the same sequence.  This comes BEFORE the inputs
+        # of the call are written: the graph updates the LSTM state buffers in place, so the warm-up and capture must not
+        # run on the state this call starts from
+        if G is None:
+            G = _Graph()
+            G.cfg = cfg
+            self._alloc_io(G)
+            self._body(G)
+            torch.cuda.current_stream(dev).synchronize()
+            G.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(G.graph):
+                self._body(G)
+            G.ws_gen = K.ws_gen
+            self._graphs[sig] = G
+            while len(self._graphs) > MAX_GRAPHS:
+                self._graphs.popitem(last=False)
+        else:
+            self._graphs.move_to_end(sig)
+        # (2)-(4) inputs of this call: frames, per-slot tables, eps, initial LSTM state
+        xs = x if torch.is_tensor(x) else torch.stack(list(x))
+        G.bufs["x"].copy_(xs.reshape(G.bufs["x"].shape))
+        tab_h = [s if s <= n_tf else T for s in range(S)]                   # h source: ground truth until the first decode
+        tab_i = [t if t >= 0 else tab_h[s] for s, (_, _, _, t) in enumerate(slots)]   # posterior: x[i] or h_cpaw's h
+        tab_z = [0 if (model_mode == "posterior" or (s < n_tf and model_mode == "full")) else 1 for s in range(S)]
+        ints = torch.tensor(tab_i + tab_h + tab_z + [T - 1], dtype=torch.int32)
+        fl = torch.tensor([t for (_, t, _, _) in slots] + [d for (_, _, d, _) in slots], dtype=torch.float64).float()
+        G.bufs["tab_int"].copy_(ints, non_blocking=True)
+        G.bufs["tab_f"][:2 * S].copy_(fl, non_blocking=True)
+        if S:
+            z = model.z_dim
+            if infer._EPS_STREAM is not None:
+                for s in range(S):
+                    for j in (0, 1):
+                        G.bufs["eps"][s, j].copy_(infer._EPS_STREAM.pop(0).to(device=dev, dtype=torch.float32).reshape(rows, z))
+            else:
+                torch.randn(S, 2, rows, z, device=dev, out=G.bufs["eps"])
+        for m in ("posterior", "prior", "frame_predictor"):
+            hs, cs = G.bufs[f"{m}_h"], G.bufs[f"{m}_c"]
+            if init_hidden:
+                hs.zero_()
+                cs.zero_()
+            else:
+                for l, (h, c) in enumerate(getattr(model, m).hidden):
+                    hs[l].copy_(h)
+                    cs[l].copy_(c)
+        # (5) replay
+        G.graph.replay()
+        # (6) fresh tensors out of the static buffers, LSTM state written back as the eager path leaves it
+        out = G.bufs["out"].clone()
+        for m in ("posterior", "prior", "frame_predictor"):
+            hs, cs = G.bufs[f"{m}_h"], G.bufs[f"{m}_c"]
+            getattr(model, m).hidden = [(hs[l].clone(), cs[l].clone()) for l in range(hs.shape[0])]
+        # (7) the returned list: ground truth while i < n_past, zeros for skipped frames
+        executed = {i for (i, _, _, _) in slots}
+        frames, j = [], 0
+        for i in range(1, len_output):
+            if i not in executed:
+                frames.append(None)
+            elif i < n_past:
+                frames.append(x[i])
+            else:
+                frames.append(out[j])
+                j += 1
+        seq = [x[0]] + frames
+        zeros = torch.zeros((rows, C, H, W), device=dev, dtype=x[0].dtype)
+        if nsample == 1:
+            return [f if f is not None else zeros.clone() for f in seq]
+        res = [[] for _ in range(nsample)]
+        for i, f in enumerate(seq):
+            if f is None:
+                f = zeros.clone()
+            elif i == 0 or i < n_past:
+                f = f.repeat(nsample, *([1] * (f.dim() - 1)))
+            for s in range(nsample):
+                res[s].append(f[s * B:(s + 1) * B])
+        return res
+
+    def memory_bytes(self):
+        """Device memory held by the cached graphs' buffers (the graphs' private pools come on top)."""
+        return sum(t.numel() * t.element_size() for G in self._graphs.values() for t in G.bufs.values())
+
+    def clear(self):
+        """Drop every cached graph and its buffers."""
+        self._graphs.clear()
+
+    # ------------------------------------------------------------------ buffers
+    def _alloc_io(self, G):
+        c, model = G.cfg, self.model
+        dev, S, rows = c["dev"], c["S"], c["rows"]
+        b = G.bufs
+        b["x"] = torch.zeros(c["T"] * c["B"], c["C"], c["W"] * c["W"], device=dev)
+        b["tab_int"] = torch.zeros(3 * S + 1, dtype=torch.int32, device=dev)
+        b["tab_f"] = torch.zeros(max(2 * S, 1), device=dev)
+        b["eps"] = torch.zeros(max(S, 1), 2, rows, model.z_dim, device=dev)
+        n_dec = max(S - c["n_tf"], 0)
+        b["out"] = torch.zeros(max(n_dec, 1), rows, c["C"], c["W"], c["W"], device=dev)[:n_dec]
+        for m in ("posterior", "prior", "frame_predictor"):
+            mod = getattr(model, m)
+            for k in ("h", "c"):
+                b[f"{m}_{k}"] = torch.zeros(mod.n_layers, rows, mod.hidden_size, device=dev)   # updated in place by the graph
+
+    def _buf(self, G, name, numel, dtype=torch.float32):
+        t = G.bufs.get(name)
+        if t is None:
+            t = G.bufs[name] = torch.zeros(int(numel), dtype=dtype, device=G.cfg["dev"])
+        assert t.numel() == numel and t.dtype == dtype, name
+        return t
+
+    # ------------------------------------------------------------------ the captured sequence
+    def _body(self, G):
+        from . import infer
+        c, model = G.cfg, self.model
+        K = infer.kernels_for(c["dev"])
+        self.K, self.G = K, G
+        adt, rows, B, T, S, n_tf = c["adt"], c["rows"], c["B"], c["T"], c["S"], c["n_tf"]
+        g, z = model.g_dim, model.z_dim
+        self.chans = infer._stages(model.encoder)
+        self._prepare_weights()
+        # ground truth: one time-batched encode at B rows, tiled to the nsample*B rows of the recurrent part
+        N = T * B
+        hw, nc, W = c["W"] * c["W"], c["C"], c["W"]
+        a = self._buf(G, "gt_in", N * hw * nc, adt)
+        K.permute4(G.bufs["x"], a, (N, hw, nc, 1), (nc * hw, 1, hw, 0))
+        h_gt = self._buf(G, "gt_h", N * g)
+        gt_skips = self._encode("gt", a, N, h_gt)
+        Hsrc = self._buf(G, "Hsrc", (T + 1) * rows * g)     # [T + 1][rows][g]: ground truth frames, then this step's h
+        K.permute4(h_gt, Hsrc, (T, c["ns"], B * g, 1), (B * g, 0, 1, 0))
+        h_cur = Hsrc[T * rows * g:]
+        gsrc_b = self._buf(G, "grp_zero", max(c["ns"], 1), torch.int32)   # source image n % B for every sample
+        n = len(self.chans)
+
+        def gt_skip(f):
+            return [s[f * B * s.numel() // N:(f + 1) * B * s.numel() // N] for s in gt_skips]
+
+        if S > n_tf and not c["lfs"]:
+            # models/p2p_model.py:143-144: the last skip set while i == 1 or i < n_past comes from x[max(n_past - 2, 0)]
+            halves = self._skip_halves("skip", gt_skip(max(c["n_past"] - 2, 0)), B)
+        ti, tf = G.bufs["tab_int"], G.bufs["tab_f"]
+        zbuf = self._buf(G, "Z", 2 * rows * z)
+        h_pred = self._buf(G, "h_pred", rows * g)
+        eps = G.bufs["eps"]
+        prev_frame = None
+        for s in range(S):
+            tuc, dt = tf[s:s + 1], tf[S + s:S + s + 1]
+            skips_cur = None
+            if s > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
+                xin = self._buf(G, "step_in", rows * hw * nc, adt)
+                K.permute4(prev_frame, xin, (rows, hw, nc, 1), (nc * hw, 1, hw, 0))
+                skips_cur = self._encode("step", xin, rows, h_cur)
+            glob = ti[3 * S:3 * S + 1]
+            # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
+            K.lstm_step([self._module("posterior", Hsrc, ti[s:s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 0], out=zbuf[:rows * z]),
+                         self._module("prior", Hsrc, ti[S + s:S + s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 1], out=zbuf[rows * z:])],
+                        rows, model.rnn_size)
+            K.lstm_step([self._module("frame_predictor", Hsrc, ti[S + s:S + s + 1], zbuf, ti[2 * S + s:2 * S + s + 1], z, tuc, dt,
+                                      out=h_pred)], rows, model.rnn_size)
+            if s < n_tf:
+                continue   # teacher-forced step: the predictor only advances its state (models/p2p_model.py:157-163)
+            if c["lfs"]:
+                src = gt_skip(s) if s == n_tf else skips_cur
+                halves = self._skip_halves("skip", src, B if s == n_tf else rows)
+            prev_frame = G.bufs["out"][s - n_tf]
+            self._decode(h_pred, halves, prev_frame)
+
+    # ------------------------------------------------------------------ weights
+    def _prepare_weights(self):
+        K, G, model = self.K, self.G, self.model
+        adt = G.cfg["adt"]
+        enc, dec = model.encoder, model.decoder
+        chans, n, g = self.chans, len(self.chans), model.g_dim
+        self.wp, self.bn = {}, {}
+
+        def coeffs(tag, bn):
+            C = bn.weight.numel()
+            sc, sh = self._buf(G, f"bn_{tag}_scale", C), self._buf(G, f"bn_{tag}_shift", C)
+            K.bn_eval_coeffs(bn.weight.data, bn.bias.data, bn.running_mean, bn.running_var, C, sc, sh, eps=bn.eps)
+            self.bn[tag] = (sc, sh)
+
+        cin = enc.nc
+        for l in range(n + 1):
+            blk = getattr(enc, f"c{l + 1}")
+            conv, bn = (blk.main[0], blk.main[1]) if l < n else (blk[0], blk[1])
+            cout = conv.weight.shape[0]
+            wp = self._buf(G, f"wp_enc{l}", cout * 16 * cin, adt)
+            K.permute4(conv.weight.data, wp, (cout, 4, 4, cin), (cin * 16, 4, 1, 16))
+            self.wp[f"enc{l}"] = wp
+            coeffs(f"enc{l}", bn)
+            cin = cout
+        ctop = chans[-1]
+        convt, bn = dec.upc1[0], dec.upc1[1]
+        wp = self._buf(G, "wp_dec-1", g * 16 * ctop, adt)
+        K.permute4(convt.weight.data, wp, (g, 4, 4, ctop), (ctop * 16, 4, 1, 16))
+        b16 = self._buf(G, "bias16_dec-1", 16 * ctop)
+        K.permute4(convt.bias.data, b16, (16, ctop, 1, 1), (0, 1, 0, 0))
+        self.wp["dec-1"], self.wp["dec-1.bias16"] = wp, b16
+        coeffs("dec-1", bn)
+        for k in range(n):
+            last = k == n - 1
+            blk = getattr(dec, f"upc{k + 2}")
+            convt = blk[0] if last else blk.main[0]
+            ci2, cout = convt.weight.shape[0], convt.weight.shape[1]
+            wp = self._buf(G, f"wp_dec{k}", ci2 * 16 * cout, adt)
+            K.permute4(convt.weight.data, wp, (ci2, 4, 4, cout), (cout * 16, 4, 1, 16))
+            self.wp[f"dec{k}"] = wp
+            if not last:
+                coeffs(f"dec{k}", blk.main[1])
+
+    # ------------------------------------------------------------------ encoder / decoder
+    def _implicit(self, cin, cout):
+        return self.G.cfg["adt"] == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0
+
+    def _encode(self, tag, a, N, h_out):
+        """a: NHWC frames [N, W, W, nc] in the activation dtype -> h_out fp32 [N, g]; returns the skip maps (NHWC)."""
+        K, G, model = self.K, self.G, self.model
+        adt = G.cfg["adt"]
+        enc = model.encoder
+        H, cin = G.cfg["W"], enc.nc
+        skips = []
+        for l, cout in enumerate(self.chans):
+            conv = getattr(enc, f"c{l + 1}").main[0]
+            Ho = H // 2
+            M = N * Ho * Ho
+            sc, sh = self.bn[f"enc{l}"]
+            y = self._buf(G, f"{tag}_enc_y{l}", M * cout, adt)
+            if self._implicit(cin, cout):
+                K.conv_gemm(0, a, self.wp[f"enc{l}"], y, N, Ho, Ho, cin, cout, bias=conv.bias.data, eval_scale=sc, eval_shift=sh,
+                            act=ACT_LRELU)
+            else:
+                col = self._buf(G, f"{tag}_enc_col{l}", M * 16 * cin, adt)
+                raw = self._buf(G, f"{tag}_enc_raw{l}", M * cout, adt)
+                K.im2col(a, col, N, H, H, cin)
+                K.gemm(col, self.wp[f"enc{l}"], raw, M, cout, 16 * cin, bias=conv.bias.data)
+                K.bn_act(raw, y, sc, sh, 1, M, cout, ACT_LRELU)
+            skips.append(y)
+            a, H, cin = y, Ho, cout
+        conv = getattr(enc, f"c{len(self.chans) + 1}")[0]
+        g = model.g_dim
+        sc, sh = self.bn[f"enc{len(self.chans)}"]
+        raw = self._buf(G, f"{tag}_enc_rawf", N * g, adt)
+        y = h_out if adt == torch.float32 else self._buf(G, f"{tag}_enc_yf", N * g, adt)
+        K.gemm(a, self.wp[f"enc{len(self.chans)}"], raw, N, g, 16 * cin, bias=conv.bias.data)
+        K.bn_act(raw, y, sc, sh, 1, N, g, ACT_TANH)
+        if y is not h_out:
+            K.permute4(y, h_out, (N * g, 1, 1, 1), (1, 0, 0, 0))
+        return skips
+
+    def _skip_halves(self, tag, skips, nsrc):
+        """The skip half of every decoder stage's torch.cat([d, skip]) ConvTranspose for one skip source of nsrc images:
+        implicit stages get the bias-free kind-2 product (added in the main GEMM's epilogue), explicit stages the tap
+        products col2 of p2pvg_col2im_k4s2p1.  Returns per stage (tensor, imgs_per_group) for the decodes."""
+        K, G = self.K, self.G
+        adt = G.cfg["adt"]
+        n = len(self.chans)
+        out = []
+        Hi = 4
+        for k in range(n):
+            cd = self.chans[n - 1 - k]
+            cout = self.model.decoder.nc if k == n - 1 else self.chans[n - 2 - k]
+            wS = self.wp[f"dec{k}"][cd * 16 * cout:]
+            sk = skips[n - 1 - k]
+            if self._implicit(cd, cout) and k < n - 1:
+                addS = self._buf(G, f"{tag}_addS{k}", nsrc * 4 * Hi * Hi * cout, adt)
+                K.conv_gemm(2, sk, wS, addS, nsrc, Hi, Hi, cd, cout)
+            else:
+                addS = self._buf(G, f"{tag}_colS{k}", nsrc * Hi * Hi * 16 * cout, adt)
+                K.gemm(sk, wS, addS, nsrc * Hi * Hi, 16 * cout, cd, b_mn=True)
+            out.append((addS, nsrc))
+            Hi *= 2
+        return out
+
+    def _decode(self, h_pred, halves, frame_out):
+        """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied)."""
+        K, G, model = self.K, self.G, self.model
+        adt, rows = G.cfg["adt"], G.cfg["rows"]
+        dec, g = model.decoder, model.g_dim
+        n = len(self.chans)
+        ctop = self.chans[-1]
+        if adt == torch.float32:
+            hp = h_pred
+        else:
+            hp = self._buf(G, "dec_hp", rows * g, adt)
+            K.permute4(h_pred, hp, (rows * g, 1, 1, 1), (1, 0, 0, 0))
+        raw = self._buf(G, "dec_raw-1", rows * 16 * ctop, adt)
+        d = self._buf(G, "dec_d-1", rows * 16 * ctop, adt)
+        K.gemm(hp, self.wp["dec-1"], raw, rows, 16 * ctop, g, b_mn=True, bias=self.wp["dec-1.bias16"])
+        sc, sh = self.bn["dec-1"]
+        K.bn_act(raw, d, sc, sh, 1, rows * 16, ctop, ACT_LRELU)
+        Hi = 4
+        for k in range(n):
+            last = k == n - 1
+            cd = self.chans[n - 1 - k]
+            cout = dec.nc if last else self.chans[n - 2 - k]
+            blk = getattr(dec, f"upc{k + 2}")
+            convt = blk[0] if last else blk.main[0]
+            wD = self.wp[f"dec{k}"][:cd * 16 * cout]
+            addS, nsrc = halves[k]
+            gsrc = self.G.bufs["grp_zero"]
+            Mo = rows * 4 * Hi * Hi
+            y = self._buf(G, f"dec_y{k}", Mo * cout, adt)
+            if self._implicit(cd, cout) and not last:
+                sc, sh = self.bn[f"dec{k}"]
+                K.conv_gemm(2, d, wD, y, rows, Hi, Hi, cd, cout, bias=convt.bias.data, addend=addS, grp_src=gsrc,
+                            imgs_per_group=nsrc, eval_scale=sc, eval_shift=sh, act=ACT_LRELU)
+            else:
+                colD = self._buf(G, f"dec_colD{k}", rows * Hi * Hi * 16 * cout, adt)
+                K.gemm(d, wD, colD, rows * Hi * Hi, 16 * cout, cd, b_mn=True)
+                raw = y if last else self._buf(G, f"dec_raw{k}", Mo * cout, adt)
+                K.col2im(colD, raw, rows, Hi, Hi, cout, bias=convt.bias.data, col2=addS, grp_src=gsrc, imgs_per_group=nsrc)
+                if not last:
+                    sc, sh = self.bn[f"dec{k}"]
+                    K.bn_act(raw, y, sc, sh, 1, Mo, cout, ACT_LRELU)
+            d = y
+            Hi *= 2
+        W, nc = Hi, dec.nc
+        out32 = self._buf(G, "dec_out32", rows * W * W * nc)
+        K.permute4(d, out32, (rows * W * W * nc, 1, 1, 1), (1, 0, 0, 0))
+        K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
+        K.permute4(out32, frame_out, (rows, nc, W * W, 1), (W * W * nc, 1, nc, 0))
+
+    # ------------------------------------------------------------------ recurrent modules
+    def _module(self, m, seg_a, idx_a, seg_b, idx_b, gb, tuc, dt, eps=None, out=None):
+        """p2pvg_lstm_step operands of module m for one step: input [seg_a[idx_a] | seg_b[idx_b] | tuc | dt], state updated in
+        place in the graph's [L][rows][R] buffers, gaussian head (with eps) or Linear + tanh head."""
+        from ._lib import LSTM_HEAD_GAUSSIAN, LSTM_HEAD_LINEAR_TANH
+        G, mod = self.G, getattr(self.model, m)
+        dev = G.cfg["dev"]
+        tabs = G.bufs.get(f"{m}_ptrs")
+        if tabs is None:   # device tables of pointers (the parameter addresses are part of the graph's signature)
+            hs, cs = G.bufs[f"{m}_h"], G.bufs[f"{m}_c"]
+            w = [t.data_ptr() for c in mod.lstm for t in (c.weight_ih, c.bias_ih, c.weight_hh, c.bias_hh)]
+            st = [t.data_ptr() for l in range(mod.n_layers) for t in (hs[l], cs[l], hs[l], cs[l])]
+            tabs = G.bufs[f"{m}_ptrs"] = torch.tensor(w + st, dtype=torch.int64, device=dev)
+        L = mod.n_layers
+        d = dict(seg_a=seg_a, idx_a=idx_a, ga=self.model.g_dim, seg_b=seg_b, idx_b=idx_b, gb=gb, tuc=tuc, dt=dt,
+                 w_embed=mod.embed.weight, b_embed=mod.embed.bias, layers=L, layer_w=tabs[:4 * L], state=tabs[4 * L:], out=out)
+        if hasattr(mod, "mu_net"):
+            d.update(head=LSTM_HEAD_GAUSSIAN, out_dim=mod.output_size, w_out=mod.mu_net.weight, b_out=mod.mu_net.bias,
+                     w_out2=mod.logvar_net.weight, b_out2=mod.logvar_net.bias, eps=eps)
+        else:
+            d.update(head=LSTM_HEAD_LINEAR_TANH, out_dim=mod.output_size, w_out=mod.output[0].weight, b_out=mod.output[0].bias)
+        return d

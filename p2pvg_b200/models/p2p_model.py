@@ -195,6 +195,15 @@ class P2PModel(nn.Module):
         from ..infer import p2p_generate_samples
         return p2p_generate_samples(self, x, nsample, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame)
 
+    def p2p_generate_graphed(self, x, len_output, eval_cp_ix, model_mode='full', skip_frame=False, init_hidden=True, nsample=1):
+        """p2p_generate (nsample=1) or p2p_generate_samples (nsample>1) as one CUDA-graph replay per call (an addition to the
+        reference API; see gen_engine.py).  dcgan_64 / dcgan_128 in eval mode only: anything else raises ValueError."""
+        from ..gen_engine import GenerateEngine
+        if getattr(self, "_gen_engine", None) is None:
+            self._gen_engine = GenerateEngine(self)
+        return self._gen_engine.generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
+                                         init_hidden=init_hidden, nsample=nsample)
+
     # ---- checkpoints (same dict layout as reference p2p_model.py:289-330) --------------------------
     def save(self, fname, epoch):
         backbone_net, optimizer = self.opt.backbone_net, getattr(self.opt, "optimizer", None)
