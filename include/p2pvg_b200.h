@@ -225,7 +225,7 @@ int p2pvg_lstm_scan_fwd(const float* pre, const float* whh, const float* bhh, fl
 int p2pvg_lstm_scan_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
                         int tf32, unsigned* counter, void* stream);
 /* diagnostics: cudaOccupancyMaxActiveClusters of the hidden-size-512 scans (clusters of 16 CTAs): which = 0 / 1 / 3 forward with
- * 16- / 32- / 48-row slabs, 2 / 4 / 5 backward with 16- / 32- / 48-row slabs; -1 on error */
+ * 16- / 32- / 48-row slabs; any other value the backward scan (its only instance, 16-row slabs); -1 on error */
 int p2pvg_lstm_cluster512_max_clusters(int which);
 /* the same for the hidden-size-256 scans (clusters of 8 CTAs): which = 0 / 1 forward with 16- / 32-row slabs, 2 / 3 backward */
 int p2pvg_lstm_cluster_max_clusters(int which);

@@ -173,7 +173,9 @@ lstm_cl_fwd_kernel(const float* __restrict__ pre, const float* __restrict__ whh,
 #pragma unroll
       for (int g = 0; g < 4; g++) z[g] = (Gs[row * GL + g * UBc + uu] + Gs[MB * GL + row * GL + g * UBc + uu]) + (zp[h][g] + bh[h][g]);
       const float ig = fast_sigmoid(z[0]), fg = fast_sigmoid(z[1]), gg = fast_tanh(z[2]), og = fast_sigmoid(z[3]);
-      const float c = fg * c_reg[h] + ig * gg;
+      // the rounding order is spelled out: left to FMA contraction, instances differed (R = 128 fused f*c at 16-row slabs and
+      // i*g at 32-row slabs), and a row's c depended on the batch size
+      const float c = fmaf(ig, gg, __fmul_rn(fg, c_reg[h]));
       c_reg[h] = c;
       // the state the other CTAs wait for goes out first
       hs[((long long)(s + 1) * B + r0 + row) * R + u0 + uu] = og * fast_tanh(c);
