@@ -116,6 +116,12 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Second pass of split-K (gemm_simt.cu, gemm_tc.cu, conv_gemm.cu), defined in gemm_tc.cu: C[M, N] = sum_z partial[z] + bias[n]
+// + addend[m, n] + (accumulate ? C : 0), partial [splits][M][N] fp32, or [splits][N][M] when transposed; C and addend are
+// c_dtype.  Deterministic: each element is summed by one thread in ascending z.
+int p2pvg_splitk_reduce(const float* partial, int splits, void* C, int c_dtype, long long ldc, int M, int N, int accumulate,
+                        const float* bias, const void* addend, long long ldd, int transposed, cudaStream_t st);
+
 #define DISPATCH_DTYPE(dt, T, ...)                                   \
   do {                                                               \
     if ((dt) == P2PVG_F32) { typedef float T; __VA_ARGS__; }         \

@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const TI* __restrict__ A
       int gn = n0 + tx * 4 + j;
       if (gn >= N) continue;
       float v = acc[i][j];
-      if (partial) {  // split-K: raw partial sums, finished by simt_splitk_reduce_kernel
+      if (partial) {  // split-K: raw partial sums, finished by p2pvg_splitk_reduce
         partial[((long long)blockIdx.z * M + gm) * N + gn] = v;
         continue;
       }
@@ -89,22 +89,6 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const TI* __restrict__ A
       if (accumulate) v += ld_f<TO>(&C[gm * ldc + gn]);
       st_f<TO>(&C[gm * ldc + gn], v);
     }
-  }
-}
-
-template <typename TO>
-__global__ void simt_splitk_reduce_kernel(const float* __restrict__ partial, int splits, TO* __restrict__ C, long long ldc, int M, int N,
-                                          int accumulate, const float* __restrict__ bias, const TO* __restrict__ addend, long long ldd) {
-  const long long total = (long long)M * N;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-    const long long m = idx / N;
-    const int n = (int)(idx - m * N);
-    float acc = 0.f;
-    for (int z = 0; z < splits; z++) acc += partial[(long long)z * total + idx];
-    if (bias) acc += bias[n];
-    if (addend) acc += ld_f<TO>(&addend[m * ldd + n]);
-    if (accumulate) acc += ld_f<TO>(&C[m * ldc + n]);
-    st_f<TO>(&C[m * ldc + n], acc);
   }
 }
 
@@ -142,13 +126,6 @@ int p2pvg_gemm_simt(const void* A, int in_dtype, int a_mn, long long lda, const 
     return P2PVG_ERR_BAD_ARG;
   }
 #undef LAUNCH
-  if (splits > 1) {
-    long long total = (long long)M * N;
-    int blocks = (int)((total + 255) / 256 > 1184 ? 1184 : (total + 255) / 256);
-    if (c_dtype == P2PVG_BF16)
-      simt_splitk_reduce_kernel<bf16><<<blocks, 256, 0, stream>>>(partial, splits, (bf16*)C, ldc, M, N, accumulate, bias, (const bf16*)addend, ldd);
-    else
-      simt_splitk_reduce_kernel<float><<<blocks, 256, 0, stream>>>(partial, splits, (float*)C, ldc, M, N, accumulate, bias, (const float*)addend, ldd);
-  }
+  if (splits > 1) return p2pvg_splitk_reduce(partial, splits, C, c_dtype, ldc, M, N, accumulate, bias, addend, ldd, 0, stream);
   return p2pvg_check_launch("gemm_simt");
 }

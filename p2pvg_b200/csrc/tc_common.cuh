@@ -1,4 +1,6 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a).
+// The persistent wgmma skeleton of the tensor-core GEMM (gemm_tc.cu) and the implicit-GEMM convolutions (conv_gemm.cu), sm_90a:
+// the wgmma / TMA / mbarrier PTX wrappers, the tile configuration and shared-memory carve-up, the MMA warpgroup loop, the
+// epilogue's staging-buffer reads and row stores, and the host side (driver entry point, SM count, tensor maps, launch).
 #pragma once
 #include <cuda.h>
 
@@ -150,15 +152,6 @@ __device__ __forceinline__ void acc_to_smem(const float (&acc)[2][BN / 2], float
     }
   }
 }
-// 32 consecutive fp32 accumulator columns of one staged row
-__device__ __forceinline__ void acc_row32(const float* src, uint32_t* v) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 x = *reinterpret_cast<const float4*>(src + j);
-    v[j] = __float_as_uint(x.x); v[j + 1] = __float_as_uint(x.y); v[j + 2] = __float_as_uint(x.z); v[j + 3] = __float_as_uint(x.w);
-  }
-}
-
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -192,5 +185,250 @@ __device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
   return v[0];
 }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// ------------------------------------------------------------------ the persistent skeleton
+// 384 threads: warps 0..3 = epilogue (one tile row per thread), warps 4..7 = the MMA warpgroup, warp 8 = TMA producer (warps
+// 9..11 only complete its warpgroup).  grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...  The
+// MMA warpgroup accumulates tile i+1 in registers while the epilogue drains tile i from the staging buffer.  Each kernel keeps
+// its own TMA producer loop and tile decode, and what its epilogue does between reading a chunk and storing it.
+constexpr int BLOCK_M = 128;
+constexpr int ROW_BYTES = 128;  // one SWIZZLE_128B row: 64 bf16 or 32 fp32 (tf32) along the contiguous dimension
+constexpr int A_STAGE_BYTES = BLOCK_M * ROW_BYTES;
+constexpr int NUM_THREADS = 384;
+
+// 128 x 64 / 128 x 128 tiles: one warpgroup holds the whole fp32 accumulator in registers (64 / 128 per thread)
+template <int BN> struct Cfg {
+  static constexpr int B_STAGE_BYTES = BN * ROW_BYTES;
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  static constexpr int STAGES = (BN == 128) ? 4 : 7;
+  static constexpr int ACC_LD = BN + 4;   // staging row pitch in floats: the row-per-thread float4 reads are conflict-free
+  static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
+};
+
+// resident-weight mode (conv kind 0, BN = 64): weights at [0, 9 * 8 KB), A ring of 6 x 16 KB behind them
+constexpr int BRES_B_BYTES = 9 * 64 * 128, BRES_STAGES = 6;
+static_assert(BRES_B_BYTES + BRES_STAGES * A_STAGE_BYTES <= Cfg<64>::STAGES * Cfg<64>::STAGE_BYTES, "resident weights + A ring");
+
+// the dynamic shared memory: operand stages, [BLOCK_M][ACC_LD] staging buffer, barriers
+struct Smem {
+  uint8_t* ring;
+  float* accs;
+  uint64_t *full_bar, *empty_bar, *acc_full_bar, *acc_empty_bar;
+  uint64_t* bres_bar;   // the resident weights have landed (conv only)
+};
+
+template <int BN>
+__device__ __forceinline__ Smem smem_setup(uint8_t* smem_raw) {
+  using C_ = Cfg<BN>;
+  Smem s;
+  s.ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  s.accs = reinterpret_cast<float*>(s.ring + C_::STAGES * C_::STAGE_BYTES);
+  s.full_bar = reinterpret_cast<uint64_t*>(s.ring + C_::STAGES * C_::STAGE_BYTES + C_::ACC_BYTES);
+  s.empty_bar = s.full_bar + C_::STAGES;
+  s.acc_full_bar = s.empty_bar + C_::STAGES;
+  s.acc_empty_bar = s.acc_full_bar + 1;
+  s.bres_bar = s.acc_empty_bar + 1;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < C_::STAGES; i++) {
+      mbar_init(&s.full_bar[i], 1);
+      mbar_init(&s.empty_bar[i], 128);   // every thread of the MMA warpgroup
+    }
+    mbar_init(s.acc_full_bar, 128);
+    mbar_init(s.acc_empty_bar, 4);       // one arrival per epilogue warp
+    mbar_init(s.bres_bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  return s;
+}
+
+// The MMA warpgroup: for each tile of this CTA, the K blocks of its split z, then the accumulator into the staging buffer.
+// bres: B is the resident weight tap kb and A streams through the BRES_STAGES ring (gemm_tc passes false).
+template <bool TF32, int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_loop(const Smem& sm, int num_tiles, int tiles_mn, int splits, int kb_per_split, int nkb_total,
+                                         bool bres) {
+  using C_ = Cfg<BN>;
+  const int wt = threadIdx.x - 128;
+  const uint32_t smem0 = smem_u32(sm.ring);
+  // MN-major: the 64-element chunks along m / n are 8 KB apart (MN-major operands are bf16)
+  const uint64_t da0 = A_MN ? make_desc(smem0, 64 * 128, 1024) : make_desc(smem0, 0, 1024);
+  const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, 64 * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
+  uint32_t it = 0, lt = 0;
+  if (bres) mbar_wait(sm.bres_bar, 0);   // the resident weights have landed
+  const uint64_t da0r = make_desc(smem0 + BRES_B_BYTES, 0, 1024), db0r = make_desc(smem0, 0, 1024);
+  float acc[2][BN / 2];
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
+    const int z = (splits == 1) ? 0 : t / tiles_mn;   // phases (conv kind 2) never split K
+    const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
+    int prev = -1;   // stage of the previous K block: released once its MMAs have completed
+    for (int kb = kb0; kb < kb1; kb++, it++) {
+      // (both divisors are compile-time constants: no runtime division in the per-K-block path)
+      const int s = bres ? (int)(it % BRES_STAGES) : (int)(it % C_::STAGES);
+      const uint32_t par = (bres ? (it / BRES_STAGES) : (it / C_::STAGES)) & 1;
+      mbar_wait(&sm.full_bar[s], par);
+      // descriptors of stage 0 / k 0 are built once; the start-address field (bits 0-13, address >> 4) is advanced by
+      // plain additions
+      const uint64_t stage_off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
+      const uint64_t a_off = bres ? (uint64_t)((uint32_t)s * (uint32_t)(A_STAGE_BYTES >> 4)) : stage_off;
+      const uint64_t b_off = bres ? (uint64_t)((uint32_t)kb * (uint32_t)((64 * 128) >> 4)) : stage_off;   // resident: tap kb
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      wgmma_fence();
+      wgmma_kblock<TF32, BN, A_MN, B_MN>(acc, (bres ? da0r : da0) + a_off, (bres ? db0r : db0) + b_off, kb == kb0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (prev >= 0) mbar_arrive(&sm.empty_bar[prev]);
+      prev = s;
+    }
+    wgmma_wait<0>();
+    fence_regs(acc[0]);
+    fence_regs(acc[1]);
+    if (prev >= 0) mbar_arrive(&sm.empty_bar[prev]);
+    mbar_wait(sm.acc_empty_bar, (lt & 1) ^ 1);   // the epilogue has drained the previous tile
+    acc_to_smem<BN>(acc, sm.accs, C_::ACC_LD, wt);
+    mbar_arrive(sm.acc_full_bar);
+  }
+}
+
+// Epilogue (threads 0..127): dst[i] = src[n0 + i] for i < BN (0 past N), staged while the MMAs are still running.  The
+// caller double-buffers dst by tile parity and synchronises the epilogue warps before reading it.
+template <int BN>
+__device__ __forceinline__ void stage_cols(float* dst, const float* src, int n0, int N) {
+  for (int i = threadIdx.x; i < BN; i += 128) dst[i] = (n0 + i < N) ? src[n0 + i] : 0.f;
+}
+
+// Epilogue: the staged accumulator columns [32 c, 32 c + 32) of tile row `row`.  After the tile's last chunk is read the
+// staging buffer goes back to the MMA warpgroup *before* the caller's global stores.
+template <int BN>
+__device__ __forceinline__ void read_chunk(const Smem& sm, int row, int c, float (&f)[32]) {
+  const float* src = sm.accs + row * Cfg<BN>::ACC_LD + c * 32;
+#pragma unroll
+  for (int j = 0; j < 32; j += 4) {
+    const float4 x = *reinterpret_cast<const float4*>(src + j);
+    f[j] = x.x; f[j + 1] = x.y; f[j + 2] = x.z; f[j + 3] = x.w;
+  }
+  if (c == BN / 32 - 1) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(sm.acc_empty_bar);
+  }
+}
+
+// f[0..31] += 32 columns staged by stage_cols
+__device__ __forceinline__ void add_staged32(float (&f)[32], const float* s) {
+#pragma unroll
+  for (int j = 0; j < 32; j += 4) {
+    const float4 b4 = *reinterpret_cast<const float4*>(s + j);
+    f[j] += b4.x; f[j + 1] += b4.y; f[j + 2] += b4.z; f[j + 3] += b4.w;
+  }
+}
+
+// f[j] += row[j] for the j < ncols (TAIL) or all 32 (!TAIL) columns
+template <typename T, bool TAIL>
+__device__ __forceinline__ void add_row32(float (&f)[32], const T* row, int ncols) {
+#pragma unroll
+  for (int j = 0; j < 32; j++)
+    if (!TAIL || j < ncols) f[j] += ld_f<T>(row + j);
+}
+
+// One 32-column segment of an output row: (accumulate ? crow : 0) + f, stored as 256-bit stores when crow is 32-byte aligned,
+// 128-bit stores otherwise.  TAIL (gemm_tc): fewer than 32 valid columns (ncols) or a row that is not 16-byte aligned is
+// stored element by element; without TAIL all 32 columns are valid and crow is 16-byte aligned.
+template <typename T, bool TAIL>
+__device__ __forceinline__ void store_row32(T* crow, float (&f)[32], int accumulate, int ncols) {
+  if (accumulate) add_row32<T, TAIL>(f, crow, ncols);
+  const bool vec = !TAIL || (ncols >= 32 && (reinterpret_cast<uintptr_t>(crow) & 15) == 0);
+  if (vec && (reinterpret_cast<uintptr_t>(crow) & 31) == 0) {
+    if constexpr (sizeof(T) == 2) {
+#pragma unroll
+      for (int j = 0; j < 32; j += 16)
+        st_global_256(crow + j, pack_bf16x2(f[j], f[j + 1]), pack_bf16x2(f[j + 2], f[j + 3]), pack_bf16x2(f[j + 4], f[j + 5]),
+                      pack_bf16x2(f[j + 6], f[j + 7]), pack_bf16x2(f[j + 8], f[j + 9]), pack_bf16x2(f[j + 10], f[j + 11]),
+                      pack_bf16x2(f[j + 12], f[j + 13]), pack_bf16x2(f[j + 14], f[j + 15]));
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; j += 8)
+        st_global_256(crow + j, __float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
+                      __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7]));
+    }
+  } else if (vec) {
+    if constexpr (sizeof(T) == 2) {
+#pragma unroll
+      for (int j = 0; j < 32; j += 8)
+        *reinterpret_cast<uint4*>(crow + j) =
+            make_uint4(pack_bf16x2(f[j], f[j + 1]), pack_bf16x2(f[j + 2], f[j + 3]), pack_bf16x2(f[j + 4], f[j + 5]), pack_bf16x2(f[j + 6], f[j + 7]));
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(crow + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; j++)
+      if (j < ncols) st_f<T>(crow + j, f[j]);
+  }
+}
+
+// ------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+struct Driver {
+  EncodeTiledFn encode = nullptr;   // cuTensorMapEncodeTiled; nullptr when the driver does not provide it
+  int sms = 132;                    // SMs of the device that is current at the first call
+};
+
+// resolved once, on first use
+inline const Driver& driver() {
+  static const Driver d = [] {
+    Driver r;
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
+      r.sms = sms;
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      r.encode = reinterpret_cast<EncodeTiledFn>(fn);
+    (void)cudaGetLastError();
+    return r;
+  }();
+  return d;
+}
+
+// 2-D tensor map of bf16 (elem 2) or fp32 (elem 4) elements: dim0 (contiguous) x dim1, row pitch ld elements, box
+// (128 B x box1), 128B swizzle, zero OOB fill
+inline int map2d(CUtensorMap* map, const void* base, long long dim0, long long dim1, long long ld, int box1, int elem = 2) {
+  cuuint64_t dims[2] = {(cuuint64_t)dim0, (cuuint64_t)dim1};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * elem};
+  cuuint32_t box[2] = {(cuuint32_t)(ROW_BYTES / elem), (cuuint32_t)box1};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = driver().encode(map, elem == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base),
+                               dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    p2pvg_set_error("cuTensorMapEncodeTiled failed (%d): base=%p dims=(%lld,%lld) ld=%lld box1=%d", (int)r, base, dim0, dim1, ld, box1);
+    return P2PVG_ERR_CUDA;
+  }
+  return P2PVG_OK;
+}
+
+// Launches KERN (a skeleton kernel with BN-wide tiles) on the persistent grid min(tiles, SMs).  The dynamic shared memory limit
+// is raised on the first launch of each kernel instance.
+template <auto KERN, int BN, typename... Args>
+int launch_persistent(long long tiles, cudaStream_t st, const char* what, Args... args) {
+  static bool smem_attr_set = false;
+  if (!smem_attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
+    if (e != cudaSuccess) {
+      p2pvg_set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
+      return P2PVG_ERR_CUDA;
+    }
+    smem_attr_set = true;
+  }
+  const int sms = driver().sms;
+  KERN<<<(int)(tiles < sms ? tiles : sms), NUM_THREADS, Cfg<BN>::SMEM_BYTES, st>>>(args...);
+  return p2pvg_check_launch(what);
+}
 
 }  // namespace tc

@@ -1,5 +1,4 @@
 """h36m pose backbone: host-side schedule (p2pvg_b200/engine_mlp.py) on CPU against the oracle."""
-import os
 
 import numpy as np
 import torch
@@ -18,7 +17,7 @@ CFG = dict(g_dim=128, z_dim=10, rnn_size=64, backbone="mlp", predictor_rnn_layer
 
 
 def run(optkw, T, B, np_seed=0, mode="A"):
-    torch.set_num_threads(min(8, os.cpu_count() or 1))
+    torch.set_num_threads(8)   # the split of torch's CPU reductions follows the thread count: the same on every host
     state = O.build_state(CFG, seed=1)
     opt = O.default_opt(**optkw)
     opt["batch_size"] = opt["batch_size"] or B

@@ -1,5 +1,4 @@
 """vgg_64 backbone: host-side schedule (p2pvg_b200/engine_vgg.py) on CPU against the oracle."""
-import os
 
 import numpy as np
 import torch
@@ -31,7 +30,7 @@ def make_cfg(channels, width=64):
 
 
 def run(optkw, T, B, channels=3, np_seed=0, mode="A", width=64):
-    torch.set_num_threads(min(8, os.cpu_count() or 1))
+    torch.set_num_threads(8)   # the split of torch's CPU reductions follows the thread count: the same on every host
     cfg = make_cfg(channels, width)
     state = O.build_state(cfg, seed=1)
     opt = O.default_opt(**optkw)

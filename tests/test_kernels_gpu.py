@@ -71,8 +71,8 @@ TC_SHAPES = [
 
 
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn", TC_SHAPES)
-def test_gemm_tcgen05(KS, M, N, K, a_mn, b_mn):
-    """The tensor-core GEMM (the name predates its port from tcgen05 to wgmma) against the emulation, every operand major."""
+def test_gemm_tc(KS, M, N, K, a_mn, b_mn):
+    """The tensor-core GEMM against the emulation, every operand major."""
     Kc, Ke = KS
     assert Kc.has_tc_gemm(), "driver entry point cuTensorMapEncodeTiled not available"
     Kc.set_gemm_impl("tc")
@@ -96,7 +96,7 @@ def test_gemm_tcgen05(KS, M, N, K, a_mn, b_mn):
         Kc.set_gemm_impl("auto")
 
 
-def test_gemm_tcgen05_strided_views(KS):
+def test_gemm_tc_strided_views(KS):
     """Sub-matrix operands (leading dimension > extent), as the engine uses for packed weight halves."""
     Kc, Ke = KS
     Kc.set_gemm_impl("tc")

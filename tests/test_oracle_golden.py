@@ -73,7 +73,9 @@ def test_skip_schedule_bit_exact(case):
 @pytest.mark.parametrize("case", CASES)
 def test_train_step_matches_reference(case):
     fix = load(case)
-    torch.set_num_threads(min(8, os.cpu_count() or 1))
+    # the fixtures were made with 8 threads (golden/make_golden.py); torch splits its CPU reductions by thread count, not
+    # by core count, so a host with fewer cores must still run 8 to reproduce them within the tolerances below
+    torch.set_num_threads(8)
     state = O.build_state(fix["cfg"], seed=fix["init_seed"])
     adam = {m: O.new_adam_state(state[m]) for m in O.MODULES}
     width = fix["cfg"]["image_width"]
