@@ -37,7 +37,7 @@ struct p2pvg_conv_fusion;
 #define P2PVG_ACT_LRELU 1 /* LeakyReLU(0.2): models/dcgan_64.py:10,22 */
 #define P2PVG_ACT_TANH 2  /* models/dcgan_64.py:45, models/lstm.py:18 */
 #define P2PVG_ACT_RELU 4   /* models/h36m_mlp.py:33-41 */
-#define P2PVG_ACT_SIGMOID 3 /* models/dcgan_64.py:77 (stand-alone decoder forward; act_fwd only) */
+#define P2PVG_ACT_SIGMOID 3 /* models/dcgan_64.py:77 (stand-alone decoder forward) */
 
 /* 200: the sm_90a library (wgmma tensor-core kernels); p2pvg_has_tcgen05 of version 100 is now p2pvg_has_tc_gemm. */
 int p2pvg_version(void);
@@ -289,6 +289,7 @@ int p2pvg_align(const float* H, const int* in_idx, const float* h_pred, int P, i
 int p2pvg_colsum(const void* x, int dtype, int64_t rows, int cols, int64_t ld, float* out, int accumulate, void* ws /* >= 1024*cols floats */,
                  size_t ws_bytes, void* stream);
 int p2pvg_act_fwd(float* x, int64_t n, int act, void* stream);
+/* dx = dy * act'(x), the derivative taken from the forward output y = act(x) (in place: x == y). */
 int p2pvg_act_bwd(const float* dy, const float* y, float* dx, int64_t n, int act, void* stream);
 
 /* nn.Sigmoid (models/dcgan_64.py:77) + nn.MSELoss (models/p2p_model.py:254,256): per-group sum of squared error

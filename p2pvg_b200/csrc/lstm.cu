@@ -242,6 +242,7 @@ __global__ void act_bwd_kernel(const float* __restrict__ dy, const float* __rest
     float yv = y[i], g = 1.f;
     if (act == P2PVG_ACT_TANH) g = 1.f - yv * yv;
     else if (act == P2PVG_ACT_LRELU) g = yv > 0.f ? 1.f : 0.2f;
+    else if (act == P2PVG_ACT_SIGMOID) g = yv * (1.f - yv);
     else if (act == P2PVG_ACT_RELU) g = yv > 0.f ? 1.f : 0.f;
     dx[i] = dy[i] * g;
   }
