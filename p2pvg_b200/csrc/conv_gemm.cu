@@ -237,6 +237,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     constexpr bool do_stat = STAT;   // a separate instantiation: the statistics cost ~50 registers in this epilogue
     // eval-mode BatchNorm coefficients of the tile's columns, double-buffered by tile parity like bias_s: [parity][scale | shift][BN]
     __shared__ float ev_s[EVAL ? 2 * 2 * BN : 1];
+    // plain bf16 stores of kinds 0 / 2 (no statistics, no eval epilogue, no accumulation, no addend) take the row-cooperative
+    // path.  With an addend the thread-per-row path stays: it requests a row's addend before waiting for the accumulator, and
+    // the row-cooperative loads, issued after it, made the skip-connection layers slower (dcgan_64 dec2 2.18 -> 3.08 ms).
+    const bool row_major_store = !STAT && !EVAL && KIND != 1 && c_bf16 && !accumulate && addend == nullptr;
     uint32_t lt = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
       const int ph = (KIND == 2) ? (t & 3) : 0;
@@ -284,6 +288,36 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const bool use_add = (KIND != 1) && addend != nullptr && row_ok;
       const long long aoff0 = add_row * g.Ntot + n0;   // element offset of this row's first addend column
       const bool abf = g.add_bf16 != 0;
+      if (row_major_store) {
+        // Row-cooperative bf16 stores: LPR lanes share one output row, 16 B (8 columns) each, so one warp instruction writes
+        // RPI whole rows instead of 32 scattered 16-byte pieces of 32 rows.  The row addresses come from the lane that owns
+        // the row.  Same arithmetic per element as below: acc + bias, rounded once to bf16.
+        constexpr int LPR = BN / 8, RPI = 32 / LPR;
+        const int sub = lane / LPR, cl = (lane % LPR) * 8;
+        const bool col_ok = n0 + cl < g.Ntot;   // Ntot is a multiple of 32: 8-column groups are all in or all out
+        bf16* cbase = reinterpret_cast<bf16*>(Cv) + n0 + cl;
+        mbar_wait(sm.acc_full_bar, lt & 1);
+#pragma unroll
+        for (int i = 0; i < 32 / RPI; i++) {
+          const int src = i * RPI + sub;   // the warp row this lane writes in step i
+          const long long orow = __shfl_sync(0xffffffffu, out_row, src);
+          const bool ok = __shfl_sync(0xffffffffu, (int)row_ok, src) != 0;
+          const float* s = sm.accs + (q * 32 + src) * C_::ACC_LD + cl;
+          const float4 x0 = *reinterpret_cast<const float4*>(s), x1 = *reinterpret_cast<const float4*>(s + 4);
+          if (i == 32 / RPI - 1) {   // the warp's last staging read of this tile
+            __syncwarp();
+            if (lane == 0) mbar_arrive(sm.acc_empty_bar);
+          }
+          if (!ok || !col_ok) continue;
+          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+          if (bias) {
+#pragma unroll
+            for (int j = 0; j < 8; j++) f[j] += bias_s[acc * BN + cl + j];
+          }
+          *reinterpret_cast<uint4*>(cbase + orow * ldc) = pack16<bf16>(f);
+        }
+        continue;
+      }
       float4 a4[16];  // addend of the next 64 columns, requested before the accumulator is waited for
       if (use_add) addend_load64(a4, addend, aoff0, abf);
       mbar_wait(sm.acc_full_bar, lt & 1);
