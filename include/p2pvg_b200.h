@@ -327,6 +327,19 @@ int p2pvg_adam_legacy(float* p, const float* g, float* m, float* v, int64_t n, d
                       double eps, const int* step_ptr, void* stream);
 int p2pvg_scale(float* x, int64_t n, float a, void* stream);
 
+/* Moving MNIST training batches (DynamicLengthMovingMNIST.__getitem__, data/moving_mnist.py:51-105) rendered on the device.
+ *   digits [n_digits][32][32] uint8 (MNIST resized to 32 x 32), converted to fp32 as u / 255 (ToTensor)
+ *   draws  [B][num_digits][draw_stride] int32: the values every np.random.randint(lo, hi) call of (sequence b, digit n) returns,
+ *          in the reference's call order (digit index, sx, sy, dx, dy, then up to four per step at the wall bounces), taken as
+ *          lo + r % (hi - lo); draw_stride >= 5 + 4T
+ *   out    [T][B][1][S][S] fp32, time-major (the generator's permute(1, 0, 2, 3, 4)[:T]); 16-byte aligned
+ * Each frame is the fp32 sum of the digits in digit order, clipped at 1 (x[x > 1] = 1): bit-identical to the reference for the
+ * same draws.  T frames of a max_seq_len sequence are its first T frames (later draws do not change earlier frames).
+ * P2PVG_ERR_BAD_ARG: S < 33 or S % 4 != 0, num_digits outside 1..4, draw_stride < 5 + 4T, NULL pointers, n_digits < 1.
+ * P2PVG_ERR_UNSUPPORTED: num_digits * (1024 + 5 + 4T) * 4 bytes of draws and digits exceed 48 KB of shared memory. */
+int p2pvg_moving_mnist(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B, int S,
+                       int num_digits, int deterministic, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

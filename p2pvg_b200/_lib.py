@@ -396,3 +396,11 @@ class CudaKernels:
 
     def scale(self, x, n, a):
         self._ck(self.lib.p2pvg_scale(_p(x), _i64(n), _f(a), self._stream()))
+
+    # -- data ------------------------------------------------------------------------------
+    def moving_mnist(self, digits, draws, out, T, B, S, num_digits, deterministic):
+        """digits uint8 [N,32,32], draws int32 [B,num_digits,stride], out fp32 [T,B,1,S,S] (p2pvg_moving_mnist)."""
+        assert digits.dtype == torch.uint8 and draws.dtype == torch.int32 and out.dtype == torch.float32
+        assert digits.is_contiguous() and draws.is_contiguous() and out.is_contiguous()
+        self._ck(self.lib.p2pvg_moving_mnist(_p(digits), _i(digits.shape[0]), _p(draws), _i(draws.shape[-1]), _p(out), _i(T), _i(B),
+                                             _i(S), _i(num_digits), _i(int(deterministic)), self._stream()))

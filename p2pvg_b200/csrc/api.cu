@@ -105,6 +105,7 @@ int p2pvg_convt_c1_loss_impl(const void*, const void*, int, const int*, const fl
                              int, void*, float*, cudaStream_t);
 int p2pvg_adam_legacy_impl(float*, const float*, float*, float*, long long, double, double, double, double, const int*, cudaStream_t);
 int p2pvg_scale_impl(float*, long long, float, cudaStream_t);
+int p2pvg_moving_mnist_impl(const uint8_t*, int, const int32_t*, int, float*, int, int, int, int, int, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -354,5 +355,9 @@ int p2pvg_adam_legacy(float* p, const float* g, float* m, float* v, int64_t n, d
   return p2pvg_adam_legacy_impl(p, g, m, v, n, lr, beta1, beta2, eps, step_ptr, ST);
 }
 int p2pvg_scale(float* x, int64_t n, float a, void* stream) { return p2pvg_scale_impl(x, n, a, ST); }
+int p2pvg_moving_mnist(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B, int S,
+                       int num_digits, int deterministic, void* stream) {
+  return p2pvg_moving_mnist_impl(digits, n_digits, draws, draw_stride, out, T, B, S, num_digits, deterministic, ST);
+}
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-"""Host -> device input pipeline for the train step (SURVEY.md §8f rank 3: "device-side data path").
+"""Input pipeline for the train step (SURVEY.md §8f rank 3: "device-side data path").
 
 The reference loop (train.py:212, data/data_utils.py:129-137) does ``x = next(generator); x = x.cuda()`` and then calls the
 model, so the H2D copy of a 126 MB batch (T=30, B=256, 64x64) sits on the critical path of every step.
@@ -7,10 +7,87 @@ batch i trains, and is handed out only after the compute stream has been made to
 
     for x in DevicePrefetcher(loader, device):      # x: device tensor, time-major like the reference's normalize_data
         losses = model(x, 0, cp_ix)
+
+Moving MNIST needs no host batches at all: ``MovingMNIST`` renders each batch on the device (``p2pvg_moving_mnist``) from
+the digits loaded once by ``load_mnist_digits``.
+
+    for x in MovingMNIST(load_mnist_digits(root), batch_size=256, max_seq_len=30, delta_len=5):
+        losses = model(x, 0, len(x) - 1)
 """
 from __future__ import annotations
 
+import gzip
+import os
+
+import numpy as np
 import torch
+
+DIGIT_SIZE = 32
+
+
+def _read_idx_images(path):
+    opener = gzip.open if path.endswith(".gz") else open
+    with opener(path, "rb") as f:
+        raw = f.read()
+    if len(raw) < 16 or int.from_bytes(raw[0:4], "big") != 0x803:
+        raise ValueError(f"{path}: not an idx3-ubyte image file")
+    n, rows, cols = (int.from_bytes(raw[i:i + 4], "big") for i in (4, 8, 12))
+    if len(raw) != 16 + n * rows * cols:
+        raise ValueError(f"{path}: {len(raw) - 16} bytes of pixels for {n} images of {rows}x{cols}")
+    return np.frombuffer(raw, dtype=np.uint8, offset=16).reshape(n, rows, cols)
+
+
+def load_mnist_digits(root, train=True):
+    """MNIST images as uint8 [N, 32, 32]: torchvision's raw files ``<root>/MNIST/raw/{train,t10k}-images-idx3-ubyte[.gz]``,
+    each 28x28 digit resized with PIL bilinear, which is what the reference's ``transforms.Scale(32)`` did to the PIL image
+    (data/moving_mnist.py:27-35).  Never downloads: missing files raise FileNotFoundError."""
+    from PIL import Image
+    base = os.path.join(root, "MNIST", "raw", ("train" if train else "t10k") + "-images-idx3-ubyte")
+    path = next((p for p in (base, base + ".gz") if os.path.isfile(p)), None)
+    if path is None:
+        raise FileNotFoundError(f"MNIST images not found: expected {base} or {base}.gz")
+    imgs = _read_idx_images(path)
+    out = np.empty((len(imgs), DIGIT_SIZE, DIGIT_SIZE), dtype=np.uint8)
+    for i, a in enumerate(imgs):
+        out[i] = np.asarray(Image.fromarray(a).resize((DIGIT_SIZE, DIGIT_SIZE), Image.BILINEAR))
+    return torch.from_numpy(out)
+
+
+class MovingMNIST:
+    """Endless iterator of Moving MNIST training batches rendered on the device: fp32 [T, B, 1, S, S], time-major, what the
+    reference's ``get_generator`` yields after ``.permute(1, 0, 2, 3, 4).cuda()[:seq_len]`` (data/data_utils.py:112-122).
+
+    Per batch: ``T = np.random.randint(max_seq_len - 2 * delta_len, max_seq_len + 1)`` from NumPy's global stream, exactly
+    where ``get_seq_len()`` is called there (so the stream ``P2PModel.forward`` draws from is unchanged); one ``torch.randint``
+    of the trajectory draws on the device from ``generator`` (same distribution as the reference's worker-process NumPy draws,
+    other values); one kernel launch into a fresh tensor (a batch handed out is never written again)."""
+
+    def __init__(self, digits, batch_size, max_seq_len, delta_len, image_size=64, num_digits=2, deterministic=False,
+                 device="cuda", generator=None):
+        from ._lib import kernels_for
+        digits = torch.as_tensor(digits)
+        if digits.dtype != torch.uint8 or digits.dim() != 3 or tuple(digits.shape[1:]) != (DIGIT_SIZE, DIGIT_SIZE) or len(digits) == 0:
+            raise ValueError(f"digits must be a non-empty uint8 tensor [N, 32, 32], got {digits.dtype} {tuple(digits.shape)}")
+        if max_seq_len - 2 * delta_len < 1 or delta_len < 0:
+            raise ValueError(f"max_seq_len = {max_seq_len}, delta_len = {delta_len}: sequence lengths must be >= 1")
+        self.K = kernels_for(device)
+        self.device = self.K.device
+        self.digits = digits.to(self.device).contiguous()
+        self.batch_size, self.max_seq_len, self.delta_len = int(batch_size), int(max_seq_len), int(delta_len)
+        self.image_size, self.num_digits, self.deterministic = int(image_size), int(num_digits), bool(deterministic)
+        self.generator = generator
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        T = int(np.random.randint(self.max_seq_len - 2 * self.delta_len, self.max_seq_len + 1))
+        B, S, nd = self.batch_size, self.image_size, self.num_digits
+        with torch.cuda.device(self.device):
+            draws = torch.randint(0, 2 ** 31 - 1, (B, nd, 5 + 4 * T), dtype=torch.int32, device=self.device, generator=self.generator)
+            out = torch.empty(T, B, 1, S, S, dtype=torch.float32, device=self.device)
+            self.K.moving_mnist(self.digits, draws, out, T, B, S, nd, self.deterministic)
+        return out
 
 
 def _chain_front(first, rest):
