@@ -39,7 +39,9 @@ struct p2pvg_conv_fusion;
 #define P2PVG_ACT_RELU 4   /* models/h36m_mlp.py:33-41 */
 #define P2PVG_ACT_SIGMOID 3 /* models/dcgan_64.py:77 (stand-alone decoder forward) */
 
-/* 200: the sm_90a library (wgmma tensor-core kernels); p2pvg_has_tcgen05 of version 100 is now p2pvg_has_tc_gemm. */
+/* 200: the sm_90a library (wgmma tensor-core kernels); p2pvg_has_tcgen05 of version 100 is now p2pvg_has_tc_gemm.
+ * 201: p2pvg_conv_fusion lost its reserved backward-BatchNorm members (bwd_raw ... bwd_stat_partial, rows_per_group), and
+ *      p2pvg_conv_thin_in, p2pvg_convT_thin_out, p2pvg_bn_bwd_finalize_tiles and p2pvg_bn_bwd_apply were removed. */
 int p2pvg_version(void);
 const char* p2pvg_last_error(void);
 /* 1 when the wgmma/TMA GEMM can be used on this process' device (driver entry points resolved). */
@@ -97,7 +99,6 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
  *                     (sum y, sum y^2) of the tile's rows, y as stored (bf16-rounded for a bf16 output).  The tile of GEMM
  *                     row block mt and phase ph is row mt*phases + ph; reduce per group with p2pvg_bn_fwd_finalize_tiles
  *                     (rows of one BatchNorm group must be a multiple of 128).
- *   bwd_*             reserved for the BatchNorm-backward reduction of a data-gradient GEMM (sum dz, sum dz*xhat).
  *   addend_dtype      the skip-half addend may be stored in bf16 (it is the output of another p2pvg_conv_gemm call).
  *   eval_scale/shift  kinds 0 and 2: nn.BatchNorm2d in eval mode + activation applied in the epilogue (generation,
  *                     models/p2p_model.py:80-183 with running statistics): the stored output is
@@ -106,13 +107,6 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
  *                     fwd_stat_partial or accumulate (P2PVG_ERR_BAD_ARG). */
 typedef struct p2pvg_conv_fusion {
   void* fwd_stat_partial;
-  const void* bwd_raw;
-  const float* bwd_mean;
-  const float* bwd_invstd;
-  const float* bwd_scale;
-  const float* bwd_shift;
-  void* bwd_stat_partial;
-  int64_t rows_per_group;
   int addend_dtype; /* dtype of `addend`: P2PVG_F32 (default, also without a fusion struct) or P2PVG_BF16 (half the epilogue read traffic) */
   const float* eval_scale;
   const float* eval_shift;
@@ -134,17 +128,6 @@ int p2pvg_maxpool2_bwd(const void* x, const void* dy, void* dx, int dtype, int N
 int p2pvg_upsample2_fwd(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream);
 int p2pvg_upsample2_bwd(const void* dy, void* dx, int dtype, int N, int H, int W, int C, void* stream);
 int p2pvg_gather_add(void* dst, int dtype, const float* src, const int* grp_src, int G, int64_t n, void* stream);
-
-/* Thin ends of the dcgan stacks (1 or 3 image channels on one side; HBM-bound direct kernels, fp32 master weights):
- *   conv_thin_in : y[N,H/2,W/2,Co] = conv4x4/s2/p1(x[N,H,W,Ci<=4]) . w[Co][Ci][4][4] + bias   — encoder c1 forward
- *                  (models/dcgan_64.py:34) and the data-gradient of the last decoder layer (its ConvT weight [Cin][nc][4][4]
- *                  has this layout with Co = Cin)
- *   convT_thin_out: y[N,2H,2W,Co<=3] = convT4x4/s2/p1(x[N,H,W,Ci]) . w[Ci][Co][4][4] + bias + addend[src] — last decoder layer
- *                  forward (models/dcgan_64.py:76); y_dtype = the activation dtype or fp32 (for the skip addend). */
-int p2pvg_conv_thin_in(const void* x, int dtype, const float* w, const float* bias, void* y, int N, int H, int W, int Ci, int Co,
-                       void* stream);
-int p2pvg_convT_thin_out(const void* x, int dtype, const float* w, const float* bias, const float* addend, const int* grp_src,
-                         int imgs_per_group, void* y, int y_dtype, int N, int H, int W, int Ci, int Co, void* stream);
 
 /* 4x4 / stride 2 / pad 1 lowering (nn.Conv2d(nin,nout,4,2,1), models/dcgan_64.py:8; and the data-gradient of
  * nn.ConvTranspose2d(nin,nout,4,2,1), models/dcgan_64.py:20): x [N,H,W,C] -> col [N*H/2*W/2, 16*C], K order (kh,kw,c). */
@@ -183,19 +166,13 @@ int p2pvg_bn_act(const void* x, void* y, int dtype, const float* scale, const fl
 int p2pvg_bn_bwd(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
                  const float* gamma, int G, int64_t R, int C, int act, void* ws, size_t ws_bytes, void* dx, float* sum_dz,
                  float* sum_dzx, const float* scale, const float* shift, void* stream);
-/* The same two BatchNorm reductions when their per-tile column sums were produced by a GEMM epilogue (p2pvg_conv_fusion):
+/* The forward statistics when their per-tile column sums were produced by a GEMM epilogue (p2pvg_conv_fusion):
  * partial is float2 [G * parts_per_group][ldp]; channel c of group g sums the group's partial rows over the `fold` column
  * groups f*C + c (a GEMM row may hold several pixels / filter taps of one channel).  R = elements per (group, channel).
  * fp64 combine in a fixed order (deterministic).  Replaces the statistics pass of nn.BatchNorm2d (models/dcgan_64.py:9). */
 int p2pvg_bn_fwd_finalize_tiles(const void* partial, int parts_per_group, int ldp, int fold, int G, int64_t R, int C,
                                 const float* gamma, const float* beta, float eps, float* mean, float* invstd, float* var_unbiased,
                                 float* scale, float* shift, void* stream);
-int p2pvg_bn_bwd_finalize_tiles(const void* partial, int parts_per_group, int ldp, int fold, int G, int C, float* sum_dz,
-                                float* sum_dzx, void* stream);
-/* apply pass of the BatchNorm + activation backward alone (the per-channel sums sum_dz / sum_dzx are given) */
-int p2pvg_bn_bwd_apply(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
-                       const float* gamma, int G, int64_t R, int C, int act, void* dx, const float* sum_dz, const float* sum_dzx,
-                       const float* scale, const float* shift, void* stream);
 /* eval-mode BatchNorm (running statistics; generate.py / p2p_generate): scale = gamma/sqrt(rvar+eps), shift = beta-rmean*scale */
 int p2pvg_bn_eval_coeffs(const float* gamma, const float* beta, const float* rmean, const float* rvar, float eps, int C,
                          float* scale, float* shift, void* stream);
@@ -209,11 +186,11 @@ int p2pvg_lstm_pointwise_fwd(float* gates, const float* c_prev, float* c_out, fl
 int p2pvg_lstm_pointwise_bwd(const float* dh, const float* dc_next, const float* gates, const float* c_prev, const float* c,
                              float* dgates, float* dc_prev, int B, int R, void* stream);
 /* Whole-sequence recurrence of one nn.LSTMCell layer in ONE persistent launch (the W_hh slice of a CTA stays on chip for all
- * timesteps).  tf32 = 1 dispatches by hidden size: R in {64,128,256}: thread-block clusters of 8 CTAs, hardware cluster barrier per
- * timestep; R = 512: clusters of 16 CTAs (non-portable size), forward slabs of 16 / 32 / 48 batch rows per cluster chosen so that
+ * timesteps).  tf32 = 1 dispatches by hidden size: R in {64,128,256}: thread-block clusters of 8 CTAs, slabs of 16 batch rows per
+ * cluster (32 above 128 rows), hardware cluster barrier per timestep; R = 512: clusters of 16 CTAs (non-portable size), forward slabs of 16 / 32 / 48 batch rows per cluster chosen so that
  * the resident clusters cover the batch in as few waves as possible, backward in 16-row slabs with the reduction scattered through
- * distributed shared memory; the part of the weight slice that does not fit the registers lives in shared memory.  tf32 = 0 (and
- * P2PVG_LSTM_CLUSTER=0): cooperative grid with a grid barrier per timestep, exact fp32 FFMA products.
+ * distributed shared memory; the part of the weight slice that does not fit the registers lives in shared memory.  tf32 = 0:
+ * cooperative grid with a grid barrier per timestep, exact fp32 FFMA products.
  *   forward : gates_s = pre_s + b_hh + h_{s-1}.W_hh^T -> (i,f,g,o) -> c_s, h_s       pre [S,B,4R] = x-part incl. b_ih
  *             gates [S,B,4R] out (activations), hs / cs [S+1,B,R] with slot 0 = initial state (zeros, models/lstm.py:21-27)
  *   backward: dh_s = dhtop_s + dG_{s+1}.W_hh, cell backward -> dG [S,B,4R] (gradient w.r.t. the gate pre-activations)

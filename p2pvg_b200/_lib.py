@@ -60,10 +60,8 @@ def _p(t):
 
 class ConvFusion(ctypes.Structure):
     """p2pvg_conv_fusion_t (include/p2pvg_b200.h)."""
-    _fields_ = [("fwd_stat_partial", ctypes.c_void_p), ("bwd_raw", ctypes.c_void_p), ("bwd_mean", ctypes.c_void_p),
-                ("bwd_invstd", ctypes.c_void_p), ("bwd_scale", ctypes.c_void_p), ("bwd_shift", ctypes.c_void_p),
-                ("bwd_stat_partial", ctypes.c_void_p), ("rows_per_group", ctypes.c_int64), ("addend_dtype", ctypes.c_int),
-                ("eval_scale", ctypes.c_void_p), ("eval_shift", ctypes.c_void_p), ("act", ctypes.c_int)]
+    _fields_ = [("fwd_stat_partial", ctypes.c_void_p), ("addend_dtype", ctypes.c_int), ("eval_scale", ctypes.c_void_p),
+                ("eval_shift", ctypes.c_void_p), ("act", ctypes.c_int)]
 
 
 class LstmStepModule(ctypes.Structure):
@@ -202,13 +200,6 @@ class CudaKernels:
                                           _i(Cn), _i(Cm), _p(bias), _p(addend), _p(grp_src), _i(imgs_per_group), _i(int(accumulate)),
                                           _p(ws), _sz(ws.numel()), fusion, self._stream()))
 
-    def conv_thin_in(self, x, w, bias, y, N, H, W, Ci, Co):
-        self._ck(self.lib.p2pvg_conv_thin_in(_p(x), _i(_dt(x)), _p(w), _p(bias), _p(y), _i(N), _i(H), _i(W), _i(Ci), _i(Co), self._stream()))
-
-    def convT_thin_out(self, x, w, bias, y, N, H, W, Ci, Co, addend=None, grp_src=None, imgs_per_group=0):
-        self._ck(self.lib.p2pvg_convT_thin_out(_p(x), _i(_dt(x)), _p(w), _p(bias), _p(addend), _p(grp_src), _i(imgs_per_group), _p(y),
-                                               _i(_dt(y)), _i(N), _i(H), _i(W), _i(Ci), _i(Co), self._stream()))
-
     # -- conv lowering ---------------------------------------------------------------------
     def im2col(self, x, col, N, H, W, C):
         self._ck(self.lib.p2pvg_im2col_k4s2p1(_p(x), _p(col), _i(_dt(x)), _i(N), _i(H), _i(W), _i(C), self._stream()))
@@ -273,14 +264,6 @@ class CudaKernels:
         self._ck(self.lib.p2pvg_bn_fwd_finalize_tiles(_p(partial), _i(parts_per_group), _i(ldp), _i(fold), _i(G), _i64(R), _i(C), _p(gamma),
                                                       _p(beta), _f(eps), _p(mean), _p(invstd), _p(var_unb), _p(scale), _p(shift),
                                                       self._stream()))
-
-    def bn_bwd_finalize_tiles(self, partial, parts_per_group, ldp, fold, G, C, sum_dz, sum_dzx):
-        self._ck(self.lib.p2pvg_bn_bwd_finalize_tiles(_p(partial), _i(parts_per_group), _i(ldp), _i(fold), _i(G), _i(C), _p(sum_dz),
-                                                      _p(sum_dzx), self._stream()))
-
-    def bn_bwd_apply(self, dy, x, y, mean, invstd, gamma, G, R, C, act, dx, sum_dz, sum_dzx, scale=None, shift=None):
-        self._ck(self.lib.p2pvg_bn_bwd_apply(_p(dy), _p(x), _p(y), _i(_dt(x)), _p(mean), _p(invstd), _p(gamma), _i(G), _i64(R), _i(C),
-                                             _i(act), _p(dx), _p(sum_dz), _p(sum_dzx), _p(scale), _p(shift), self._stream()))
 
     def bn_act(self, x, y, scale, shift, G, R, C, act):
         self._ck(self.lib.p2pvg_bn_act(_p(x), _p(y), _i(_dt(x)), _p(scale), _p(shift), _i(G), _i64(R), _i(C), _i(act), self._stream()))

@@ -4,7 +4,6 @@
 #include <string.h>
 
 #include "../../include/p2pvg_b200.h"
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -39,16 +38,10 @@ int p2pvg_layernorm_fwd_impl(const float*, const float*, const float*, float*, f
 int p2pvg_layernorm_bwd_impl(const float*, const float*, const float*, const float*, const float*, float*, float*, float*, long long, int,
                              void*, size_t, cudaStream_t);
 int p2pvg_mse_plain_impl(const float*, const float*, const int*, const float*, int, long long, float*, float*, int, cudaStream_t);
-int p2pvg_conv_thin_in_impl(const void*, int, const float*, const float*, void*, int, int, int, int, int, cudaStream_t);
-int p2pvg_convT_thin_out_impl(const void*, int, const float*, const float*, const float*, const int*, int, void*, int, int, int, int, int,
-                              int, cudaStream_t);
 int p2pvg_conv_gemm_impl(int, const void*, const void*, long long, void*, int, long long, int, int, int, int, int, int, const float*,
                          const float*, const int*, int, int, void*, size_t, void*, int, const float*, const float*, int, cudaStream_t);
 int p2pvg_bn_fwd_finalize_tiles_impl(const void*, int, int, int, int, long long, int, const float*, const float*, float, float*, float*, float*,
                                      float*, float*, cudaStream_t);
-int p2pvg_bn_bwd_finalize_tiles_impl(const void*, int, int, int, int, int, float*, float*, cudaStream_t);
-int p2pvg_bn_bwd_apply_impl(const void*, const void*, const void*, int, const float*, const float*, const float*, int, long long, int, int,
-                            void*, const float*, const float*, const float*, const float*, cudaStream_t);
 int p2pvg_im2col_k4s2p1_impl(const void*, void*, int, int, int, int, int, cudaStream_t);
 int p2pvg_im2col3_impl(const void*, void*, int, int, int, int, int, int, int, cudaStream_t);
 int p2pvg_col2im3_impl(const void*, void*, int, int, int, int, int, int, const float*, cudaStream_t);
@@ -114,7 +107,7 @@ int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
 
 extern "C" {
 
-int p2pvg_version(void) { return 200; }
+int p2pvg_version(void) { return 201; }
 const char* p2pvg_last_error(void) { return g_err; }
 int p2pvg_has_tc_gemm(void) { return p2pvg_gemm_tc_available(); }
 int p2pvg_set_gemm_impl(int impl) {
@@ -154,22 +147,12 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
                     void* workspace, size_t ws_bytes, const p2pvg_conv_fusion_t* fusion, void* stream) {
   P2PVG_REQUIRE(a && b && c, P2PVG_ERR_BAD_ARG, "conv_gemm: null operand");
   void* fwd_stat = fusion ? fusion->fwd_stat_partial : nullptr;
-  P2PVG_REQUIRE(!fusion || fusion->bwd_stat_partial == nullptr, P2PVG_ERR_UNSUPPORTED, "conv_gemm: backward BatchNorm fusion is reserved");
   P2PVG_REQUIRE(!(fwd_stat && accumulate), P2PVG_ERR_BAD_ARG, "conv_gemm: statistics of an accumulating GEMM are not defined");
   const int add_dt = fusion ? fusion->addend_dtype : P2PVG_F32;
   P2PVG_REQUIRE(add_dt == P2PVG_F32 || add_dt == P2PVG_BF16, P2PVG_ERR_BAD_ARG, "conv_gemm: bad addend dtype %d", add_dt);
   return p2pvg_conv_gemm_impl(kind, a, b, ldb, c, c_dtype, ldc, N, H, W, Ck, Cn, Cm, bias, reinterpret_cast<const float*>(addend), grp_src,
                               imgs_per_group, accumulate, workspace, ws_bytes, fwd_stat, add_dt, fusion ? fusion->eval_scale : nullptr,
                               fusion ? fusion->eval_shift : nullptr, fusion ? fusion->act : 0, ST);
-}
-
-int p2pvg_conv_thin_in(const void* x, int dtype, const float* w, const float* bias, void* y, int N, int H, int W, int Ci, int Co,
-                       void* stream) {
-  return p2pvg_conv_thin_in_impl(x, dtype, w, bias, y, N, H, W, Ci, Co, ST);
-}
-int p2pvg_convT_thin_out(const void* x, int dtype, const float* w, const float* bias, const float* addend, const int* grp_src,
-                         int imgs_per_group, void* y, int y_dtype, int N, int H, int W, int Ci, int Co, void* stream) {
-  return p2pvg_convT_thin_out_impl(x, dtype, w, bias, addend, grp_src, imgs_per_group, y, y_dtype, N, H, W, Ci, Co, ST);
 }
 
 int p2pvg_im2col_k4s2p1(const void* x, void* col, int dtype, int N, int H, int W, int C, void* stream) {
@@ -240,15 +223,6 @@ int p2pvg_bn_fwd_finalize_tiles(const void* partial, int parts_per_group, int ld
   return p2pvg_bn_fwd_finalize_tiles_impl(partial, parts_per_group, ldp, fold, G, R, C, gamma, beta, eps, mean, invstd, var_unbiased, scale,
                                           shift, ST);
 }
-int p2pvg_bn_bwd_finalize_tiles(const void* partial, int parts_per_group, int ldp, int fold, int G, int C, float* sum_dz,
-                                float* sum_dzx, void* stream) {
-  return p2pvg_bn_bwd_finalize_tiles_impl(partial, parts_per_group, ldp, fold, G, C, sum_dz, sum_dzx, ST);
-}
-int p2pvg_bn_bwd_apply(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
-                       const float* gamma, int G, int64_t R, int C, int act, void* dx, const float* sum_dz, const float* sum_dzx,
-                       const float* scale, const float* shift, void* stream) {
-  return p2pvg_bn_bwd_apply_impl(dy, x, y, dtype, mean, invstd, gamma, G, R, C, act, dx, sum_dz, sum_dzx, scale, shift, ST);
-}
 int p2pvg_bn_param_grad(const float* sum_dz, const float* sum_dzx, int G, int C, float* dgamma, float* dbeta, void* stream) {
   return p2pvg_bn_param_grad_impl(sum_dz, sum_dzx, G, C, dgamma, dbeta, ST);
 }
@@ -267,24 +241,18 @@ int p2pvg_lstm_pointwise_bwd(const float* dh, const float* dc_next, const float*
                              float* dgates, float* dc_prev, int B, int R, void* stream) {
   return p2pvg_lstm_pointwise_bwd_impl(dh, dc_next, gates, c_prev, c, dgates, dc_prev, B, R, ST);
 }
-// tensor-core mode: thread-block-cluster scans (lstm_cluster.cu) for R in {64,128,256}, lstm_cluster512.cu for R = 512; P2PVG_LSTM_CLUSTER=0 keeps the
-// cooperative-grid scans, which also serve the exact-fp32 mode
-static bool cluster_scan_enabled() {
-  static const int off = [] { const char* e = getenv("P2PVG_LSTM_CLUSTER"); return (e != nullptr && e[0] == '0') ? 1 : 0; }();
-  return !off;
-}
-// R = 512 (BASELINE config 5) runs on clusters of 16 CTAs (lstm_cluster512.cu)
-static bool use_cluster_scan(int R) { return cluster_scan_enabled() && p2pvg_lstm_cluster_supported(R); }
+// tensor-core mode: thread-block-cluster scans, clusters of 16 CTAs for R = 512 (BASELINE config 5, lstm_cluster512.cu) and of 8
+// CTAs for R in {64,128,256} (lstm_cluster.cu); the exact-fp32 mode runs the cooperative-grid scans
 int p2pvg_lstm_scan_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B, int R,
                         int tf32, unsigned* counter, void* stream) {
-  if (tf32 && R == 512 && cluster_scan_enabled()) return p2pvg_lstm_cluster512_fwd_impl(pre, whh, bhh, gates, hs, cs, S, B, ST);
-  if (tf32 && use_cluster_scan(R)) return p2pvg_lstm_cluster_fwd_impl(pre, whh, bhh, gates, hs, cs, S, B, R, ST);
+  if (tf32 && R == 512) return p2pvg_lstm_cluster512_fwd_impl(pre, whh, bhh, gates, hs, cs, S, B, ST);
+  if (tf32 && p2pvg_lstm_cluster_supported(R)) return p2pvg_lstm_cluster_fwd_impl(pre, whh, bhh, gates, hs, cs, S, B, R, ST);
   return p2pvg_lstm_scan_fwd_impl(pre, whh, bhh, gates, hs, cs, S, B, R, tf32, counter, ST);
 }
 int p2pvg_lstm_scan_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
                         int tf32, unsigned* counter, void* stream) {
-  if (tf32 && R == 512 && cluster_scan_enabled()) return p2pvg_lstm_cluster512_bwd_impl(dhtop, whh, gates, cs, dG, S, B, ST);
-  if (tf32 && use_cluster_scan(R)) return p2pvg_lstm_cluster_bwd_impl(dhtop, whh, gates, cs, dG, S, B, R, ST);
+  if (tf32 && R == 512) return p2pvg_lstm_cluster512_bwd_impl(dhtop, whh, gates, cs, dG, S, B, ST);
+  if (tf32 && p2pvg_lstm_cluster_supported(R)) return p2pvg_lstm_cluster_bwd_impl(dhtop, whh, gates, cs, dG, S, B, R, ST);
   return p2pvg_lstm_scan_bwd_impl(dhtop, whh, gates, cs, dG, S, B, R, tf32, counter, ST);
 }
 int p2pvg_lstm_cluster512_max_clusters(int which) { return p2pvg_lstm_cluster512_max_clusters_impl(which); }

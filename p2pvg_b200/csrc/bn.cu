@@ -129,15 +129,14 @@ __global__ void bn_fwd_finalize_kernel(const double2* __restrict__ partial, int 
 
 // Statistics whose per-tile column sums came out of a GEMM epilogue (conv_gemm / gemm_tc `stat_partial`): partial is
 // [G * parts_per_group][ldp] float2 (sum, sum of squares); channel c of group g = sum over the group's partial rows and
-// over the `fold` column groups f*C + c (a GEMM row may hold several pixels / taps of the same channel).
-// MODE 0: forward statistics -> mean / invstd / unbiased var / scale / shift.   MODE 1: (sum dz, sum dz*xhat).
+// over the `fold` column groups f*C + c (a GEMM row may hold several pixels / taps of the same channel), giving
+// mean / invstd / unbiased var / scale / shift.
 // Block = 32 channels x 8 part-lanes, fp64 combine, fixed order (deterministic).
-template <int MODE>
 __global__ void __launch_bounds__(256) bn_finalize_tiles_kernel(const float2* __restrict__ partial, int parts_per_group, int ldp, int fold,
                                                                 int G, int C, double count, const float* __restrict__ gamma,
-                                                                const float* __restrict__ beta, float eps, float* __restrict__ o0,
-                                                                float* __restrict__ o1, float* __restrict__ o2, float* __restrict__ o3,
-                                                                float* __restrict__ o4) {
+                                                                const float* __restrict__ beta, float eps, float* __restrict__ mean,
+                                                                float* __restrict__ invstd, float* __restrict__ var_unbiased,
+                                                                float* __restrict__ scale, float* __restrict__ shift) {
   const int g = blockIdx.y, cl = threadIdx.x & 31, pl = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + cl;
   double a = 0.0, b = 0.0;
@@ -159,21 +158,16 @@ __global__ void __launch_bounds__(256) bn_finalize_tiles_kernel(const float2* __
   if (pl == 0 && c < C) {
     for (int k = 1; k < 8; k++) { a += sa[k][cl]; b += sb[k][cl]; }
     const long long idx = (long long)g * C + c;
-    if (MODE == 0) {
-      const double m = a / count;
-      double var = b / count - m * m;
-      if (var < 0.0) var = 0.0;
-      const double is = 1.0 / sqrt(var + (double)eps);
-      o0[idx] = (float)m;
-      o1[idx] = (float)is;
-      o2[idx] = (float)(count > 1.0 ? var * count / (count - 1.0) : var);
-      const float sc = gamma[c] * (float)is;
-      o3[idx] = sc;
-      o4[idx] = beta[c] - (float)m * sc;
-    } else {
-      o0[idx] = (float)a;
-      o1[idx] = (float)b;
-    }
+    const double m = a / count;
+    double var = b / count - m * m;
+    if (var < 0.0) var = 0.0;
+    const double is = 1.0 / sqrt(var + (double)eps);
+    mean[idx] = (float)m;
+    invstd[idx] = (float)is;
+    var_unbiased[idx] = (float)(count > 1.0 ? var * count / (count - 1.0) : var);
+    const float sc = gamma[c] * (float)is;
+    scale[idx] = sc;
+    shift[idx] = beta[c] - (float)m * sc;
   }
 }
 
@@ -436,33 +430,7 @@ int p2pvg_bn_fwd_finalize_tiles_impl(const void* partial, int parts_per_group, i
   P2PVG_REQUIRE(partial && parts_per_group > 0 && fold > 0 && ldp >= fold * C, P2PVG_ERR_BAD_ARG, "bn_fwd_finalize_tiles: bad partial layout");
   if (G == 0) return P2PVG_OK;
   dim3 grid(cdiv(C, 32), G);
-  bn_finalize_tiles_kernel<0><<<grid, 256, 0, st>>>((const float2*)partial, parts_per_group, ldp, fold, G, C, (double)R, gamma, beta, eps, mean,
-                                                    invstd, var_unbiased, scale, shift);
+  bn_finalize_tiles_kernel<<<grid, 256, 0, st>>>((const float2*)partial, parts_per_group, ldp, fold, G, C, (double)R, gamma, beta, eps, mean,
+                                                 invstd, var_unbiased, scale, shift);
   return p2pvg_check_launch("bn_fwd_finalize_tiles");
-}
-
-int p2pvg_bn_bwd_finalize_tiles_impl(const void* partial, int parts_per_group, int ldp, int fold, int G, int C, float* sum_dz, float* sum_dzx,
-                                     cudaStream_t st) {
-  P2PVG_REQUIRE(partial && parts_per_group > 0 && fold > 0 && ldp >= fold * C, P2PVG_ERR_BAD_ARG, "bn_bwd_finalize_tiles: bad partial layout");
-  if (G == 0) return P2PVG_OK;
-  dim3 grid(cdiv(C, 32), G);
-  bn_finalize_tiles_kernel<1><<<grid, 256, 0, st>>>((const float2*)partial, parts_per_group, ldp, fold, G, C, 1.0, nullptr, nullptr, 0.f, sum_dz,
-                                                    sum_dzx, nullptr, nullptr, nullptr);
-  return p2pvg_check_launch("bn_bwd_finalize_tiles");
-}
-
-// BatchNorm + activation backward, APPLY pass only (the two per-channel sums are given): dx = gamma*invstd*(dz - mean(dz) - xhat*mean(dz*xhat))
-int p2pvg_bn_bwd_apply_impl(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd, const float* gamma,
-                            int G, long long R, int C, int act, void* dx, const float* sum_dz, const float* sum_dzx, const float* scale,
-                            const float* shift, cudaStream_t st) {
-  P2PVG_REQUIRE(y != nullptr || (act == P2PVG_ACT_LRELU && scale && shift), P2PVG_ERR_BAD_ARG,
-                "bn_bwd_apply: y may only be omitted for LeakyReLU with scale/shift supplied");
-  const int vec = dtype == P2PVG_BF16 ? 8 : 4;
-  if (int e = check_bn_shape(C, vec, "bn_bwd_apply")) return e;
-  if (G == 0) return P2PVG_OK;
-  Chunking ch = choose_chunks(R, C, vec);
-  dim3 grid(ch.nchunk, G);
-  DISPATCH_DTYPE(dtype, T, (bn_bwd_apply_kernel<T><<<grid, 256, 0, st>>>((const T*)dy, (const T*)x, (const T*)y, mean, invstd, gamma, sum_dz,
-                                                                         sum_dzx, R, C, ch.rows_per_chunk, act, (T*)dx, scale, shift)));
-  return p2pvg_check_launch("bn_bwd_apply");
 }

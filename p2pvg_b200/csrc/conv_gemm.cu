@@ -15,7 +15,6 @@
 // kind 3  y[N,H,W,Cn] = conv3x3_s1_p1(x[N,H,W,Ck]) . W[Cn, (tap, Ck)] + bias + addend      vgg layer forward (kind 0 geometry, 9 taps)
 // kind 4  g[Cm, (tap, Cn)] = sum_pix a[pix, Cm]^T . gather_3x3(b)[pix, tap, Cn]             vgg weight gradients (kind 1 geometry)
 // kind 5  kind 3 with mirrored tap offsets (pixel - (kh-1, kw-1)): the data gradient of a 3x3 convolution
-#include <cstdlib>
 
 #include "tc_common.cuh"
 
@@ -439,11 +438,6 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, l
   return launch_t<KIND, BN, false, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
 }
 
-bool env_off(const char* name) {
-  const char* v = getenv(name);
-  return v != nullptr && v[0] == '0';
-}
-
 }  // namespace
 
 // a, b: see the kind table at the top.  H, W: SMALL-map size.  Returns P2PVG_ERR_UNSUPPORTED when the shape does not
@@ -455,9 +449,6 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   float2* stat_partial = reinterpret_cast<float2*>(stat_partial_v);
   EvalEpi ev;
   ev.scale = eval_scale; ev.shift = eval_shift; ev.act = act;
-  // 64 -> 64 channel 3x3 layers: weights resident in shared memory (P2PVG_CONV_BRES=0 disables); kind 1 / 4 with 64 output
-  // channels: swapped operand roles (P2PVG_K1_SWAP=0 disables).  Read at the first call.
-  static const bool bres_on = !env_off("P2PVG_CONV_BRES"), k1_swap_on = !env_off("P2PVG_K1_SWAP");
   P2PVG_REQUIRE(driver().encode != nullptr, P2PVG_ERR_UNSUPPORTED, "conv_gemm: cuTensorMapEncodeTiled unavailable");
   P2PVG_REQUIRE(kind >= 0 && kind <= 5, P2PVG_ERR_BAD_ARG, "conv_gemm: bad kind %d", kind);
   if (eval_scale != nullptr) {
@@ -506,7 +497,8 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
     rc = map2d(&tb, b, (long long)taps * Ck, Cn, ldb, BN);
     if (rc) return rc;
     const int nkb = taps * (Ck / 64);
-    g.bres = (BN == 64 && Cn == 64 && Ck == 64 && taps <= 9 && bres_on) ? 1 : 0;
+    // 64 -> 64 channel 3x3 layers: weights resident in shared memory
+    g.bres = (BN == 64 && Cn == 64 && Ck == 64 && taps <= 9) ? 1 : 0;
     if (BN == 128) return launch<0, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
     return launch<0, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
   }
@@ -528,7 +520,7 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   // 64 output channels would fill only half of a 128-row MMA tile: swap the operand roles (M = taps*Cn from the gathered map,
   // N = Cm); the partial sums are then [taps*Cn][Cm] and the split-K reduce kernel writes the transposed result
   const int nkb = (int)((pix + 63) / 64);
-  g.swap = (Cm == 64 && k1_swap_on && nkb >= 16 && ws != nullptr && (size_t)2 * taps * Cn * Cm * sizeof(float) <= ws_bytes) ? 1 : 0;
+  g.swap = (Cm == 64 && nkb >= 16 && ws != nullptr && (size_t)2 * taps * Cn * Cm * sizeof(float) <= ws_bytes) ? 1 : 0;
   if (g.swap) {
     g.M = taps * Cn; g.Ntot = Cm;
     rc = map4d(&ta, b, N, g.st * H, g.st * W, Cn, g.bw64, g.bh64, g.bn64, g.st);

@@ -15,7 +15,6 @@
 //             double-buffered receive slots); the owner sums the 16 partials in a fixed order (deterministic).
 // TF32 mma.sync m16n8k8 with fp32 accumulation, MUFU activations (error <= 2^-11, below the TF32 operand rounding) exactly
 // as in lstm_cluster.cu.
-#include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
@@ -477,15 +476,11 @@ int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
 // is modelled as 1.5 + 2.8*MT (barrier + L2 round trip, then MMA + pointwise per m16 tile): pick the MT with the smallest
 // waves * step time.
 static int fwd_slab_tiles(int B) {
-  static int maxc = 0, forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("P2PVG_LSTM512_MT");
-    forced = e ? atoi(e) : 0;
-    if (forced < 0 || forced > 3) forced = 0;
+  static int maxc = 0;
+  if (maxc == 0) {
     maxc = p2pvg_lstm_cluster512_max_clusters_impl(1);
     if (maxc <= 0) maxc = 7;
   }
-  if (forced) return forced;
   int best = 1;
   float best_cost = 0.f;
   for (int mt = 1; mt <= 3; mt++) {

@@ -219,7 +219,7 @@ class TrainEngineVGG(TrainEngine):
             rec = dict(inp=a, raw=raw, y=y, cout=cout, H=H, pre=pre, cat=(j == 0), k=k, j=j)
             if j == 0:
                 skip = self.venc[self.nst - 1 - k][-1]["y"]  # frames are a prefix -> the first nskip frames
-                addS = self.buf(f"vdec_addS{k}", nskip * B * H * H * cout, self.addend_dtype if self._imp(C, cout) else torch.float32)
+                addS = self.buf(f"vdec_addS{k}", nskip * B * H * H * cout, self.adt if self._imp(C, cout) else torch.float32)
                 self.conv3_fwd(skip, self._packed[f"dec.{k}.0.S.wp"], addS, nskip * B, H, C, cout, bias=P[pre + ".0.bias"])
                 sp = self.stat_buf(f"vdec{k}_{j}", M, 1, cout, B * H * H, kred=9 * C) if self._imp(C, cout) else None
                 self.conv3_fwd(a, self._packed[f"dec.{k}.0.D.wp"], raw, N, H, C, cout, addend=addS, grp_src=self.ix["skip_src"], ipg=B, stat=sp)

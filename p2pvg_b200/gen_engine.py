@@ -22,8 +22,7 @@ the eager path's LSTMs).  The module inputs torch.cat([h, global_z | z, tuc, dt]
 Layer dispatch (bf16 mode): the 4x4/s2 convolutions with >= 64 channels on both sides are implicit GEMMs
 (p2pvg_conv_gemm kinds 0 / 2) with eval-BatchNorm + activation in their epilogue; the thin 1- / 3-channel ends
 (im2col / col2im + GEMM), the 4x4-valid GEMMs (encoder final, decoder first) and all of the fp32 mode use the explicit
-lowering followed by p2pvg_bn_act, as infer.py does (the training engine's default for the thin ends is the same
-im2col + tensor-core GEMM lowering; its direct thin kernels are opt-in there because they are slower).
+lowering followed by p2pvg_bn_act, as infer.py does (the training engine lowers the thin ends the same way).
 
 Memory: every cached signature (at most MAX_GRAPHS, least recently used evicted) owns its buffers; the ground-truth encode
 covers all len(x) frames of the call.  ``GenerateEngine.memory_bytes()`` reports the total, ``clear()`` frees it.

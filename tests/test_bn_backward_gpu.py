@@ -3,8 +3,8 @@
 TrainEngine.bn_backward calls bn_bwd with y = None (the LeakyReLU slope is recomputed from sign(fmaf(x, scale, shift))), with
 scale / shift passed and dx aliasing dy.  Shapes (G groups, R rows, C channels) are the step's: C in {64, 128, 256, 512}, R = B*Ho*Ho
 from 16 to 262144, plus ragged row counts (the last row pair of a chunk has one row) and the widest channel counts the kernels
-accept (one and two row lanes per block).  Also: bit-identity of the call forms, bn_bwd_apply, both tile finalizers, tanh with y
-given, and the one-pass forward statistics on data whose mean is three standard deviations from zero.
+accept (one and two row lanes per block).  Also: bit-identity of the call forms, the forward tile finalizer, tanh with y given,
+and the one-pass forward statistics on data whose mean is three standard deviations from zero.
 """
 import pytest
 import torch
@@ -83,7 +83,7 @@ def check_bwd(res, ref, gamma, dt, name):
 
 
 @pytest.mark.parametrize("dt,G,R,C", PARAMS)
-def test_bn_bwd_as_the_step_calls_it(K, dt, G, R, C):
+def test_bn_bwd_against_float64_in_every_call_form(K, dt, G, R, C):
     torch.manual_seed(R + C)
     raw = (torch.randn(G, R, C, device="cuda") * 1.5 + 0.3).to(dt)
     gamma, beta = torch.rand(C, device="cuda") + 0.5, torch.randn(C, device="cuda") * 0.5
@@ -122,11 +122,6 @@ def test_bn_bwd_as_the_step_calls_it(K, dt, G, R, C):
                       ("y given in place", run(y, True)), ("y given out of place", run(y, False))):
         for k in ("dx", "sdz", "sdzx"):
             assert torch.equal(res[k], step[k]), f"{form}: {k} differs from the in-place y=None form"
-    # the apply pass alone, given the sums bn_bwd produced
-    for yy, ss in ((None, dict(scale=st["scale"], shift=st["shift"])), (y, {})):
-        dx = torch.empty_like(dy)
-        K.bn_bwd_apply(dy, raw, yy, *args, dx, step["sdz"], step["sdzx"], **ss)
-        assert torch.equal(dx, step["dx"]), f"bn_bwd_apply (y {'given' if yy is not None else 'None'}) differs from bn_bwd"
 
 
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float32])
@@ -152,9 +147,9 @@ def test_bn_bwd_tanh_encoder_output(K, dt, G, R):
 
 
 @pytest.mark.parametrize("C,fold,ppg", [(96, 3, 13), (200, 2, 5), (64, 4, 21)])
-def test_finalize_tiles(K, C, fold, ppg):
-    """bn_bwd_finalize_tiles / bn_fwd_finalize_tiles: float64 sums over a group's partial rows and the `fold` column groups of
-    each row (parts_per_group not a multiple of the kernel's 8 part lanes, row pitch wider than fold * C)."""
+def test_fwd_finalize_tiles(K, C, fold, ppg):
+    """bn_fwd_finalize_tiles: float64 sums over a group's partial rows and the `fold` column groups of each row
+    (parts_per_group not a multiple of the kernel's 8 part lanes, row pitch wider than fold * C)."""
     G, rows = 3, 16
     ldp = fold * C + 8
     torch.manual_seed(C + fold)
@@ -166,12 +161,6 @@ def test_finalize_tiles(K, C, fold, ppg):
     part[:, fold * C:] = float("nan")     # padding past fold * C is never read
     p64 = part[:, :fold * C].double().view(G, ppg, fold, C, 2)
     a, b = p64[..., 0].sum((1, 2)), p64[..., 1].sum((1, 2))
-    aa, ab = p64[..., 0].abs().sum((1, 2)), p64[..., 1].sum((1, 2))
-    exact = 2.0 ** -40   # float64 sums of float32 values: only the final cast to float32 (beta) rounds visibly
-    sdz, sdzx = zeros(G * C), zeros(G * C)
-    K.bn_bwd_finalize_tiles(part, ppg, ldp, fold, G, C, sdz, sdzx)
-    assert_within(sdz.view(G, C), a, aa, 0, torch.float32, alpha=exact, name=f"bn_bwd_finalize_tiles C={C} sum 0")
-    assert_within(sdzx.view(G, C), b, ab, 0, torch.float32, alpha=exact, name=f"bn_bwd_finalize_tiles C={C} sum 1")
     gamma, beta = torch.rand(C, device="cuda") + 0.5, torch.randn(C, device="cuda")
     out = [zeros(G * C) for _ in range(5)]
     count = ppg * rows * fold

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""CUDA-event timing of the persistent LSTM scan kernels (P2PVG_LSTM_CLUSTER=0|1 selects the implementation)."""
+"""CUDA-event timing of the persistent LSTM scan kernels: tf32 = 1 runs the thread-block-cluster scans, tf32 = 0 the
+cooperative-grid scans of the exact-fp32 mode."""
 import os
 import sys
 
