@@ -27,7 +27,7 @@ struct Geom {
   int Ck, Cn;           // reduction channels / output channels (kind 0,2);  kind 1: Cm = M extent, Cn = gathered channels
   int M;                // GEMM M: kind 0/2: N*H*W pixels; kind 1: Cm
   int Ntot;             // GEMM N: kind 0/2: Cn; kind 1: 16*Cn
-  int bh128, bn128;     // pixel box of 128 pixels: {W, bh128, bn128}
+  int bhm, bnm;         // pixel box of one M tile (BM = 128 or 256 pixels, kinds 0 / 2): {W, bhm, bnm}
   int bh64, bn64;       // pixel box of 64 pixels (kind 1 K-blocks): {bw64, bh64, bn64}; bw64 = 64 < W for 128-wide maps
   int bw64;
   int imgs_per_group;   // addend indexing
@@ -88,20 +88,22 @@ __device__ __forceinline__ void addend_add32(float (&f)[32], const float4 (&a4)[
 }
 
 // EVAL: eval-mode BatchNorm + activation in the epilogue, y = act(eval_scale[c] * (acc + bias + addend) + eval_shift[c]) (kinds 0 / 2)
-template <int KIND, int BN, bool STAT, bool EVAL = false>
+// BM = 256 (kind 2, BN = 64, no statistics or eval epilogue): 256-pixel tiles, twice the MMA work per filled K block
+template <int KIND, int BM, int BN, bool STAT, bool EVAL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* __restrict__ Cv, int c_bf16,
                  long long ldc, Geom g, int accumulate, const float* __restrict__ bias, const float* __restrict__ addend,
                  const int* __restrict__ grp_src, float* __restrict__ partial, int kb_per_split, int splits,
                  float2* __restrict__ stat_partial, const float* __restrict__ eval_scale, const float* __restrict__ eval_shift, int act) {
-  using C_ = Cfg<BN>;
+  static_assert(BM == 128 || (KIND == 2 && !STAT && !EVAL), "256-row tiles: kind 2 without statistics or eval epilogue");
+  using C_ = Cfg<BN, BM>;
   constexpr bool A_MN = (KIND == 1), B_MN = (KIND != 0);
   extern __shared__ uint8_t smem_raw[];
-  const Smem sm = smem_setup<BN>(smem_raw);
+  const Smem sm = smem_setup<BN, BM>(smem_raw);
   const bool bres = (KIND == 0) && (BN == 64) && g.bres != 0;   // resident weights (tc_common.cuh BRES_*)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_m = (g.M + BLOCK_M - 1) / BLOCK_M, tiles_n = (g.Ntot + BN - 1) / BN;
+  const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.Ntot + BN - 1) / BN;
   const int tiles_mn = tiles_m * tiles_n;
   const int phases = (KIND == 2) ? 4 : 1;
   const int num_tiles = tiles_mn * splits * phases;
@@ -130,7 +132,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int n0 = nt * BN;
         const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
         int pn0 = 0, py0 = 0;
-        if (KIND != 1) pix_block(mt, 128, g.H, g.W, g.bh128, g.bn128, pn0, py0);
+        if (KIND != 1) pix_block(mt, BM, g.H, g.W, g.bhm, g.bnm, pn0, py0);
         const int pa = ph >> 1, pb_ = ph & 1;
         // kind 1: everything that does not depend on the K-block is computed once per tile, the pixel-box coordinates
         // advance incrementally -- the single producer thread must not spend its K-block budget on integer divisions
@@ -160,7 +162,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (g.swap) {   // the gathered map is the A operand: (tap, channel) of the two 64-row halves of the M tile
 #pragma unroll
             for (int q = 0; q < 2; q++) {
-              const int mb = mt * BLOCK_M + 64 * q;
+              const int mb = mt * BM + 64 * q;
               int tap = mb / g.Cn;
               if (tap >= g.ks * g.ks) tap = g.ks * g.ks - 1;   // rows past M are discarded by the epilogue: any in-bounds tap will do
               const int kh = tap / g.ks;
@@ -176,7 +178,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const uint32_t par = (bres ? (it / BRES_STAGES) : (it / C_::STAGES)) & 1;
           mbar_wait(&sm.empty_bar[s], par ^ 1);
           uint8_t* sa = bres ? sm.ring + BRES_B_BYTES + s * A_STAGE_BYTES : sm.ring + s * C_::STAGE_BYTES;
-          uint8_t* sb = sa + A_STAGE_BYTES;
+          uint8_t* sb = sa + C_::A_STAGE_BYTES;
           mbar_expect_tx(&sm.full_bar[s], bres ? A_STAGE_BYTES : C_::STAGE_BYTES);
           if (KIND == 0) {
             // (kh, kw, channel chunk) advance incrementally (kinds 0 / 2 never split K: kb starts at 0)
@@ -195,7 +197,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int q = 0; q < BN / 64; q++)
               tma_load_2d(&tmB, &sm.full_bar[s], sb + q * 64 * 128, (ky * 4 + kx) * g.Cn + n0 + 64 * q, c0);
           } else {
-            const int m0 = mt * BLOCK_M;
+            const int m0 = mt * BM;
             if (g.swap) {
               tma_load_4d(&tmA, &sm.full_bar[s], sa, mc0[0], g.st * kx0 + mdx[0], g.st * ky0 + mdy[0], kn0);
               tma_load_4d(&tmA, &sm.full_bar[s], sa + 64 * 128, mc0[1], g.st * kx0 + mdx[1], g.st * ky0 + mdy[1], kn0);
@@ -224,7 +226,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else if (warp >= 4) {
     regs_worker();
-    mma_loop<false, BN, A_MN, B_MN>(sm, num_tiles, tiles_mn, splits, kb_per_split, nkb_total, bres);
+    mma_loop<false, BN, A_MN, B_MN, BM>(sm, num_tiles, tiles_mn, splits, kb_per_split, nkb_total, bres);
   } else {
     // ===================== epilogue =====================
     regs_worker();
@@ -236,11 +238,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     constexpr bool do_stat = STAT;   // a separate instantiation: the statistics cost ~50 registers in this epilogue
     // eval-mode BatchNorm coefficients of the tile's columns, double-buffered by tile parity like bias_s: [parity][scale | shift][BN]
     __shared__ float ev_s[EVAL ? 2 * 2 * BN : 1];
-    // plain bf16 stores of kinds 0 / 2 (no statistics, no eval epilogue, no accumulation, no addend) take the row-cooperative
-    // path.  With an addend the thread-per-row path stays: it requests a row's addend before waiting for the accumulator, and
-    // the row-cooperative loads, issued after it, made the skip-connection layers slower (dcgan_64 dec2 2.18 -> 3.08 ms).
-    const bool row_major_store = !STAT && !EVAL && KIND != 1 && c_bf16 && !accumulate && addend == nullptr;
-    uint32_t lt = 0;
+    // plain bf16 stores of kinds 0 / 2 (no statistics, no eval epilogue, no accumulation; a bf16 addend if any) take the
+    // row-cooperative path
+    const bool row_major_store = !STAT && !EVAL && KIND != 1 && c_bf16 && !accumulate && (addend == nullptr || g.add_bf16);
+    uint32_t lt = 0, lh = 0;   // tiles / staging-buffer hand-overs (BM / 128 per tile) so far
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
       const int ph = (KIND == 2) ? (t & 3) : 0;
       const int t2 = (KIND == 2) ? (t >> 2) : t;
@@ -248,33 +249,35 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int mt = (tiles_n == 1) ? r : r / tiles_n, nt = (tiles_n == 1) ? 0 : r - mt * tiles_n;
       const int n0 = nt * BN;
       const uint32_t acc = lt & 1;   // bias_s / stat_s half of this tile
-      const int rt = q * 32 + lane;  // row within the tile
-      long long out_row = (long long)mt * BLOCK_M + rt;
-      long long add_row = 0;
-      bool row_ok = out_row < g.M;
-      if (KIND == 2) {
-        // tile row -> small-map pixel -> big-map output pixel of this parity phase
-        int pn0, py0;
-        pix_block(mt, 128, g.H, g.W, g.bh128, g.bn128, pn0, py0);
-        const int HW = g.H * g.W;
-        int nn, yy, xx;
-        if (HW >= 128) { nn = 0; yy = rt / g.W; xx = rt - yy * g.W; }
-        else { nn = rt / HW; const int rem = rt - nn * HW; yy = rem / g.W; xx = rem - yy * g.W; }
-        const int n = pn0 + nn, y = py0 + yy;
-        row_ok = (n < g.N) && (y < g.H);
-        const int oy = 2 * y + (ph >> 1), ox = 2 * xx + (ph & 1);
-        out_row = ((long long)n * (2 * g.H) + oy) * (2 * g.W) + ox;
-        if (addend && row_ok) {
-          const int n2 = grp_src[n / g.imgs_per_group] * g.imgs_per_group + (n % g.imgs_per_group);
-          add_row = ((long long)n2 * (2 * g.H) + oy) * (2 * g.W) + ox;
+      int pn0 = 0, py0 = 0;
+      if (KIND == 2) pix_block(mt, BM, g.H, g.W, g.bhm, g.bnm, pn0, py0);
+      // tile row rt -> output row, addend row (through grp_src), whether the row exists
+      auto row_of = [&](int rt, long long& out_row, long long& add_row, bool& row_ok) {
+        out_row = (long long)mt * BM + rt;
+        add_row = 0;
+        row_ok = out_row < g.M;
+        if (KIND == 2) {
+          // tile row -> small-map pixel -> big-map output pixel of this parity phase
+          const int HW = g.H * g.W;
+          int nn, yy, xx;
+          if (HW >= BM) { nn = 0; yy = rt / g.W; xx = rt - yy * g.W; }
+          else { nn = rt / HW; const int rem = rt - nn * HW; yy = rem / g.W; xx = rem - yy * g.W; }
+          const int n = pn0 + nn, y = py0 + yy;
+          row_ok = (n < g.N) && (y < g.H);
+          const int oy = 2 * y + (ph >> 1), ox = 2 * xx + (ph & 1);
+          out_row = ((long long)n * (2 * g.H) + oy) * (2 * g.W) + ox;
+          if (addend && row_ok) {
+            const int n2 = grp_src[n / g.imgs_per_group] * g.imgs_per_group + (n % g.imgs_per_group);
+            add_row = ((long long)n2 * (2 * g.H) + oy) * (2 * g.W) + ox;
+          }
         }
-      }
-      if (KIND == 0 && addend && row_ok) {
-        const int HW = g.H * g.W;
-        const int n = (int)(out_row / HW);
-        const int n2 = grp_src[n / g.imgs_per_group] * g.imgs_per_group + (n % g.imgs_per_group);
-        add_row = (long long)n2 * HW + (out_row - (long long)n * HW);
-      }
+        if (KIND == 0 && addend && row_ok) {
+          const int HW = g.H * g.W;
+          const int n = (int)(out_row / HW);
+          const int n2 = grp_src[n / g.imgs_per_group] * g.imgs_per_group + (n % g.imgs_per_group);
+          add_row = (long long)n2 * HW + (out_row - (long long)n * HW);
+        }
+      };
       if (EVAL) {
         stage_cols<BN>(ev_s + acc * 2 * BN, eval_scale, n0, g.Ntot);
         stage_cols<BN>(ev_s + acc * 2 * BN + BN, eval_shift, n0, g.Ntot);
@@ -284,88 +287,137 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         stage_cols<BN>(bias_s + acc * BN, bias, n0, g.Ntot);
         epi_bar_sync();
       }
-      const bool use_add = (KIND != 1) && addend != nullptr && row_ok;
-      const long long aoff0 = add_row * g.Ntot + n0;   // element offset of this row's first addend column
       const bool abf = g.add_bf16 != 0;
       if (row_major_store) {
         // Row-cooperative bf16 stores: LPR lanes share one output row, 16 B (8 columns) each, so one warp instruction writes
         // RPI whole rows instead of 32 scattered 16-byte pieces of 32 rows.  The row addresses come from the lane that owns
-        // the row.  Same arithmetic per element as below: acc + bias, rounded once to bf16.
-        constexpr int LPR = BN / 8, RPI = 32 / LPR;
+        // the row.  The addend of every row the lane writes in this tile (BN = 64: 8 per 128 rows; BN = 128: 16) is
+        // requested before the accumulator is waited for.  Same arithmetic per element as the thread-per-row path:
+        // (acc + bias) + addend, rounded once to bf16.
+        constexpr int LPR = BN / 8, RPI = 32 / LPR, STEPS = 32 / RPI, HALVES = BM / 128;
         const int sub = lane / LPR, cl = (lane % LPR) * 8;
         const bool col_ok = n0 + cl < g.Ntot;   // Ntot is a multiple of 32: 8-column groups are all in or all out
         bf16* cbase = reinterpret_cast<bf16*>(Cv) + n0 + cl;
-        mbar_wait(sm.acc_full_bar, lt & 1);
+        long long orow_h[HALVES];
+        bool ok_h[HALVES];
+        uint4 av[HALVES * STEPS];   // 8 bf16 addend values per step
 #pragma unroll
-        for (int i = 0; i < 32 / RPI; i++) {
-          const int src = i * RPI + sub;   // the warp row this lane writes in step i
-          const long long orow = __shfl_sync(0xffffffffu, out_row, src);
-          const bool ok = __shfl_sync(0xffffffffu, (int)row_ok, src) != 0;
-          const float* s = sm.accs + (q * 32 + src) * C_::ACC_LD + cl;
-          const float4 x0 = *reinterpret_cast<const float4*>(s), x1 = *reinterpret_cast<const float4*>(s + 4);
-          if (i == 32 / RPI - 1) {   // the warp's last staging read of this tile
-            __syncwarp();
-            if (lane == 0) mbar_arrive(sm.acc_empty_bar);
-          }
-          if (!ok || !col_ok) continue;
-          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-          if (bias) {
+        for (int hf = 0; hf < HALVES; hf++) {
+          long long arow_h;
+          row_of(hf * 128 + q * 32 + lane, orow_h[hf], arow_h, ok_h[hf]);
+          if (addend != nullptr) {
+            const bf16* abase = reinterpret_cast<const bf16*>(addend) + n0 + cl;
 #pragma unroll
-            for (int j = 0; j < 8; j++) f[j] += bias_s[acc * BN + cl + j];
+            for (int i = 0; i < STEPS; i++) {
+              const int src = i * RPI + sub;
+              const long long arow = __shfl_sync(0xffffffffu, arow_h, src);
+              const bool aok = __shfl_sync(0xffffffffu, (int)ok_h[hf], src) != 0;
+              av[hf * STEPS + i] = (aok && col_ok) ? *reinterpret_cast<const uint4*>(abase + arow * g.Ntot) : make_uint4(0, 0, 0, 0);
+            }
           }
-          *reinterpret_cast<uint4*>(cbase + orow * ldc) = pack16<bf16>(f);
+        }
+        // the staging reads of CH steps are taken before their stores, which wait for the addend: the warp releases the
+        // staging buffer (the MMA warpgroup's second half of a 256-row tile waits for it) without waiting for the addend
+        constexpr int CH = STEPS < 8 ? STEPS : 8;
+#pragma unroll
+        for (int hf = 0; hf < HALVES; hf++, lh++) {
+          mbar_wait(sm.acc_full_bar, lh & 1);
+#pragma unroll
+          for (int c0 = 0; c0 < STEPS; c0 += CH) {
+            float4 x[CH][2];
+#pragma unroll
+            for (int k = 0; k < CH; k++) {
+              const float* s = sm.accs + (q * 32 + (c0 + k) * RPI + sub) * C_::ACC_LD + cl;
+              x[k][0] = *reinterpret_cast<const float4*>(s);
+              x[k][1] = *reinterpret_cast<const float4*>(s + 4);
+            }
+            if (c0 + CH == STEPS) {   // the warp's last staging read of this hand-over
+              __syncwarp();
+              if (lane == 0) mbar_arrive(sm.acc_empty_bar);
+            }
+#pragma unroll
+            for (int k = 0; k < CH; k++) {
+              const int i = c0 + k, src = i * RPI + sub;   // the warp row this lane writes in step i
+              const long long orow = __shfl_sync(0xffffffffu, orow_h[hf], src);
+              const bool ok = __shfl_sync(0xffffffffu, (int)ok_h[hf], src) != 0;
+              if (!ok || !col_ok) continue;
+              const float4 x0 = x[k][0], x1 = x[k][1];
+              float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+              if (bias) {
+#pragma unroll
+                for (int j = 0; j < 8; j++) f[j] += bias_s[acc * BN + cl + j];
+              }
+              if (addend != nullptr) {
+                float a[8];
+                unpack16<bf16>(av[hf * STEPS + i], a);
+#pragma unroll
+                for (int j = 0; j < 8; j++) f[j] += a[j];
+              }
+              *reinterpret_cast<uint4*>(cbase + orow * ldc) = pack16<bf16>(f);
+            }
+          }
         }
         continue;
       }
-      float4 a4[16];  // addend of the next 64 columns, requested before the accumulator is waited for
-      if (use_add) addend_load64(a4, addend, aoff0, abf);
-      mbar_wait(sm.acc_full_bar, lt & 1);
+      // thread-per-row path: one tile row per thread, BM / 128 hand-overs of the staging buffer per tile
 #pragma unroll 1
-      for (int pr = 0; pr < BN / 64; pr++) {
-        if (pr > 0 && use_add) addend_load64(a4, addend, aoff0 + pr * 64, abf);
+      for (int hf = 0; hf < BM / 128; hf++, lh++) {
+        const int rs = q * 32 + lane;  // staging-buffer row
+        long long out_row, add_row;
+        bool row_ok;
+        row_of(hf * 128 + rs, out_row, add_row, row_ok);
+        const bool use_add = (KIND != 1) && addend != nullptr && row_ok;
+        const long long aoff0 = add_row * g.Ntot + n0;   // element offset of this row's first addend column
+        float4 a4[16];  // addend of the next 64 columns, requested before the accumulator is waited for
+        if (use_add) addend_load64(a4, addend, aoff0, abf);
+        mbar_wait(sm.acc_full_bar, lh & 1);
+#pragma unroll 1
+        for (int pr = 0; pr < BN / 64; pr++) {
+          if (pr > 0 && use_add) addend_load64(a4, addend, aoff0 + pr * 64, abf);
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int c = pr * 2 + h;
-          float f[32];
-          read_chunk<BN>(sm, rt, c, f);
-          const int nbase = n0 + c * 32;
-          if (nbase >= g.Ntot) continue;             // warp-uniform
-          if (!row_ok && !do_stat) continue;         // rows past the end only matter as zeros of the column sums
-          if (KIND == 1 && partial != nullptr) {
-            float* dst = partial + ((long long)z * g.M + out_row) * g.Ntot + nbase;
+          for (int h = 0; h < 2; h++) {
+            const int c = pr * 2 + h;
+            float f[32];
+            read_chunk<BN>(sm, rs, c, f);
+            const int nbase = n0 + c * 32;
+            if (nbase >= g.Ntot) continue;             // warp-uniform
+            if (!row_ok && !do_stat) continue;         // rows past the end only matter as zeros of the column sums
+            if (KIND == 1 && partial != nullptr) {
+              float* dst = partial + ((long long)z * g.M + out_row) * g.Ntot + nbase;
 #pragma unroll
-            for (int j = 0; j < 32; j += 8)   // partial workspace rows are 32-byte aligned (Ntot and nbase are multiples of 32)
-              st_global_256(dst + j, __float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
-                            __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7]));
-            continue;
-          }
-          if (bias) add_staged32(f, bias_s + acc * BN + c * 32);
-          if (use_add) addend_add32(f, a4, h, abf);
-          if (EVAL) {
-            const float* sc = ev_s + acc * 2 * BN + c * 32;
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              float y = fmaf(f[j], sc[j], sc[BN + j]);
-              if (act == P2PVG_ACT_LRELU) y = y > 0.f ? y : 0.2f * y;
-              else if (act == P2PVG_ACT_TANH) y = tanhf(y);
-              f[j] = y;
+              for (int j = 0; j < 32; j += 8)   // partial workspace rows are 32-byte aligned (Ntot and nbase are multiples of 32)
+                st_global_256(dst + j, __float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
+                              __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7]));
+              continue;
             }
-          }
-          if (STAT) {
-            // statistics of the tensor AS STORED (bf16-rounded when the output is bf16); all 32 lanes take part
-            float s1[32], s2[32];
+            if (bias) add_staged32(f, bias_s + acc * BN + c * 32);
+            if (use_add) addend_add32(f, a4, h, abf);
+            if (EVAL) {
+              const float* sc = ev_s + acc * 2 * BN + c * 32;
 #pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const float r = row_ok ? (c_bf16 ? bf16_round(f[j]) : f[j]) : 0.f;
-              s1[j] = r;
-              s2[j] = r * r;
+              for (int j = 0; j < 32; j++) {
+                float y = fmaf(f[j], sc[j], sc[BN + j]);
+                if (act == P2PVG_ACT_LRELU) y = y > 0.f ? y : 0.2f * y;
+                else if (act == P2PVG_ACT_TANH) y = tanhf(y);
+                f[j] = y;
+              }
             }
-            const float cs = warp_colsum32(s1, lane), cq = warp_colsum32(s2, lane);
-            stat_s[(acc * 4 + q) * BN + c * 32 + lane] = make_float2(cs, cq);
-            if (!row_ok) continue;
+            if (STAT) {
+              // statistics of the tensor AS STORED (bf16-rounded when the output is bf16); all 32 lanes take part
+              float s1[32], s2[32];
+#pragma unroll
+              for (int j = 0; j < 32; j++) {
+                const float r = row_ok ? (c_bf16 ? bf16_round(f[j]) : f[j]) : 0.f;
+                s1[j] = r;
+                s2[j] = r * r;
+              }
+              const float cs = warp_colsum32(s1, lane), cq = warp_colsum32(s2, lane);
+              stat_s[(acc * 4 + q) * BN + c * 32 + lane] = make_float2(cs, cq);
+              if (!row_ok) continue;
+            }
+            if (c_bf16) store_row32<bf16, false>(reinterpret_cast<bf16*>(Cv) + out_row * ldc + nbase, f, accumulate, 32);
+            else store_row32<float, false>(reinterpret_cast<float*>(Cv) + out_row * ldc + nbase, f, accumulate, 32);
           }
-          if (c_bf16) store_row32<bf16, false>(reinterpret_cast<bf16*>(Cv) + out_row * ldc + nbase, f, accumulate, 32);
-          else store_row32<float, false>(reinterpret_cast<float*>(Cv) + out_row * ldc + nbase, f, accumulate, 32);
         }
       }
       if (STAT) {
@@ -419,23 +471,26 @@ struct EvalEpi {
   int act = 0;
 };
 
-template <int KIND, int BN, bool STAT, bool EVAL>
+template <int KIND, int BM, int BN, bool STAT, bool EVAL>
 int launch_t(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, int accumulate,
              const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
              float2* stat_partial, const EvalEpi& ev) {
-  const long long tiles = (long long)cdiv(g.M, BLOCK_M) * cdiv(g.Ntot, BN) * splits * (KIND == 2 ? 4 : 1);
-  return launch_persistent<conv_gemm_kernel<KIND, BN, STAT, EVAL>, BN>(tiles, st, "conv_gemm", ta, tb, C, (int)(c_dtype == P2PVG_BF16), ldc, g,
-                                                                       accumulate, bias, addend, grp_src, partial, kb_per_split, splits,
-                                                                       stat_partial, ev.scale, ev.shift, ev.act);
+  const long long tiles = (long long)cdiv(g.M, BM) * cdiv(g.Ntot, BN) * splits * (KIND == 2 ? 4 : 1);
+  return launch_persistent<conv_gemm_kernel<KIND, BM, BN, STAT, EVAL>, BN, BM>(tiles, st, "conv_gemm", ta, tb, C, (int)(c_dtype == P2PVG_BF16),
+                                                                               ldc, g, accumulate, bias, addend, grp_src, partial, kb_per_split,
+                                                                               splits, stat_partial, ev.scale, ev.shift, ev.act);
 }
 
-template <int KIND, int BN>
+// BM = 256 tiles have no statistics or eval-epilogue instances (the caller does not choose them for such launches)
+template <int KIND, int BN, int BM = BLOCK_M>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, long long ldc, const Geom& g, int accumulate,
            const float* bias, const float* addend, const int* grp_src, float* partial, int splits, int kb_per_split, cudaStream_t st,
            float2* stat_partial = nullptr, const EvalEpi& ev = EvalEpi()) {
-  if (KIND != 1 && ev.scale != nullptr) return launch_t<KIND, BN, false, (KIND != 1)>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
-  if (KIND != 1 && stat_partial != nullptr) return launch_t<KIND, BN, (KIND != 1), false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, stat_partial, ev);
-  return launch_t<KIND, BN, false, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
+  if constexpr (KIND != 1 && BM == 128) {
+    if (ev.scale != nullptr) return launch_t<KIND, BM, BN, false, true>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
+    if (stat_partial != nullptr) return launch_t<KIND, BM, BN, true, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, stat_partial, ev);
+  }
+  return launch_t<KIND, BM, BN, false, false>(ta, tb, C, c_dtype, ldc, g, accumulate, bias, addend, grp_src, partial, splits, kb_per_split, st, nullptr, ev);
 }
 
 }  // namespace
@@ -469,14 +524,14 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   if (kind == 3 || kind == 5) kind = 0;
   if (kind == 4) kind = 1;
   // kinds 0 / 2 tile the output in 128-pixel boxes, kind 1 reduces over 64-pixel boxes
-  g.bh128 = g.bn128 = g.bh64 = g.bn64 = 1;
+  g.bhm = g.bnm = g.bh64 = g.bn64 = 1;
   g.bw64 = W;
   bool ok;
   if (kind == 1) {
     if (W > 64 && W % 64 == 0 && W * g.st <= 256) { g.bw64 = 64; ok = true; }
     else ok = box_for(64, H, W, g.bh64, g.bn64);
   } else {
-    ok = box_for(128, H, W, g.bh128, g.bn128);
+    ok = box_for(128, H, W, g.bhm, g.bnm);
   }
   ok = ok && (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) == 0;
   if (kind == 1) ok = ok && (Cn % 64 == 0) && (Cm % 8 == 0);
@@ -491,7 +546,7 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   const long long pix = (long long)N * H * W;
   if (kind == 0) {
     g.M = (int)pix; g.Ntot = Cn;
-    rc = map4d(&ta, a, N, g.st * H, g.st * W, Ck, W, g.bh128, g.bn128, g.st);
+    rc = map4d(&ta, a, N, g.st * H, g.st * W, Ck, W, g.bhm, g.bnm, g.st);
     if (rc) return rc;
     const int BN = Cn > 64 ? 128 : 64;
     rc = map2d(&tb, b, (long long)taps * Ck, Cn, ldb, BN);
@@ -504,12 +559,19 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   }
   if (kind == 2) {
     g.M = (int)pix; g.Ntot = Cn;
-    rc = map4d(&ta, a, N, H, W, Ck, W, g.bh128, g.bn128, 1);
+    // 64 output channels: 256-pixel tiles, so that a filled K block (32 KB of pixels + 8 KB of weights) feeds twice the
+    // MMA work of a 128 x 64 one (51 instead of 43 FLOP per filled byte).  Launches with fused statistics (partials are
+    // laid out per 128-row tile) or the eval-BatchNorm epilogue keep 128 rows, as does a map that 256-pixel boxes do not tile.
+    int bh256 = 1, bn256 = 1;
+    const bool tall = Cn == 64 && stat_partial == nullptr && eval_scale == nullptr && box_for(256, H, W, bh256, bn256);
+    if (tall) { g.bhm = bh256; g.bnm = bn256; }
+    rc = map4d(&ta, a, N, H, W, Ck, W, g.bhm, g.bnm, 1);
     if (rc) return rc;
     rc = map2d(&tb, b, 16LL * Cn, Ck, ldb, 64);  // MN-major weight [Ck rows][16*Cn]
     if (rc) return rc;
     const int nkb = 4 * (Ck / 64);
     const int BN = Cn > 64 ? 128 : 64;
+    if (tall) return launch<2, 64, 256>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st);
     if (BN == 128) return launch<2, 128>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
     return launch<2, 64>(ta, tb, c, c_dtype, ldc, g, accumulate, bias, addend, grp_src, nullptr, 1, nkb, st, stat_partial, ev);
   }

@@ -66,6 +66,16 @@ __device__ __forceinline__ void wgmma_bf16_n128(float* d, uint64_t desc_a, uint6
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
+// D[64 x 256] (+)= A[64 x 16] . B[16 x 256]; 128 fp32 accumulators per thread
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n256(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
+}
 __device__ __forceinline__ void wgmma_tf32_n64(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
@@ -112,43 +122,72 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_b
   return d;
 }
 
-// One 128-byte K block of a 128 x BN tile: for every MMA-K slice, one wgmma per 64-row half.  da / db describe k-slice 0 of
-// the stage; the row halves of A are 8 KB apart in both majors (K-major: 64 rows of 128 B; MN-major: the second 64-wide m
-// chunk).  first: the first K block of the tile (overwrites the accumulator).
-template <bool TF32, int BN, bool A_MN, bool B_MN>
-__device__ __forceinline__ void wgmma_kblock(float (&acc)[2][BN / 2], uint64_t da, uint64_t db, bool first) {
+// One 128-byte K block of a BM x BN tile.  128 rows: for every MMA-K slice, one wgmma per 64-row half; the row halves of A
+// are 8 KB apart in both majors (K-major: 64 rows of 128 B; MN-major: the second 64-wide m chunk).  256 x 64 (bf16,
+// K-major A, MN-major B): the transposed product D^T[64 x 256] = B^T . A^T, one m64n256k16 per MMA-K slice with the B
+// tile as the (M-major) A operand and the A tile as the (K-major) B operand.  Four m64n64k16 would read 16 KB of shared
+// memory per k-slice where the one m64n256k16 reads 10 KB.  da / db describe k-slice 0 of the stage.  first: the first K
+// block of the tile (overwrites the accumulator).
+template <bool TF32, int BN, bool A_MN, bool B_MN, int BM>
+__device__ __forceinline__ void wgmma_kblock(float (&acc)[BM / 64][BN / 2], uint64_t da, uint64_t db, bool first) {
   constexpr int UMMA_K = TF32 ? 8 : 16;
   constexpr int KSTEPS = 4;   // 128 B of K: 4 x k8 (tf32) or 4 x k16 (bf16)
   constexpr uint32_t A_STEP = (A_MN ? UMMA_K * 128 : 32) >> 4, B_STEP = (B_MN ? UMMA_K * 128 : 32) >> 4;
+  if constexpr (BM == 256) {
+    static_assert(!TF32 && BN == 64 && !A_MN && B_MN, "256-row tiles: bf16, K-major A, MN-major B, 64 columns");
 #pragma unroll
-  for (int k = 0; k < KSTEPS; k++) {
-    const uint32_t sc = (first && k == 0) ? 0u : 1u;
+    for (int k = 0; k < KSTEPS; k++)
+      wgmma_bf16_n256<1, 0>(&acc[0][0], db + (uint64_t)(k * B_STEP), da + (uint64_t)(k * A_STEP), (first && k == 0) ? 0u : 1u);
+  } else {
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const uint64_t a = da + (uint64_t)(h * (8192 >> 4) + k * A_STEP), b = db + (uint64_t)(k * B_STEP);
-      if constexpr (TF32) {
-        if constexpr (BN == 128) wgmma_tf32_n128(acc[h], a, b, sc);
-        else wgmma_tf32_n64(acc[h], a, b, sc);
-      } else {
-        if constexpr (BN == 128) wgmma_bf16_n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], a, b, sc);
-        else wgmma_bf16_n64<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], a, b, sc);
+    for (int k = 0; k < KSTEPS; k++) {
+      const uint32_t sc = (first && k == 0) ? 0u : 1u;
+#pragma unroll
+      for (int h = 0; h < BM / 64; h++) {
+        const uint64_t a = da + (uint64_t)(h * (8192 >> 4) + k * A_STEP), b = db + (uint64_t)(k * B_STEP);
+        if constexpr (TF32) {
+          if constexpr (BN == 128) wgmma_tf32_n128(acc[h], a, b, sc);
+          else wgmma_tf32_n64(acc[h], a, b, sc);
+        } else {
+          if constexpr (BN == 128) wgmma_bf16_n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], a, b, sc);
+          else wgmma_bf16_n64<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], a, b, sc);
+        }
       }
     }
   }
 }
 
-// The MMA warpgroup's 128 x BN accumulator (wgmma fragment layout) -> row-major fp32 staging buffer (row pitch ld floats)
-// from which the epilogue warps read one tile row per thread.  t: thread index within the warpgroup.
-template <int BN>
-__device__ __forceinline__ void acc_to_smem(const float (&acc)[2][BN / 2], float* buf, int ld, int t) {
+// Rows [128 hf, 128 hf + 128) of the MMA warpgroup's BM x BN accumulator (wgmma fragment layout) -> the row-major fp32
+// staging buffer of 128 rows (row pitch ld floats) from which the epilogue warps read one tile row per thread.  t: thread
+// index within the warpgroup.
+template <int BN, int BM>
+__device__ __forceinline__ void acc_to_smem(const float (&acc)[BM / 64][BN / 2], int hf, float* buf, int ld, int t) {
   const int w = t >> 5, l = t & 31;
+  if constexpr (BM == 256) {
+    // the transposed 64 x 256 accumulator (wgmma_kblock): fragment element 4 j + 2 i + e holds tile column
+    // 16 w + (l >> 2) + 8 i of tile row 8 j + 2 (l & 3) + e.  Scalar stores; with ld = 68 the 32 lanes of one store hit
+    // 32 different banks.
+    const float* a = &acc[0][0];
+    float* r0 = buf + (2 * (l & 3)) * ld + 16 * w + (l >> 2);
 #pragma unroll
-  for (int h = 0; h < 2; h++) {
-    float* r0 = buf + (64 * h + 16 * w + (l >> 2)) * ld + 2 * (l & 3);
+    for (int j = 0; j < 16; j++) {
+      const int jj = 16 * hf + j;
 #pragma unroll
-    for (int j = 0; j < BN / 8; j++) {
-      *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
-      *reinterpret_cast<float2*>(r0 + 8 * ld + 8 * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+      for (int e = 0; e < 2; e++) {
+        r0[(8 * j + e) * ld] = a[4 * jj + e];
+        r0[(8 * j + e) * ld + 8] = a[4 * jj + 2 + e];
+      }
+    }
+  } else {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      float* r0 = buf + (64 * h + 16 * w + (l >> 2)) * ld + 2 * (l & 3);
+      const float* a = acc[2 * hf + h];
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(a[4 * j], a[4 * j + 1]);
+        *reinterpret_cast<float2*>(r0 + 8 * ld + 8 * j) = make_float2(a[4 * j + 2], a[4 * j + 3]);
+      }
     }
   }
 }
@@ -196,11 +235,15 @@ constexpr int ROW_BYTES = 128;  // one SWIZZLE_128B row: 64 bf16 or 32 fp32 (tf3
 constexpr int A_STAGE_BYTES = BLOCK_M * ROW_BYTES;
 constexpr int NUM_THREADS = 384;
 
-// 128 x 64 / 128 x 128 tiles: one warpgroup holds the whole fp32 accumulator in registers (64 / 128 per thread)
-template <int BN> struct Cfg {
+// BM x BN tiles, BM = 128 (BN = 64 / 128) or 256 (BN = 64): one warpgroup holds the whole fp32 accumulator in registers
+// (BM * BN / 128 per thread, at most 128).  The staging buffer always holds 128 rows: a 256-row tile is handed to the
+// epilogue in two halves, which leaves room for 4 stages of 40 KB (a 256-row buffer would leave 3).
+template <int BN, int BM = BLOCK_M> struct Cfg {
+  static_assert(BM == 128 || (BM == 256 && BN == 64), "tile shapes: 128 x 64, 128 x 128, 256 x 64");
+  static constexpr int A_STAGE_BYTES = BM * ROW_BYTES;
   static constexpr int B_STAGE_BYTES = BN * ROW_BYTES;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN == 128) ? 4 : 7;
+  static constexpr int STAGES = (BM == 256 || BN == 128) ? 4 : 7;
   static constexpr int ACC_LD = BN + 4;   // staging row pitch in floats: the row-per-thread float4 reads are conflict-free
   static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
@@ -218,9 +261,9 @@ struct Smem {
   uint64_t* bres_bar;   // the resident weights have landed (conv only)
 };
 
-template <int BN>
+template <int BN, int BM = BLOCK_M>
 __device__ __forceinline__ Smem smem_setup(uint8_t* smem_raw) {
-  using C_ = Cfg<BN>;
+  using C_ = Cfg<BN, BM>;
   Smem s;
   s.ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   s.accs = reinterpret_cast<float*>(s.ring + C_::STAGES * C_::STAGE_BYTES);
@@ -243,22 +286,24 @@ __device__ __forceinline__ Smem smem_setup(uint8_t* smem_raw) {
   return s;
 }
 
-// The MMA warpgroup: for each tile of this CTA, the K blocks of its split z, then the accumulator into the staging buffer.
+// The MMA warpgroup: for each tile of this CTA, the K blocks of its split z, then the accumulator into the staging buffer,
+// 128 rows at a time (a 256-row tile waits for the epilogue to drain its first half before it stages the second).
 // bres: B is the resident weight tap kb and A streams through the BRES_STAGES ring (gemm_tc passes false).
-template <bool TF32, int BN, bool A_MN, bool B_MN>
+template <bool TF32, int BN, bool A_MN, bool B_MN, int BM = BLOCK_M>
 __device__ __forceinline__ void mma_loop(const Smem& sm, int num_tiles, int tiles_mn, int splits, int kb_per_split, int nkb_total,
                                          bool bres) {
-  using C_ = Cfg<BN>;
+  using C_ = Cfg<BN, BM>;
+  static_assert(BM == 128 || !A_MN, "256-row tiles take a K-major A");
   const int wt = threadIdx.x - 128;
   const uint32_t smem0 = smem_u32(sm.ring);
   // MN-major: the 64-element chunks along m / n are 8 KB apart (MN-major operands are bf16)
   const uint64_t da0 = A_MN ? make_desc(smem0, 64 * 128, 1024) : make_desc(smem0, 0, 1024);
-  const uint64_t db0 = B_MN ? make_desc(smem0 + A_STAGE_BYTES, 64 * 128, 1024) : make_desc(smem0 + A_STAGE_BYTES, 0, 1024);
-  uint32_t it = 0, lt = 0;
+  const uint64_t db0 = B_MN ? make_desc(smem0 + C_::A_STAGE_BYTES, 64 * 128, 1024) : make_desc(smem0 + C_::A_STAGE_BYTES, 0, 1024);
+  uint32_t it = 0, lh = 0;   // lh: staging-buffer hand-overs so far
   if (bres) mbar_wait(sm.bres_bar, 0);   // the resident weights have landed
   const uint64_t da0r = make_desc(smem0 + BRES_B_BYTES, 0, 1024), db0r = make_desc(smem0, 0, 1024);
-  float acc[2][BN / 2];
-  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, lt++) {
+  float acc[BM / 64][BN / 2];
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
     const int z = (splits == 1) ? 0 : t / tiles_mn;   // phases (conv kind 2) never split K
     const int kb0 = z * kb_per_split, kb1 = min(kb0 + kb_per_split, nkb_total);
     int prev = -1;   // stage of the previous K block: released once its MMAs have completed
@@ -272,24 +317,27 @@ __device__ __forceinline__ void mma_loop(const Smem& sm, int num_tiles, int tile
       const uint64_t stage_off = (uint64_t)((uint32_t)s * (uint32_t)(C_::STAGE_BYTES >> 4));
       const uint64_t a_off = bres ? (uint64_t)((uint32_t)s * (uint32_t)(A_STAGE_BYTES >> 4)) : stage_off;
       const uint64_t b_off = bres ? (uint64_t)((uint32_t)kb * (uint32_t)((64 * 128) >> 4)) : stage_off;   // resident: tap kb
-      fence_regs(acc[0]);
-      fence_regs(acc[1]);
+#pragma unroll
+      for (int h = 0; h < BM / 64; h++) fence_regs(acc[h]);
       wgmma_fence();
-      wgmma_kblock<TF32, BN, A_MN, B_MN>(acc, (bres ? da0r : da0) + a_off, (bres ? db0r : db0) + b_off, kb == kb0);
+      wgmma_kblock<TF32, BN, A_MN, B_MN, BM>(acc, (bres ? da0r : da0) + a_off, (bres ? db0r : db0) + b_off, kb == kb0);
       wgmma_commit();
       wgmma_wait<1>();
-      fence_regs(acc[0]);
-      fence_regs(acc[1]);
+#pragma unroll
+      for (int h = 0; h < BM / 64; h++) fence_regs(acc[h]);
       if (prev >= 0) mbar_arrive(&sm.empty_bar[prev]);
       prev = s;
     }
     wgmma_wait<0>();
-    fence_regs(acc[0]);
-    fence_regs(acc[1]);
+#pragma unroll
+    for (int h = 0; h < BM / 64; h++) fence_regs(acc[h]);
     if (prev >= 0) mbar_arrive(&sm.empty_bar[prev]);
-    mbar_wait(sm.acc_empty_bar, (lt & 1) ^ 1);   // the epilogue has drained the previous tile
-    acc_to_smem<BN>(acc, sm.accs, C_::ACC_LD, wt);
-    mbar_arrive(sm.acc_full_bar);
+#pragma unroll
+    for (int hf = 0; hf < BM / 128; hf++, lh++) {
+      mbar_wait(sm.acc_empty_bar, (lh & 1) ^ 1);   // the epilogue has drained the previous hand-over
+      acc_to_smem<BN, BM>(acc, hf, sm.accs, C_::ACC_LD, wt);
+      mbar_arrive(sm.acc_full_bar);
+    }
   }
 }
 
@@ -413,13 +461,14 @@ inline int map2d(CUtensorMap* map, const void* base, long long dim0, long long d
   return P2PVG_OK;
 }
 
-// Launches KERN (a skeleton kernel with BN-wide tiles) on the persistent grid min(tiles, SMs).  The dynamic shared memory limit
-// is raised on the first launch of each kernel instance.
-template <auto KERN, int BN, typename... Args>
+// Launches KERN (a skeleton kernel with BM x BN tiles) on the persistent grid min(tiles, SMs).  The dynamic shared memory
+// limit is raised on the first launch of each kernel instance.
+template <auto KERN, int BN, int BM = BLOCK_M, typename... Args>
 int launch_persistent(long long tiles, cudaStream_t st, const char* what, Args... args) {
+  constexpr int SMEM_BYTES = Cfg<BN, BM>::SMEM_BYTES;
   static bool smem_attr_set = false;
   if (!smem_attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES);
+    const cudaError_t e = cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) {
       p2pvg_set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
       return P2PVG_ERR_CUDA;
@@ -427,7 +476,7 @@ int launch_persistent(long long tiles, cudaStream_t st, const char* what, Args..
     smem_attr_set = true;
   }
   const int sms = driver().sms;
-  KERN<<<(int)(tiles < sms ? tiles : sms), NUM_THREADS, Cfg<BN>::SMEM_BYTES, st>>>(args...);
+  KERN<<<(int)(tiles < sms ? tiles : sms), NUM_THREADS, SMEM_BYTES, st>>>(args...);
   return p2pvg_check_launch(what);
 }
 

@@ -24,16 +24,38 @@ sys.path.insert(0, ROOT)
 
 import bench  # noqa: E402  (CONFIGS, synth_batch, ClockSampler)
 
-A_BYTES = 128 * 128   # one 128-pixel x 64-channel bf16 operand stage
+ROW_BYTES = 128   # one pixel's 64 bf16 channels of an operand stage
 
 
-def operand_bytes(kind, N, H, W, Ck, Cn):
-    """Bytes L2 -> shared memory of the tile walk of a kind-0 / kind-2 launch (4x4 filters): every 128 x BN tile loads a
-    128-pixel box and a BN x 64 weight tile per K block (kind 0: 16 taps x Ck / 64 blocks; kind 2: 4 taps per phase)."""
+def box_fits(P, H, W):
+    """a P-pixel box {W, bh, bn} tiles the H x W maps (conv_gemm.cu box_for)"""
+    HW = H * W
+    if HW >= P:
+        if P % W or H % (P // W):
+            return False
+        bh, bn = P // W, 1
+    else:
+        if P % HW:
+            return False
+        bh, bn = H, P // HW
+    return bh * 2 <= 256 and W * 2 <= 256 and bn <= 256
+
+
+def tile_shape(kind, H, W, Cn, stats):
+    """BM x BN as conv_gemm.cu picks it: 256 x 64 for kind 2 with 64 output channels and no fused statistics, when
+    256-pixel boxes tile the map; 128 x 64 / 128 x 128 otherwise"""
     BN = 128 if Cn > 64 else 64
-    tiles = -(-N * H * W // 128) * -(-Cn // BN) * (4 if kind == 2 else 1)
+    BM = 256 if kind == 2 and Cn == 64 and not stats and box_fits(256, H, W) else 128
+    return BM, BN
+
+
+def operand_bytes(kind, N, H, W, Ck, Cn, stats):
+    """Bytes L2 -> shared memory of the tile walk of a kind-0 / kind-2 launch (4x4 filters): every BM x BN tile loads a
+    BM-pixel box and a BN x 64 weight tile per K block (kind 0: 16 taps x Ck / 64 blocks; kind 2: 4 taps per phase)."""
+    BM, BN = tile_shape(kind, H, W, Cn, stats)
+    tiles = -(-N * H * W // BM) * -(-Cn // BN) * (4 if kind == 2 else 1)
     nkb = (16 if kind == 0 else 4) * (Ck // 64)
-    return tiles * nkb * (A_BYTES + BN * 128)
+    return tiles * nkb * (BM + BN) * ROW_BYTES
 
 
 def gpu_info():
@@ -108,22 +130,26 @@ def main():
         torch.cuda.synchronize()
         t = e0.elapsed_time(e1) / args.reps
         flop = 2.0 * N * H * W * 16 * Ck * Cn
-        by = operand_bytes(kind, N, H, W, Ck, Cn)
-        rows.append(dict(kind=kind, N=N, H=H, Ck=Ck, Cn=Cn, stats=kw.get("stat_partial") is not None, addend=kw.get("addend") is not None,
-                         grp_src=kw.get("grp_src") is not None, tflop=flop / 1e12, ms=t, tflops=flop / (t * 1e-3) / 1e12,
-                         operand_gb=by / 1e9, operand_tbs=by / (t * 1e-3) / 1e12))
+        stats = kw.get("stat_partial") is not None
+        by = operand_bytes(kind, N, H, W, Ck, Cn, stats)
+        BM, BN = tile_shape(kind, H, W, Cn, stats)
+        rows.append(dict(kind=kind, N=N, H=H, Ck=Ck, Cn=Cn, stats=stats, addend=kw.get("addend") is not None,
+                         grp_src=kw.get("grp_src") is not None, tile=f"{BM}x{BN}", tflop=flop / 1e12, ms=t, tflops=flop / (t * 1e-3) / 1e12,
+                         operand_gb=by / 1e9, operand_tbs=by / (t * 1e-3) / 1e12, flop_per_byte=flop / by))
     t1 = time.time()
     clocks = sampler.stop(t0, t1)
     info = gpu_info()
     info["sm_clock_during_replays"] = clocks
     print(f"# {info['name']}, power limit {info['power_limit']}, max SM clock {info['sm_max_clock']}, "
           f"SM clock during the replays {clocks}")
-    print("# operand bytes: L2 -> shared memory of the tile walk (computed); time: CUDA events, mean of %d launches" % args.reps)
-    print(f"{'kind':>4} {'N':>5} {'H':>3} {'Ck':>4} {'Cn':>4} {'epilogue':>13} | {'ms':>7} {'TFLOP/s':>7} {'GB':>6} {'TB/s':>5}")
+    print("# operand bytes: L2 -> shared memory of the tile walk (computed); FLOP/B: FLOP per filled operand byte; "
+          "time: CUDA events, mean of %d launches" % args.reps)
+    print(f"{'kind':>4} {'N':>5} {'H':>3} {'Ck':>4} {'Cn':>4} {'epilogue':>13} {'tile':>7} | {'ms':>7} {'TFLOP/s':>7} {'GB':>6} "
+          f"{'TB/s':>5} {'FLOP/B':>6}")
     for r in rows:
         epi = " ".join(n for n in ("stats", "addend") if r[n])
-        print(f"{r['kind']:>4} {r['N']:>5} {r['H']:>3} {r['Ck']:>4} {r['Cn']:>4} {epi or '-':>13} | "
-              f"{r['ms']:>7.3f} {r['tflops']:>7.0f} {r['operand_gb']:>6.2f} {r['operand_tbs']:>5.2f}")
+        print(f"{r['kind']:>4} {r['N']:>5} {r['H']:>3} {r['Ck']:>4} {r['Cn']:>4} {epi or '-':>13} {r['tile']:>7} | "
+              f"{r['ms']:>7.3f} {r['tflops']:>7.0f} {r['operand_gb']:>6.2f} {r['operand_tbs']:>5.2f} {r['flop_per_byte']:>6.1f}")
     print(f"# sum over {len(rows)} launches: {sum(r['ms'] for r in rows):.3f} ms")
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
