@@ -25,6 +25,8 @@ from collections import OrderedDict
 import numpy as np
 import torch
 
+from .layouts import cast, implicit_shape, nchw_to_nhwc, pack_conv4, pack_convt4, tile_bias, unpack_conv4, unpack_convt4, up8
+
 ACT_NONE, ACT_LRELU, ACT_TANH = 0, 1, 2
 BN_MOMENTUM = 0.1
 # BatchNorm forward statistics come out of the producing GEMM's epilogue only where the tile's MMA time can hide the extra
@@ -288,8 +290,7 @@ class TrainEngine:
         return f"upc{self.n + 1}.0", None
 
     def pack_weights(self, which=("encoder", "decoder")):
-        """fp32 master weights -> GEMM-layout copies in the activation dtype.
-        Conv   W[Cout,Cin,4,4]  -> Wp[Cout,(kh,kw,ci)];   ConvT  W[Cin,Cout,4,4] -> Wp[Cin,(kh,kw,co)]."""
+        """fp32 master weights -> GEMM-layout copies in the activation dtype (layouts.pack_conv4 / pack_convt4)."""
         K = self.K
         if "encoder" in which:
             P = self.arena["encoder"].p
@@ -297,13 +298,13 @@ class TrainEngine:
                 w = P[self.enc_names(l)[0] + ".weight"]
                 co, ci = w.shape[0], w.shape[1]
                 wp = self.buf(f"wp_enc{l}", co * 16 * ci)
-                K.transpose_batched(w, wp, co, ci, 16)   # [co][ci][tap] -> [co][tap][ci]
+                pack_conv4(K, w, wp)
                 self._packed[f"enc{l}"] = wp
                 if self.bd and l == 0 and (16 * ci) % 64 != 0:
                     bd = self.buf("wbd_enc0", 4 * co * 64 * ci)
                     K.blockdiag(wp, bd, co, 16 * ci, 4)
                     b4 = self.fbuf("bias4_enc0", 4 * co)
-                    K.permute4(P[self.enc_names(l)[0] + ".bias"], b4, (4, co, 1, 1), (0, 1, 0, 0))
+                    tile_bias(K, P[self.enc_names(l)[0] + ".bias"], b4, 4)
                     self._packed["enc0.bd"], self._packed["enc0.bias4"] = bd, b4
         if "decoder" in which:
             P = self.arena["decoder"].p
@@ -312,7 +313,7 @@ class TrainEngine:
                 w = P[cn + ".weight"]
                 ci, co = w.shape[0], w.shape[1]
                 wp = self.buf(f"wp_dec{k}", ci * 16 * co)
-                K.transpose_batched(w, wp, ci, co, 16)   # [ci][co][tap] -> [ci][tap][co]
+                pack_convt4(K, w, wp)
                 self._packed[f"dec{k}"] = wp
                 if self.bd and k == self.n - 1 and (16 * co) % 64 != 0:
                     cd = ci // 2
@@ -322,7 +323,7 @@ class TrainEngine:
                         self._packed[f"dec_last.bd{half}"] = bd
                 if k == -1:  # bias of the 1x1 -> 4x4 ConvTranspose, repeated over the 16 taps
                     b16 = self.fbuf("bias16_upc1", 16 * co)
-                    K.permute4(P[cn + ".bias"], b16, (16, co, 1, 1), (0, 1, 0, 0))
+                    tile_bias(K, P[cn + ".bias"], b16, 16)
                     self._packed["dec-1.bias16"] = b16
 
     def pack_lstm_weights(self):
@@ -337,7 +338,7 @@ class TrainEngine:
             R = self.R
             w = P["embed.weight"]
             in_dim = w.shape[1]
-            in_p = (in_dim + 7) // 8 * 8
+            in_p = up8(in_dim)
             # re-pitch [R,in_dim] -> [R,in_p]: columns >= in_dim pick up the first elements of the next row
             # (finite weights); they only ever multiply the zero padding columns of the input, so the product is exact
             wp = self.fbuf(f"{m}_embed_pad", R * in_p)
@@ -366,8 +367,8 @@ class TrainEngine:
             a = self.lbuf("wg_castA", rows * out_dim, torch.bfloat16)
             b = self.lbuf("wg_castB", rows * ldx, torch.bfloat16)
             if not reuse_dy:
-                K.permute4(dY, a, (rows * out_dim, 1, 1, 1), (1, 0, 0, 0))
-            K.permute4(X, b, (rows * ldx, 1, 1, 1), (1, 0, 0, 0))
+                cast(K, dY, a, rows * out_dim)
+            cast(K, X, b, rows * ldx)
             K.gemm(a, b, gW, out_dim, in_dim, rows, a_mn=True, b_mn=True, lda=out_dim, ldb=ldx)
         else:
             K.gemm(dY, X, gW, out_dim, in_dim, rows, a_mn=True, b_mn=True, lda=out_dim, ldb=ldx)
@@ -602,7 +603,7 @@ class TrainEngine:
             self.x_nhwc = self.fbuf("x_nhwc", N * hw * nc)
             dual = xs.dtype == torch.float32 and nc in (2, 3, 4) and hw % 4 == 0 and xs.is_cuda
             if not dual:
-                K.permute4(xs, self.x_nhwc, (N, hw, nc, 1), (nc * hw, 1, hw, 0))
+                nchw_to_nhwc(K, xs, self.x_nhwc, N, hw, nc)
         if self.adt == torch.float32:
             a = self.x_nhwc
             if dual:
@@ -612,7 +613,7 @@ class TrainEngine:
             if dual:  # one read of the frames, both copies
                 K.nchw_to_nhwc_dual(xs, self.x_nhwc, a, N, hw, nc)
             else:
-                K.permute4(xs, a, (N, hw, nc, 1), (nc * hw, 1, hw, 0))
+                nchw_to_nhwc(K, xs, a, N, hw, nc)
         return a
 
     # -- Phase E ----------------------------------------------------------------------------
@@ -632,7 +633,7 @@ class TrainEngine:
             raw = self.buf(f"enc_raw{l}", M * cout)
             y = self.buf(f"enc_y{l}", M * cout)
             cn, bn = self.enc_names(l)
-            imp = self.implicit and cin % 64 == 0 and cout % 64 == 0
+            imp = self.implicit and implicit_shape(cin, cout)
             col = sp = None
             if imp:
                 sp = self.stat_buf(f"enc{l}", M, 1, cout, B * Ho * Ho, kred=16 * cin)
@@ -660,7 +661,7 @@ class TrainEngine:
             self.Hlat = y
         else:
             self.Hlat = self.fbuf("Hlat", N * self.g)
-            K.permute4(y, self.Hlat, (N * self.g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, y, self.Hlat, N * self.g)
         # running statistics: one EMA update per reference call, in call order
         ncalls = len(plan.enc_order)
         Bf = self.buffers["encoder"]
@@ -699,7 +700,7 @@ class TrainEngine:
     # -- Phase R ----------------------------------------------------------------------------
     def in_pitch(self, in_dim):
         """Row pitch of the LSTM input matrices: padded to a multiple of 8 floats in tensor-core mode."""
-        return (in_dim + 7) // 8 * 8 if self.tc_lstm else in_dim
+        return up8(in_dim) if self.tc_lstm else in_dim
 
     def lstm_layers(self, m):
         return len({k.split(".")[1] for k in self.arena[m].p if k.startswith("lstm.")})
@@ -781,7 +782,7 @@ class TrainEngine:
         self.Zp = self.fbuf("Zp", n)
         self.kl_sum = self.fbuf("kl_sum", 4)
         K.reparam_kl_fwd(self.mu, self.lv, self.mu_p, self.lv_p, self.eps_post, self.eps_prior, self.Zall, self.Zp, n, self.kl_sum)
-        K.permute4(self.Zp[(S - 1) * B * z:], self.Zall[S * B * z:], (B * z, 1, 1, 1), (1, 0, 0, 0))
+        cast(K, self.Zp[(S - 1) * B * z:], self.Zall[S * B * z:], B * z)
         # frame predictor over S recon steps + the CPC step (models/p2p_model.py:247,252)
         wp = g + z + 2
         Xpred = self.fbuf("Xpred", (S + 1) * B * self.in_pitch(wp))
@@ -803,7 +804,7 @@ class TrainEngine:
             hp = self.h_pred
         else:
             hp = self.buf("hp_act", N * g)
-            K.permute4(self.h_pred, hp, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, self.h_pred, hp, N * g)
         ctop = self.chans[-1]
         cn, bn = self.dec_names(-1)
         raw = self.buf("dec_raw_1", N * 16 * ctop)
@@ -824,7 +825,7 @@ class TrainEngine:
             cn, bn = self.dec_names(k)
             Mo = N * 4 * Hi * Hi
             raw = self.buf(f"dec_raw{k}", Mo * cout)
-            imp = self.implicit and cd % 64 == 0 and cout % 64 == 0
+            imp = self.implicit and implicit_shape(cd, cout)
             sp = rec_fused = None
             if imp:
                 # skip half once per distinct source frame (activation dtype, bias folded in), added in the epilogue of the
@@ -930,7 +931,7 @@ class TrainEngine:
                     if want_wgrad:
                         K.conv_gemm(1, rec["skip"], dyS, gw[cd * 16 * cout:], nskip * B, Hi, Hi, 0, cout, Cm=cd)
                 if want_wgrad:
-                    K.transpose_batched(gw, A.g[cn + ".weight"], 2 * cd, 16, cout)   # [2cd][tap][co] -> [2cd][co][tap]
+                    unpack_convt4(K, gw, A.g[cn + ".weight"])
                 K.conv_gemm(0, dy, wD, dd, N, Hi, Hi, cout, cd)
             else:
                 dcol = self.buf("scratch_dcol", Md * 16 * cout)
@@ -954,7 +955,7 @@ class TrainEngine:
                     if want_wgrad:
                         K.gemm(rec["skip"], dcolS, gw[cd * 16 * cout:], cd, 16 * cout, Ms, a_mn=True, b_mn=True, lda=cd, ldb=16 * cout)
                 if want_wgrad:
-                    K.transpose_batched(gw, A.g[cn + ".weight"], 2 * cd, 16, cout)   # [2cd][tap][co] -> [2cd][co][tap]
+                    unpack_convt4(K, gw, A.g[cn + ".weight"])
             dy = dd
         # upc1: BatchNorm + LeakyReLU, then the g -> 4x4xCtop GEMM
         ctop = self.chans[-1]
@@ -969,14 +970,14 @@ class TrainEngine:
             A.g[cn + ".bias"].zero_()
             gw = self.fbuf("gwp_dec-1", g * 16 * ctop)
             K.gemm(hp, dy, gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-            K.transpose_batched(gw, A.g[cn + ".weight"], g, 16, ctop)
+            unpack_convt4(K, gw, A.g[cn + ".weight"])
         dhp = self.d_hpred[g0 * B * g:g1 * B * g]
         if self.adt == torch.float32:
             K.gemm(dy, self._packed["dec-1"], dhp, N, g, 16 * ctop)
         else:
             tmp = self.buf("dhp_act", N * g)
             K.gemm(dy, self._packed["dec-1"], tmp, N, g, 16 * ctop)
-            K.permute4(tmp, dhp, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, tmp, dhp, N * g)
 
     def bn_backward(self, dy, raw, y, st, c0, c1, G, R, C, act):
         """BatchNorm + activation backward in place (dy -> d raw).  On the CUDA backend the LeakyReLU derivative is
@@ -1124,7 +1125,7 @@ class TrainEngine:
             dy = self.dH
         else:
             dy = self.buf("dH_act", N * g)
-            K.permute4(self.dH, dy, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, self.dH, dy, N * g)
         cn, bn = self.enc_names(n)
         fin = self.enc_final
         st = fin["st"]
@@ -1134,7 +1135,7 @@ class TrainEngine:
         ctop = self.chans[-1]
         gw = self.fbuf(f"gwp_enc{n}", g * 16 * ctop)
         K.gemm(dy, fin["inp"], gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-        K.transpose_batched(gw, A.g[cn + ".weight"], g, 16, ctop)
+        unpack_conv4(K, gw, A.g[cn + ".weight"])
         gy = self.buf(f"enc_gy{n - 1}", N * 16 * ctop)
         K.gemm(dy, self._packed[f"enc{n}"], gy, N, 16 * ctop, g, b_mn=True)
         for l in range(n - 1, -1, -1):
@@ -1155,7 +1156,7 @@ class TrainEngine:
                 K.conv_gemm(1, gy, rec["inp"], gw, N, Ho, Ho, 0, cin, Cm=cout)
             else:
                 K.gemm(gy, rec["col"], gw, cout, 16 * cin, M, a_mn=True, b_mn=True, lda=cout, ldb=16 * cin)
-            K.transpose_batched(gw, A.g[cn + ".weight"], cout, 16, cin)   # [co][tap][ci] -> [co][ci][tap]
+            unpack_conv4(K, gw, A.g[cn + ".weight"])
             if l > 0:
                 gprev = self.buf(f"enc_gy{l - 1}", N * rec["Hin"] * rec["Hin"] * cin)
                 if rec["imp"]:

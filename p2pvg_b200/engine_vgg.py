@@ -18,16 +18,14 @@ from __future__ import annotations
 import torch
 
 from .engine import ACT_LRELU, ACT_TANH, BN_MOMENTUM, TrainEngine
+from .layouts import cast, implicit_shape, pack_conv3, pack_conv3_t, pack_conv4, pack_convt4, tile_bias, unpack_conv3, \
+    unpack_conv4, unpack_convt4, up8
 
 VGG_ENC = [[(None, 64), (64, 64)], [(64, 128), (128, 128)], [(128, 256), (256, 256), (256, 256)], [(256, 512), (512, 512), (512, 512)]]
 VGG_DEC = [[(1024, 512), (512, 512), (512, 256)], [(512, 256), (256, 256), (256, 128)], [(256, 128), (128, 64)], [(128, 64)]]
 # models/vgg_128.py:16-105: one more 512-channel stage on both sides
 VGG_ENC_128 = VGG_ENC + [[(512, 512), (512, 512), (512, 512)]]
 VGG_DEC_128 = [[(1024, 512), (512, 512), (512, 512)]] + VGG_DEC
-
-
-def _up8(n):
-    return (n + 7) // 8 * 8
 
 
 class TrainEngineVGG(TrainEngine):
@@ -38,7 +36,7 @@ class TrainEngineVGG(TrainEngine):
         self.ENC, self.DEC = (VGG_ENC_128, VGG_DEC_128) if self.W0 == 128 else (VGG_ENC, VGG_DEC)
         self.nst = len(self.ENC)                 # stages; the final 4x4 conv is c{nst+1}, the last decoder block upc{nst+1}
         self.top, self.last = f"c{self.nst + 1}", f"upc{self.nst + 1}"
-        self.ldl = _up8(9 * self.nc)  # row pitch of the last layer's [pix, 9*nc] matrix
+        self.ldl = up8(9 * self.nc)  # row pitch of the last layer's [pix, 9*nc] matrix
 
     # ------------------------------------------------------------------ weights
     def enc_layers(self):
@@ -51,22 +49,18 @@ class TrainEngineVGG(TrainEngine):
             for j, (cin, cout) in enumerate(stage):
                 yield k, j, cin, cout, f"upc{k + 2}.{j}.main"
 
-    def _pack_conv3(self, key, w, cin_total, c0, cin, cout, want_t=True):
-        """Wp[cout,(tap,ci)] (row pitch padded to 8 for thin inputs) and Wt[ci,(tap,cout)] of input channels [c0, c0+cin)."""
+    def _pack_conv3(self, key, w, c0, cin, want_t=True):
+        """pack_conv3 and (want_t) pack_conv3_t of input channels [c0, c0+cin); thin inputs are packed via the wp_ scratch."""
         K = self.K
-        src = w.view(-1)[c0 * 9:]
-        ld = _up8(9 * cin)
+        cout = w.shape[0]
+        ld = up8(9 * cin)
         wp = self.buf(f"wp_{key}", cout * 9 * cin + 8)
-        K.permute4(src, wp, (cout, 3, 3, cin), (cin_total * 9, 3, 1, 9))
-        if ld != 9 * cin:
-            # re-pitch [cout, 9cin] -> [cout, ld]; the pad columns pick up finite neighbours and only ever meet zero columns
-            wq = self.buf(f"wq_{key}", cout * ld)
-            K.permute4(wp, wq, (cout, ld, 1, 1), (9 * cin, 1, 0, 0))
-            wp = wq
-        self._packed[key + ".wp"] = wp
+        out = self.buf(f"wq_{key}", cout * ld) if ld != 9 * cin else wp
+        pack_conv3(K, w, out, c0, cin, scratch=wp)
+        self._packed[key + ".wp"] = out
         if want_t:
             wt = self.buf(f"wt_{key}", cin * 9 * cout)
-            K.permute4(src, wt, (cin, 3, 3, cout), (9, 3, 1, cin_total * 9))
+            pack_conv3_t(K, w, wt, c0, cin)
             self._packed[key + ".wt"] = wt
 
     def pack_weights(self, which=("encoder", "decoder")):
@@ -74,49 +68,43 @@ class TrainEngineVGG(TrainEngine):
         if "encoder" in which:
             P = self.arena["encoder"].p
             for i, j, cin, cout, pre in self.enc_layers():
-                self._pack_conv3(f"enc.{i}.{j}", P[pre + ".0.weight"], cin, 0, cin, cout, want_t=not (i == 0 and j == 0))
+                self._pack_conv3(f"enc.{i}.{j}", P[pre + ".0.weight"], 0, cin, want_t=not (i == 0 and j == 0))
             w = P[self.top + ".0.weight"]
             wp = self.buf("wp_enc_c5", self.g * 16 * 512)
-            K.permute4(w, wp, (self.g, 4, 4, 512), (512 * 16, 4, 1, 16))
+            pack_conv4(K, w, wp)
             self._packed["enc.c5"] = wp
         if "decoder" in which:
             P = self.arena["decoder"].p
             w = P["upc1.0.weight"]
             wp = self.buf("wp_dec-1", self.g * 16 * 512)
-            K.permute4(w, wp, (self.g, 4, 4, 512), (512 * 16, 4, 1, 16))
+            pack_convt4(K, w, wp)
             self._packed["dec-1"] = wp
             b16 = self.fbuf("bias16_upc1", 16 * 512)
-            K.permute4(P["upc1.0.bias"], b16, (16, 512, 1, 1), (0, 1, 0, 0))
+            tile_bias(K, P["upc1.0.bias"], b16, 16)
             self._packed["dec-1.bias16"] = b16
             for k, j, cin, cout, pre in self.dec_layers():
                 w = P[pre + ".0.weight"]
                 if j == 0:
                     C = cin // 2
-                    self._pack_conv3(f"dec.{k}.{j}.D", w, cin, 0, C, cout)
-                    self._pack_conv3(f"dec.{k}.{j}.S", w, cin, C, C, cout)
+                    self._pack_conv3(f"dec.{k}.{j}.D", w, 0, C)
+                    self._pack_conv3(f"dec.{k}.{j}.S", w, C, C)
                 else:
-                    self._pack_conv3(f"dec.{k}.{j}", w, cin, 0, cin, cout)
+                    self._pack_conv3(f"dec.{k}.{j}", w, 0, cin)
             # ConvTranspose2d(64, nc, 3, 1, 1): Wl[64, (kh,kw,co)] with the row pitch padded to ldl
-            nc, ldl = self.nc, self.ldl
-            w27 = self.buf("wp_dec_last27", 64 * 9 * nc + 8)
-            K.permute4(P[self.last + ".1.weight"], w27, (64, 3, 3, nc), (nc * 9, 3, 1, 9))
-            wl = self.buf("wp_dec_last", 64 * ldl)
-            K.permute4(w27, wl, (64, ldl, 1, 1), (9 * nc, 1, 0, 0))
+            wl = self.buf("wp_dec_last", 64 * self.ldl)
+            pack_conv3(K, P[self.last + ".1.weight"], wl, scratch=self.buf("wp_dec_last27", 64 * 9 * self.nc + 8))
             self._packed["dec.last"] = wl
 
     # ------------------------------------------------------------------ 3x3 layer primitives
-    def _imp(self, cin, cout):
-        return self.implicit and cin % 64 == 0 and cout % 64 == 0
-
     def conv3_fwd(self, a, wp, out, N, H, cin, cout, bias=None, addend=None, grp_src=None, ipg=0, stat=None):
         """stat: stat_buf() workspace -> the BatchNorm statistics of `out` come from the GEMM epilogue (implicit path only)."""
         K = self.K
-        if self._imp(cin, cout):
+        if self.implicit and implicit_shape(cin, cout):
             K.conv_gemm(3, a, wp, out, N, H, H, cin, cout, bias=bias, addend=addend, grp_src=grp_src, imgs_per_group=ipg,
                         stat_partial=stat["buf"] if stat else None)
             return
         assert stat is None
-        ld = _up8(9 * cin)
+        ld = up8(9 * cin)
         col = self.buf("vgg_col", N * H * H * ld)
         K.im2col3(a, col, N, H, H, cin, ld, 1)
         K.gemm(col, wp, out, N * H * H, cout, ld, bias=bias)
@@ -125,7 +113,7 @@ class TrainEngineVGG(TrainEngine):
 
     def conv3_dgrad(self, dy, wt, out, N, H, cout, cin):
         K = self.K
-        if self._imp(cout, cin):
+        if self.implicit and implicit_shape(cout, cin):
             K.conv_gemm(5, dy, wt, out, N, H, H, cout, cin)
             return
         col = self.buf("vgg_dcol", N * H * H * 9 * cout)
@@ -133,19 +121,15 @@ class TrainEngineVGG(TrainEngine):
         K.gemm(col, wt, out, N * H * H, cin, 9 * cout)
 
     def conv3_wgrad(self, dy, inp, gw, N, H, cout, cin):
-        """gw[cout, (tap, cin)] (row pitch _up8(9 cin), fp32)."""
+        """gw[cout, (tap, cin)] (row pitch up8(9 cin), fp32)."""
         K = self.K
-        if self._imp(cin, cout):
+        if self.implicit and implicit_shape(cin, cout):
             K.conv_gemm(4, dy, inp, gw, N, H, H, 0, cin, Cm=cout)
             return
-        ld = _up8(9 * cin)
+        ld = up8(9 * cin)
         col = self.buf("vgg_col", N * H * H * ld)
         K.im2col3(inp, col, N, H, H, cin, ld, 1)
         K.gemm(dy, col, gw, cout, ld, N * H * H, a_mn=True, b_mn=True, lda=cout, ldb=ld)
-
-    def _store_wgrad(self, gw, gdst, cout, cin):
-        ld = _up8(9 * cin)
-        self.K.permute4(gw, gdst, (cout, cin, 3, 3), (ld, 1, 3 * cin, cin))
 
     # ------------------------------------------------------------------ Phase E
     def encode(self, x, plan):
@@ -163,7 +147,7 @@ class TrainEngineVGG(TrainEngine):
             M = N * H * H
             raw = self.buf(f"venc_raw{i}_{j}", M * cout)
             y = self.buf(f"venc_y{i}_{j}", M * cout)
-            sp = self.stat_buf(f"venc{i}_{j}", M, 1, cout, B * H * H, kred=9 * cin) if self._imp(cin, cout) else None
+            sp = self.stat_buf(f"venc{i}_{j}", M, 1, cout, B * H * H, kred=9 * cin) if self.implicit and implicit_shape(cin, cout) else None
             self.conv3_fwd(a, self._packed[f"enc.{i}.{j}.wp"], raw, N, H, cin, cout, bias=P[pre + ".0.bias"], stat=sp)
             st = self.bn_forward("venc", f"{i}_{j}", raw, y, T, B * H * H, cout, P[pre + ".1.weight"], P[pre + ".1.bias"], ACT_LRELU, tiles=sp)
             self.venc[i].append(dict(inp=a, raw=raw, y=y, st=st, cin=cin, cout=cout, H=H, pre=pre))
@@ -179,7 +163,7 @@ class TrainEngineVGG(TrainEngine):
             self.Hlat = y
         else:
             self.Hlat = self.fbuf("Hlat", N * self.g)
-            K.permute4(y, self.Hlat, (N * self.g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, y, self.Hlat, N * self.g)
         ncalls = len(plan.enc_order)
         Bf = self.buffers["encoder"]
         bns = [(rec["pre"] + ".1", rec["st"]) for recs in self.venc for rec in recs] + [(self.top + ".1", st)]
@@ -197,7 +181,7 @@ class TrainEngineVGG(TrainEngine):
             hp = self.h_pred
         else:
             hp = self.buf("hp_act", N * g)
-            K.permute4(self.h_pred, hp, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, self.h_pred, hp, N * g)
         raw = self.buf("dec_raw_1", N * 16 * 512)
         d = self.buf("dec_d_1", N * 16 * 512)
         K.gemm(hp, self._packed["dec-1"], raw, N, 16 * 512, g, b_mn=True, bias=self._packed["dec-1.bias16"])
@@ -219,13 +203,14 @@ class TrainEngineVGG(TrainEngine):
             rec = dict(inp=a, raw=raw, y=y, cout=cout, H=H, pre=pre, cat=(j == 0), k=k, j=j)
             if j == 0:
                 skip = self.venc[self.nst - 1 - k][-1]["y"]  # frames are a prefix -> the first nskip frames
-                addS = self.buf(f"vdec_addS{k}", nskip * B * H * H * cout, self.adt if self._imp(C, cout) else torch.float32)
+                imp = self.implicit and implicit_shape(C, cout)
+                addS = self.buf(f"vdec_addS{k}", nskip * B * H * H * cout, self.adt if imp else torch.float32)
                 self.conv3_fwd(skip, self._packed[f"dec.{k}.0.S.wp"], addS, nskip * B, H, C, cout, bias=P[pre + ".0.bias"])
-                sp = self.stat_buf(f"vdec{k}_{j}", M, 1, cout, B * H * H, kred=9 * C) if self._imp(C, cout) else None
+                sp = self.stat_buf(f"vdec{k}_{j}", M, 1, cout, B * H * H, kred=9 * C) if imp else None
                 self.conv3_fwd(a, self._packed[f"dec.{k}.0.D.wp"], raw, N, H, C, cout, addend=addS, grp_src=self.ix["skip_src"], ipg=B, stat=sp)
                 rec.update(cin=C, skip=skip)
             else:
-                sp = self.stat_buf(f"vdec{k}_{j}", M, 1, cout, B * H * H, kred=9 * cin) if self._imp(cin, cout) else None
+                sp = self.stat_buf(f"vdec{k}_{j}", M, 1, cout, B * H * H, kred=9 * cin) if self.implicit and implicit_shape(cin, cout) else None
                 self.conv3_fwd(a, self._packed[f"dec.{k}.{j}.wp"], raw, N, H, cin, cout, bias=P[pre + ".0.bias"], stat=sp)
                 rec.update(cin=cin)
             rec["st"] = self.bn_forward("vdec", f"{k}_{j}", raw, y, G, B * H * H, cout, P[pre + ".1.weight"], P[pre + ".1.bias"], ACT_LRELU, tiles=sp)
@@ -268,7 +253,7 @@ class TrainEngineVGG(TrainEngine):
             K.colsum(dy, M, nc, nc, A.g[self.last + ".1.bias"])
             gwl = self.fbuf("gwp_dec_last", 64 * ldl)
             K.gemm(x_in, dcolT, gwl, 64, ldl, M, a_mn=True, b_mn=True, lda=64, ldb=ldl)
-            K.permute4(gwl, A.g[self.last + ".1.weight"], (64, nc, 3, 3), (ldl, 1, 3 * nc, nc))
+            unpack_conv3(K, gwl, A.g[self.last + ".1.weight"])
         dy = dd
         for k in range(self.nst - 1, -1, -1):
             for rec in reversed(self.vdec[k]):
@@ -299,8 +284,8 @@ class TrainEngineVGG(TrainEngine):
                             self.conv3_wgrad(dyS, rec["skip"], gw[cout * 9 * C:], nskip * B, H, cout, C)
                     elif want_wgrad:
                         gw[cout * 9 * C:].zero_()
-                    if want_wgrad:  # W[co, half*C + ci, kh, kw] = gw[half][co][tap][ci]
-                        K.permute4(gw, A.g[pre + ".0.weight"], (cout, 2, C, 9), (9 * C, cout * 9 * C, 1, C))
+                    if want_wgrad:
+                        unpack_conv3(K, gw, A.g[pre + ".0.weight"], halves=2)
                     dd = self.buf(f"vdec_gd{k}", N * (H // 2) * (H // 2) * C)
                     K.upsample2_bwd(dprev, dd, N, H // 2, H // 2, C)
                     dy = dd
@@ -310,7 +295,7 @@ class TrainEngineVGG(TrainEngine):
                     if want_wgrad:
                         gw = self.fbuf(f"gwp_vdec{k}_{j}", cout * 9 * cin)
                         self.conv3_wgrad(dy, x_in, gw, N, H, cout, cin)
-                        self._store_wgrad(gw, A.g[pre + ".0.weight"], cout, cin)
+                        unpack_conv3(K, gw, A.g[pre + ".0.weight"])
                     dy = dprev
         # upc1: BatchNorm + LeakyReLU, then the g -> 4x4x512 GEMM
         ctop = 512
@@ -324,14 +309,14 @@ class TrainEngineVGG(TrainEngine):
             A.g["upc1.0.bias"].zero_()
             gw = self.fbuf("gwp_dec-1", g * 16 * ctop)
             K.gemm(hp, dy, gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-            K.permute4(gw, A.g["upc1.0.weight"], (g, ctop, 4, 4), (16 * ctop, 1, 4 * ctop, ctop))
+            unpack_convt4(K, gw, A.g["upc1.0.weight"])
         dhp = self.d_hpred[g0 * B * g:g1 * B * g]
         if self.adt == torch.float32:
             K.gemm(dy, self._packed["dec-1"], dhp, N, g, 16 * ctop)
         else:
             tmp = self.buf("dhp_act", N * g)
             K.gemm(dy, self._packed["dec-1"], tmp, N, g, 16 * ctop)
-            K.permute4(tmp, dhp, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, tmp, dhp, N * g)
 
     def encoder_backward(self, plan):
         K, T, B, g = self.K, self.T, self.B, self.g
@@ -342,7 +327,7 @@ class TrainEngineVGG(TrainEngine):
             dy = self.dH
         else:
             dy = self.buf("dH_act", N * g)
-            K.permute4(self.dH, dy, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, self.dH, dy, N * g)
         fin = self.enc_final
         st = fin["st"]
         K.bn_bwd(dy, fin["raw"], fin["y"], st["mean"], st["invstd"], st["gamma"], T, B, g, ACT_TANH, dy, st["sdz"], st["sdzx"])
@@ -350,7 +335,7 @@ class TrainEngineVGG(TrainEngine):
         A.g[self.top + ".0.bias"].zero_()
         gw = self.fbuf("gwp_enc_c5", g * 16 * 512)
         K.gemm(dy, fin["inp"], gw, g, 16 * 512, N, a_mn=True, b_mn=True, lda=g, ldb=16 * 512)
-        K.transpose_batched(gw, A.g[self.top + ".0.weight"], g, 16, 512)
+        unpack_conv4(K, gw, A.g[self.top + ".0.weight"])
         gy = self.buf("venc_gpool4", N * 16 * 512)
         K.gemm(dy, self._packed["enc.c5"], gy, N, 16 * 512, g, b_mn=True)
         for i in range(self.nst - 1, -1, -1):
@@ -371,9 +356,9 @@ class TrainEngineVGG(TrainEngine):
                 self.bn_backward(gy, rec["raw"], rec["y"], st, 0, T * cout, T, B * H * H, cout, ACT_LRELU)
                 K.bn_param_grad(st["sdz"], st["sdzx"], T, cout, A.g[pre + ".1.weight"], A.g[pre + ".1.bias"])
                 A.g[pre + ".0.bias"].zero_()
-                gw = self.fbuf(f"gwp_venc{i}_{j}", cout * _up8(9 * cin))
+                gw = self.fbuf(f"gwp_venc{i}_{j}", cout * up8(9 * cin))
                 self.conv3_wgrad(gy, rec["inp"], gw, N, H, cout, cin)
-                self._store_wgrad(gw, A.g[pre + ".0.weight"], cout, cin)
+                unpack_conv3(K, gw, A.g[pre + ".0.weight"])
                 if i > 0 or j > 0:
                     gprev = self.buf(f"venc_g{i}_{j}", N * H * H * cin)
                     self.conv3_dgrad(gy, self._packed[f"enc.{i}.{j}.wt"], gprev, N, H, cout, cin)

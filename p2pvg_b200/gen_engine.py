@@ -39,6 +39,7 @@ import numpy as np
 import torch
 
 from ._lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH
+from .layouts import cast, implicit_shape, nchw_to_nhwc, nhwc_to_nchw, pack_conv4, pack_convt4, tile_bias
 
 MAX_GRAPHS = 4
 
@@ -248,7 +249,7 @@ class GenerateEngine:
         N = T * B
         hw, nc, W = c["W"] * c["W"], c["C"], c["W"]
         a = self._buf(G, "gt_in", N * hw * nc, adt)
-        K.permute4(G.bufs["x"], a, (N, hw, nc, 1), (nc * hw, 1, hw, 0))
+        nchw_to_nhwc(K, G.bufs["x"], a, N, hw, nc)
         h_gt = self._buf(G, "gt_h", N * g)
         gt_skips = self._encode("gt", a, N, h_gt)
         Hsrc = self._buf(G, "Hsrc", (T + 1) * rows * g)     # [T + 1][rows][g]: ground truth frames, then this step's h
@@ -273,7 +274,7 @@ class GenerateEngine:
             skips_cur = None
             if s > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
                 xin = self._buf(G, "step_in", rows * hw * nc, adt)
-                K.permute4(prev_frame, xin, (rows, hw, nc, 1), (nc * hw, 1, hw, 0))
+                nchw_to_nhwc(K, prev_frame, xin, rows, hw, nc)
                 skips_cur = self._encode("step", xin, rows, h_cur)
             glob = ti[3 * S:3 * S + 1]
             # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
@@ -310,16 +311,16 @@ class GenerateEngine:
             conv, bn = (blk.main[0], blk.main[1]) if l < n else (blk[0], blk[1])
             cout = conv.weight.shape[0]
             wp = self._buf(G, f"wp_enc{l}", cout * 16 * cin, adt)
-            K.permute4(conv.weight.data, wp, (cout, 4, 4, cin), (cin * 16, 4, 1, 16))
+            pack_conv4(K, conv.weight.data, wp)
             self.wp[f"enc{l}"] = wp
             coeffs(f"enc{l}", bn)
             cin = cout
         ctop = chans[-1]
         convt, bn = dec.upc1[0], dec.upc1[1]
         wp = self._buf(G, "wp_dec-1", g * 16 * ctop, adt)
-        K.permute4(convt.weight.data, wp, (g, 4, 4, ctop), (ctop * 16, 4, 1, 16))
+        pack_convt4(K, convt.weight.data, wp)
         b16 = self._buf(G, "bias16_dec-1", 16 * ctop)
-        K.permute4(convt.bias.data, b16, (16, ctop, 1, 1), (0, 1, 0, 0))
+        tile_bias(K, convt.bias.data, b16, 16)
         self.wp["dec-1"], self.wp["dec-1.bias16"] = wp, b16
         coeffs("dec-1", bn)
         for k in range(n):
@@ -328,15 +329,12 @@ class GenerateEngine:
             convt = blk[0] if last else blk.main[0]
             ci2, cout = convt.weight.shape[0], convt.weight.shape[1]
             wp = self._buf(G, f"wp_dec{k}", ci2 * 16 * cout, adt)
-            K.permute4(convt.weight.data, wp, (ci2, 4, 4, cout), (cout * 16, 4, 1, 16))
+            pack_convt4(K, convt.weight.data, wp)
             self.wp[f"dec{k}"] = wp
             if not last:
                 coeffs(f"dec{k}", blk.main[1])
 
     # ------------------------------------------------------------------ encoder / decoder
-    def _implicit(self, cin, cout):
-        return self.G.cfg["adt"] == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0
-
     def _encode(self, tag, a, N, h_out):
         """a: NHWC frames [N, W, W, nc] in the activation dtype -> h_out fp32 [N, g]; returns the skip maps (NHWC)."""
         K, G, model = self.K, self.G, self.model
@@ -350,7 +348,7 @@ class GenerateEngine:
             M = N * Ho * Ho
             sc, sh = self.bn[f"enc{l}"]
             y = self._buf(G, f"{tag}_enc_y{l}", M * cout, adt)
-            if self._implicit(cin, cout):
+            if adt == torch.bfloat16 and implicit_shape(cin, cout):
                 K.conv_gemm(0, a, self.wp[f"enc{l}"], y, N, Ho, Ho, cin, cout, bias=conv.bias.data, eval_scale=sc, eval_shift=sh,
                             act=ACT_LRELU)
             else:
@@ -369,7 +367,7 @@ class GenerateEngine:
         K.gemm(a, self.wp[f"enc{len(self.chans)}"], raw, N, g, 16 * cin, bias=conv.bias.data)
         K.bn_act(raw, y, sc, sh, 1, N, g, ACT_TANH)
         if y is not h_out:
-            K.permute4(y, h_out, (N * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, y, h_out, N * g)
         return skips
 
     def _skip_halves(self, tag, skips, nsrc):
@@ -386,7 +384,7 @@ class GenerateEngine:
             cout = self.model.decoder.nc if k == n - 1 else self.chans[n - 2 - k]
             wS = self.wp[f"dec{k}"][cd * 16 * cout:]
             sk = skips[n - 1 - k]
-            if self._implicit(cd, cout) and k < n - 1:
+            if adt == torch.bfloat16 and implicit_shape(cd, cout) and k < n - 1:
                 addS = self._buf(G, f"{tag}_addS{k}", nsrc * 4 * Hi * Hi * cout, adt)
                 K.conv_gemm(2, sk, wS, addS, nsrc, Hi, Hi, cd, cout)
             else:
@@ -407,7 +405,7 @@ class GenerateEngine:
             hp = h_pred
         else:
             hp = self._buf(G, "dec_hp", rows * g, adt)
-            K.permute4(h_pred, hp, (rows * g, 1, 1, 1), (1, 0, 0, 0))
+            cast(K, h_pred, hp, rows * g)
         raw = self._buf(G, "dec_raw-1", rows * 16 * ctop, adt)
         d = self._buf(G, "dec_d-1", rows * 16 * ctop, adt)
         K.gemm(hp, self.wp["dec-1"], raw, rows, 16 * ctop, g, b_mn=True, bias=self.wp["dec-1.bias16"])
@@ -425,7 +423,7 @@ class GenerateEngine:
             gsrc = self.G.bufs["grp_zero"]
             Mo = rows * 4 * Hi * Hi
             y = self._buf(G, f"dec_y{k}", Mo * cout, adt)
-            if self._implicit(cd, cout) and not last:
+            if adt == torch.bfloat16 and implicit_shape(cd, cout) and not last:
                 sc, sh = self.bn[f"dec{k}"]
                 K.conv_gemm(2, d, wD, y, rows, Hi, Hi, cd, cout, bias=convt.bias.data, addend=addS, grp_src=gsrc,
                             imgs_per_group=nsrc, eval_scale=sc, eval_shift=sh, act=ACT_LRELU)
@@ -441,9 +439,9 @@ class GenerateEngine:
             Hi *= 2
         W, nc = Hi, dec.nc
         out32 = self._buf(G, "dec_out32", rows * W * W * nc)
-        K.permute4(d, out32, (rows * W * W * nc, 1, 1, 1), (1, 0, 0, 0))
+        cast(K, d, out32, rows * W * W * nc)
         K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
-        K.permute4(out32, frame_out, (rows, nc, W * W, 1), (W * W * nc, 1, nc, 0))
+        nhwc_to_nchw(K, out32, frame_out, rows, W * W, nc)
 
     # ------------------------------------------------------------------ recurrent modules
     def _module(self, m, seg_a, idx_a, seg_b, idx_b, gb, tuc, dt, eps=None, out=None):

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from ._lib import ACT_LRELU, ACT_NONE, ACT_SIGMOID, ACT_TANH, CudaKernels
+from .layouts import cast, nchw_to_nhwc, nhwc_to_nchw, pack_conv4, pack_convt4, tile_bias
 
 _EXACT = {}
 
@@ -81,7 +82,7 @@ def encoder_forward(mod, x):
     n = len(chans)
     B, nc, H = int(x.shape[0]), int(x.shape[1]), int(x.shape[2])
     a = torch.empty(B * H * H * nc, device=dev, dtype=adt)
-    K.permute4(x.contiguous().float(), a, (B, H * H, nc, 1), (nc * H * H, 1, H * H, 0))
+    nchw_to_nhwc(K, x.contiguous().float(), a, B, H * H, nc)
     skips = []
     cin = nc
     for l in range(n):
@@ -90,7 +91,7 @@ def encoder_forward(mod, x):
         cout, Ho = chans[l], H // 2
         M = B * Ho * Ho
         wp = torch.empty(cout * 16 * cin, device=dev, dtype=adt)
-        K.permute4(conv.weight.data, wp, (cout, 4, 4, cin), (cin * 16, 4, 1, 16))
+        pack_conv4(K, conv.weight.data, wp)
         col = torch.empty(M * 16 * cin, device=dev, dtype=adt)
         raw = torch.empty(M * cout, device=dev, dtype=adt)
         y = torch.empty(M * cout, device=dev, dtype=adt)
@@ -98,7 +99,7 @@ def encoder_forward(mod, x):
         K.gemm(col, wp, raw, M, cout, 16 * cin, bias=conv.bias.data)
         _bn(K, bn, raw, y, 1, B * Ho * Ho, cout, ACT_LRELU, dev)
         nchw = torch.empty(B, cout, Ho, Ho, device=dev)
-        K.permute4(y, nchw, (B, cout, Ho * Ho, 1), (Ho * Ho * cout, 1, cout, 0))
+        nhwc_to_nchw(K, y, nchw, B, Ho * Ho, cout)
         nchw._p2pvg_nhwc = y  # decoder_forward reuses the NHWC copy when it gets this very tensor back
         skips.append(nchw)
         a, H, cin = y, Ho, cout
@@ -106,13 +107,13 @@ def encoder_forward(mod, x):
     conv, bn = fin[0], fin[1]
     g = mod.dim
     wp = torch.empty(g * 16 * cin, device=dev, dtype=adt)
-    K.permute4(conv.weight.data, wp, (g, 4, 4, cin), (cin * 16, 4, 1, 16))
+    pack_conv4(K, conv.weight.data, wp)
     raw = torch.empty(B * g, device=dev, dtype=adt)
     y = torch.empty(B * g, device=dev, dtype=adt)
     K.gemm(a, wp, raw, B, g, 16 * cin, bias=conv.bias.data)
     _bn(K, bn, raw, y, 1, B, g, ACT_TANH, dev)
     h = torch.empty(B, g, device=dev)
-    K.permute4(y, h, (B * g, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, y, h, B * g)
     return h, skips
 
 
@@ -122,7 +123,7 @@ def _to_nhwc(K, t, adt):
         return cached
     B, C, H, W = (int(v) for v in t.shape)
     out = torch.empty(B * H * W * C, device=t.device, dtype=adt)
-    K.permute4(t.contiguous().float(), out, (B, H * W, C, 1), (C * H * W, 1, H * W, 0))
+    nchw_to_nhwc(K, t.contiguous().float(), out, B, H * W, C)
     return out
 
 
@@ -135,13 +136,13 @@ def decoder_forward(mod, vec, skip):
     vec = vec.reshape(-1, g).float().contiguous()
     B = int(vec.shape[0])
     hp = torch.empty(B * g, device=dev, dtype=adt)
-    K.permute4(vec, hp, (B * g, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, vec, hp, B * g)
     ctop = chans[-1]
     convt, bn = mod.upc1[0], mod.upc1[1]
     wp = torch.empty(g * 16 * ctop, device=dev, dtype=adt)
-    K.permute4(convt.weight.data, wp, (g, 4, 4, ctop), (ctop * 16, 4, 1, 16))
+    pack_convt4(K, convt.weight.data, wp)
     b16 = torch.empty(16 * ctop, device=dev)
-    K.permute4(convt.bias.data, b16, (16, ctop, 1, 1), (0, 1, 0, 0))
+    tile_bias(K, convt.bias.data, b16, 16)
     raw = torch.empty(B * 16 * ctop, device=dev, dtype=adt)
     d = torch.empty_like(raw)
     K.gemm(hp, wp, raw, B, 16 * ctop, g, b_mn=True, bias=b16)
@@ -156,7 +157,7 @@ def decoder_forward(mod, vec, skip):
         convt = blk[0] if last else blk.main[0]
         sk = _to_nhwc(K, skip[n - 1 - k], adt)
         wp = torch.empty(2 * cd * 16 * cout, device=dev, dtype=adt)
-        K.permute4(convt.weight.data, wp, (2 * cd, 4, 4, cout), (cout * 16, 4, 1, 16))
+        pack_convt4(K, convt.weight.data, wp)
         Md = B * Hi * Hi
         colD = torch.empty(Md * 16 * cout, device=dev, dtype=adt)
         colS = torch.empty(Md * 16 * cout, device=dev, dtype=adt)
@@ -171,10 +172,10 @@ def decoder_forward(mod, vec, skip):
         Hi *= 2
     W = Hi
     out32 = torch.empty(B * W * W * mod.nc, device=dev)
-    K.permute4(raw, out32, (B * W * W * mod.nc, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, raw, out32, B * W * W * mod.nc)
     K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
     out = torch.empty(B, mod.nc, W, W, device=dev)
-    K.permute4(out32, out, (B, mod.nc, W * W, 1), (W * W * mod.nc, 1, mod.nc, 0))
+    nhwc_to_nchw(K, out32, out, B, W * W, mod.nc)
     return out
 
 

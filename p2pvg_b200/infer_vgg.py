@@ -5,27 +5,21 @@ import torch
 
 from ._lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH
 from .infer import _act_dtype, _bn, _to_nhwc, kernels_for
-
-
-def _up8(n):
-    return (n + 7) // 8 * 8
+from .layouts import cast, implicit_shape, nchw_to_nhwc, nhwc_to_nchw, pack_conv3, pack_conv4, pack_convt4, tile_bias, up8
 
 
 def _conv3(K, a, conv, c0, cin, out, N, H, adt, dev, bias=True, accumulate_from=None):
     """out[N,H,H,cout] = conv3x3 over input channels [c0, c0+cin) of ``conv`` applied to a[N,H,H,cin]."""
     w = conv.weight.data
-    cout, cin_total = int(w.shape[0]), int(w.shape[1])
-    ld = _up8(9 * cin)
-    wp = torch.zeros(cout * 9 * cin + 8, device=dev, dtype=adt)
-    K.permute4(w.view(-1)[c0 * 9:], wp, (cout, 3, 3, cin), (cin_total * 9, 3, 1, 9))
+    cout = int(w.shape[0])
+    ld = up8(9 * cin)
+    scratch = torch.zeros(cout * 9 * cin + 8, device=dev, dtype=adt)
+    wp = torch.empty(cout * ld, device=dev, dtype=adt) if ld != 9 * cin else scratch
+    pack_conv3(K, w, wp, c0, cin, scratch=scratch)
     b = conv.bias.data if bias else None
-    if adt == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0:
+    if adt == torch.bfloat16 and implicit_shape(cin, cout):
         K.conv_gemm(3, a, wp, out, N, H, H, cin, cout, bias=b)
         return
-    if ld != 9 * cin:
-        wq = torch.empty(cout * ld, device=dev, dtype=adt)
-        K.permute4(wp, wq, (cout, ld, 1, 1), (9 * cin, 1, 0, 0))
-        wp = wq
     col = torch.empty(N * H * H * ld, device=dev, dtype=adt)
     K.im2col3(a, col, N, H, H, cin, ld, 1)
     K.gemm(col, wp, out, N * H * H, cout, ld, bias=b)
@@ -56,7 +50,7 @@ def vgg_encoder_forward(mod, x):
         raise ValueError(f"this vgg backbone expects {mod.image_width}x{mod.image_width} frames")
     nst = mod.nstage
     a = torch.empty(B * H * H * nc, device=dev, dtype=adt)
-    K.permute4(x.contiguous().float(), a, (B, H * H, nc, 1), (nc * H * H, 1, H * H, 0))
+    nchw_to_nhwc(K, x.contiguous().float(), a, B, H * H, nc)
     skips, C = [], nc
     for i in range(1, nst + 1):
         if i > 1:
@@ -66,7 +60,7 @@ def vgg_encoder_forward(mod, x):
         for blk in getattr(mod, f"c{i}"):
             a, C = _layer(K, blk, a, B, H, adt, dev)
         nchw = torch.empty(B, C, H, H, device=dev)
-        K.permute4(a, nchw, (B, C, H * H, 1), (H * H * C, 1, C, 0))
+        nhwc_to_nchw(K, a, nchw, B, H * H, C)
         nchw._p2pvg_nhwc = a
         skips.append(nchw)
     p = torch.empty(B * 16 * C, device=dev, dtype=adt)
@@ -75,13 +69,13 @@ def vgg_encoder_forward(mod, x):
     conv, bn = top[0], top[1]
     g = mod.dim
     wp = torch.empty(g * 16 * C, device=dev, dtype=adt)
-    K.permute4(conv.weight.data, wp, (g, 4, 4, C), (C * 16, 4, 1, 16))
+    pack_conv4(K, conv.weight.data, wp)
     raw = torch.empty(B * g, device=dev, dtype=adt)
     y = torch.empty(B * g, device=dev, dtype=adt)
     K.gemm(p, wp, raw, B, g, 16 * C, bias=conv.bias.data)
     _bn(K, bn, raw, y, 1, B, g, ACT_TANH, dev)
     h = torch.empty(B, g, device=dev)
-    K.permute4(y, h, (B * g, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, y, h, B * g)
     return h, skips
 
 
@@ -93,12 +87,12 @@ def vgg_decoder_forward(mod, vec, skip):
     vec = vec.reshape(-1, g).float().contiguous()
     B = int(vec.shape[0])
     hp = torch.empty(B * g, device=dev, dtype=adt)
-    K.permute4(vec, hp, (B * g, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, vec, hp, B * g)
     convt, bn = mod.upc1[0], mod.upc1[1]
     wp = torch.empty(g * 16 * 512, device=dev, dtype=adt)
-    K.permute4(convt.weight.data, wp, (g, 4, 4, 512), (512 * 16, 4, 1, 16))
+    pack_convt4(K, convt.weight.data, wp)
     b16 = torch.empty(16 * 512, device=dev)
-    K.permute4(convt.bias.data, b16, (16, 512, 1, 1), (0, 1, 0, 0))
+    tile_bias(K, convt.bias.data, b16, 16)
     raw = torch.empty(B * 16 * 512, device=dev, dtype=adt)
     d = torch.empty_like(raw)
     K.gemm(hp, wp, raw, B, 16 * 512, g, b_mn=True, bias=b16)
@@ -116,19 +110,17 @@ def vgg_decoder_forward(mod, vec, skip):
         for blk in layers[1:]:
             d, C = _layer(K, blk, d, B, H, adt, dev)
     convt = getattr(mod, f"upc{nst + 1}")[1]
-    ldl = _up8(9 * nc)
-    w27 = torch.zeros(64 * 9 * nc + 8, device=dev, dtype=adt)
-    K.permute4(convt.weight.data, w27, (64, 3, 3, nc), (nc * 9, 3, 1, 9))
+    ldl = up8(9 * nc)
     wl = torch.empty(64 * ldl, device=dev, dtype=adt)
-    K.permute4(w27, wl, (64, ldl, 1, 1), (9 * nc, 1, 0, 0))
+    pack_conv3(K, convt.weight.data, wl, scratch=torch.zeros(64 * 9 * nc + 8, device=dev, dtype=adt))
     M = B * W0 * W0
     colT = torch.empty(M * ldl, device=dev, dtype=adt)
     K.gemm(d, wl, colT, M, ldl, 64, b_mn=True)
     raw = torch.empty(M * nc, device=dev, dtype=adt)
     K.col2im3(colT, raw, B, W0, W0, nc, ldl, bias=convt.bias.data)
     out32 = torch.empty(M * nc, device=dev)
-    K.permute4(raw, out32, (M * nc, 1, 1, 1), (1, 0, 0, 0))
+    cast(K, raw, out32, M * nc)
     K.act_fwd(out32, M * nc, ACT_SIGMOID)
     out = torch.empty(B, nc, W0, W0, device=dev)
-    K.permute4(out32, out, (B, nc, W0 * W0, 1), (W0 * W0 * nc, 1, nc, 0))
+    nhwc_to_nchw(K, out32, out, B, W0 * W0, nc)
     return out
