@@ -1,6 +1,6 @@
-"""Shadow of the reference's ``data`` package: ``data.data_utils`` comes from here (Moving MNIST rendered on the GPU), every
-other submodule (``data.moving_mnist``, ``data.weizmann``, ``data.bair``, ...) keeps resolving to the reference checkout named
-by $P2PVG_REF (or any later ``data`` directory on sys.path)."""
+"""Shadow of the reference's ``data`` package: ``data.data_utils`` comes from here (Moving MNIST, Weizmann and BAIR batches
+made on the GPU), every other submodule (``data.moving_mnist``, ``data.weizmann``, ``data.bair``, ...) keeps resolving to the
+reference checkout named by $P2PVG_REF (or any later ``data`` directory on sys.path)."""
 import os
 import sys
 

@@ -1,6 +1,7 @@
 """Drop-in for the reference's ``data/data_utils.py``: the ``mnist`` branches of ``load_dataset`` and ``get_data_generator``
-render Moving MNIST batches on the GPU (``p2pvg_b200.data.MovingMNIST``); every other call and dataset is delegated
-unchanged to the reference's own module, loaded from the reference's ``data/`` directory.
+render Moving MNIST batches on the GPU (``p2pvg_b200.data.MovingMNIST``), the ``weizmann`` and ``bair`` branches cut them
+from clips decoded once into device memory (``p2pvg_b200.data.ClipBatches``); every other call and dataset (``h36m``) is
+delegated unchanged to the reference's own module, loaded from the reference's ``data/`` directory.
 
 The generator yields what the reference's ``get_generator`` yields, fp32 [T, B, 1, S, S] on the device, and draws T from
 NumPy's global stream at the same point; the digit trajectories are drawn on the device (torch's CUDA generator, seeded by
@@ -12,7 +13,7 @@ import os
 import numpy as np
 
 import data as _pkg
-from p2pvg_b200.data import MovingMNIST, load_mnist_digits
+from p2pvg_b200.data import ClipBatches, MovingMNIST, load_bair_clips, load_mnist_digits, load_weizmann_clips
 
 _here = os.path.dirname(os.path.abspath(__file__))
 _ref = None
@@ -59,7 +60,39 @@ class MovingMNISTDigits:
         return self.N
 
 
+class VideoClipSet:
+    """Stands in for ``WeizmannDataset`` (data/weizmann.py) or ``BairRobotPush`` (data/bair.py) wherever ``train.py`` and
+    ``get_generator`` use the dataset object: the same ``get_seq_len`` bounds and ``__len__``; the frames are the device clip
+    store ``clips`` (a ``p2pvg_b200.data.VideoClips``), cut into batches by ``ClipBatches`` with ``sampling``."""
+
+    def __init__(self, clips, train, seq_len, sampling, length):
+        self.clips, self.train, self.seq_len, self.sampling, self.length = clips, train, seq_len, sampling, length
+        self.max_seq_len, self.channels, self.image_size = clips.max_seq_len, 3, clips.frames.shape[-1]
+
+    def get_seq_len(self):
+        return np.random.randint(low=self.seq_len[0], high=self.seq_len[1] + 1)
+
+    def __len__(self):
+        return self.length
+
+
+def _weizmann(opt, train):
+    L = 18 if train else 10    # data_utils.py: train_max_seq_len / test_max_seq_len
+    clips = load_weizmann_clips(opt.data_root, train, L, opt.image_width)
+    return VideoClipSet(clips, train, (10 if train else 6, L), "permutation", len(clips))
+
+
+def _bair(opt, train):
+    clips = load_bair_clips(opt.data_root, train, opt.max_seq_len, opt.image_width)
+    return VideoClipSet(clips, train, (opt.max_seq_len - 2 * opt.delta_len, opt.max_seq_len),
+                        "uniform" if train else "ordered", 10000)
+
+
 def load_dataset(opt, eval=False, eval_len=None, id_act=None):
+    if opt.dataset in ("weizmann", "bair"):
+        assert opt.channels == 3, "=> %s has 3 channels, but opt.channels = %d" % (opt.dataset, opt.channels)
+        make = _weizmann if opt.dataset == "weizmann" else _bair
+        return make(opt, True), make(opt, False)
     if opt.dataset != "mnist":
         return _reference().load_dataset(opt, eval=eval, eval_len=eval_len, id_act=id_act)
     kw = dict(data_root=opt.data_root, max_seq_len=opt.max_seq_len, delta_len=opt.delta_len, image_size=opt.image_width,
@@ -68,6 +101,10 @@ def load_dataset(opt, eval=False, eval_len=None, id_act=None):
 
 
 def get_data_generator(data, train=True, dynamic_length=True, opt=None):
+    if opt.dataset in ("weizmann", "bair"):
+        if not dynamic_length:
+            raise NotImplementedError("device clip batches always have the dynamic length get_seq_len() draws")
+        return ClipBatches(data.clips, opt.batch_size, data.sampling, data.seq_len, device="cuda")
     if opt.dataset != "mnist":
         return _reference().get_data_generator(data, train=train, dynamic_length=dynamic_length, opt=opt)
     if not dynamic_length:

@@ -317,6 +317,23 @@ int p2pvg_scale(float* x, int64_t n, float a, void* stream);
 int p2pvg_moving_mnist(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B, int S,
                        int num_digits, int deterministic, void* stream);
 
+/* Video training batches cut from a device-resident uint8 clip store: the windows WeizmannDataset.__getitem__
+ * (data/weizmann.py:103-114) and BairRobotPush.get_seq (data/bair.py:51-75) return, time-major and truncated to T frames.
+ *   frames     [F][C][H][W] uint8, 4-byte aligned; clip c is frames[clip_first[c] .. clip_first[c] + clip_len[c])
+ *   entries    [B] int32: paired_flips = 1: entry e is clip e >> 1, mirrored left-right when e is odd (the reference appends
+ *              each clip, then its RandomHorizontalFlip(p=1) copy); paired_flips = 0: entry e is clip e, never mirrored
+ *   draws      [B] int32 or NULL: row b's window starts at (unsigned)draws[b] % (clip_len - L + 1), i.e.
+ *              np.random.randint(0, n_frames - L + 1) as lo + r % (hi - lo); NULL: every window starts at frame 0
+ *   out        [T][B][C][H][W] fp32, 16-byte aligned: out[t, b, c, y, x] = frames[first + start + t][c][y][x'] / 255 (ToTensor,
+ *              correctly rounded), x' = W - 1 - x for a mirrored entry.  T <= L: the first T frames of the L-frame window.
+ * Precondition (not checked on the device): every entry lies in [0, n_clips * (paired_flips ? 2 : 1)) and every clip an entry
+ * names has clip_len >= L; p2pvg_b200.data.ClipBatches builds entries and draws that way.
+ * P2PVG_ERR_BAD_ARG: NULL frames / clip tables / entries / out, misaligned frames or out, n_clips < 1, B < 0, T < 0, T > L,
+ * L < 1, C < 1, H < 1, W % 4 != 0 or W < 4.  P2PVG_ERR_UNSUPPORTED: C * H * W > 2^30 or T * B >= 2^31. */
+int p2pvg_video_windows(const uint8_t* frames, const int64_t* clip_first, const int32_t* clip_len, int n_clips,
+                        const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H, int W,
+                        float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

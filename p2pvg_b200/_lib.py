@@ -387,3 +387,16 @@ class CudaKernels:
         assert digits.is_contiguous() and draws.is_contiguous() and out.is_contiguous()
         self._ck(self.lib.p2pvg_moving_mnist(_p(digits), _i(digits.shape[0]), _p(draws), _i(draws.shape[-1]), _p(out), _i(T), _i(B),
                                              _i(S), _i(num_digits), _i(int(deterministic)), self._stream()))
+
+    def video_windows(self, frames, clip_first, clip_len, entries, draws, paired_flips, L, out):
+        """frames uint8 [F,C,H,W], clip_first int64 / clip_len int32 [n_clips], entries int32 [B], draws int32 [B] or None,
+        out fp32 [T,B,C,H,W] (p2pvg_video_windows)."""
+        assert frames.dtype == torch.uint8 and clip_first.dtype == torch.int64 and clip_len.dtype == torch.int32
+        assert entries.dtype == torch.int32 and (draws is None or draws.dtype == torch.int32) and out.dtype == torch.float32
+        assert all(t is None or t.is_contiguous() for t in (frames, clip_first, clip_len, entries, draws, out))
+        T, B, C, H, W = out.shape
+        assert frames.dim() == 4 and tuple(frames.shape[1:]) == (C, H, W) and len(entries) == B
+        assert len(clip_len) == len(clip_first) and (draws is None or len(draws) == B)
+        self._ck(self.lib.p2pvg_video_windows(_p(frames), _p(clip_first), _p(clip_len), _i(len(clip_len)), _p(entries), _p(draws),
+                                              _i(int(paired_flips)), _i(B), _i(L), _i(T), _i(C), _i(H), _i(W), _p(out),
+                                              self._stream()))

@@ -99,6 +99,8 @@ int p2pvg_convt_c1_loss_impl(const void*, const void*, int, const int*, const fl
 int p2pvg_adam_legacy_impl(float*, const float*, float*, float*, long long, double, double, double, double, const int*, cudaStream_t);
 int p2pvg_scale_impl(float*, long long, float, cudaStream_t);
 int p2pvg_moving_mnist_impl(const uint8_t*, int, const int32_t*, int, float*, int, int, int, int, int, cudaStream_t);
+int p2pvg_video_windows_impl(const uint8_t*, const int64_t*, const int32_t*, int, const int32_t*, const int32_t*, int, int, int, int,
+                             int, int, int, float*, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -326,6 +328,11 @@ int p2pvg_scale(float* x, int64_t n, float a, void* stream) { return p2pvg_scale
 int p2pvg_moving_mnist(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B, int S,
                        int num_digits, int deterministic, void* stream) {
   return p2pvg_moving_mnist_impl(digits, n_digits, draws, draw_stride, out, T, B, S, num_digits, deterministic, ST);
+}
+int p2pvg_video_windows(const uint8_t* frames, const int64_t* clip_first, const int32_t* clip_len, int n_clips,
+                        const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H, int W,
+                        float* out, void* stream) {
+  return p2pvg_video_windows_impl(frames, clip_first, clip_len, n_clips, entries, draws, paired_flips, B, L, T, C, H, W, out, ST);
 }
 
 }  // extern "C"

@@ -13,11 +13,18 @@ the digits loaded once by ``load_mnist_digits``.
 
     for x in MovingMNIST(load_mnist_digits(root), batch_size=256, max_seq_len=30, delta_len=5):
         losses = model(x, 0, len(x) - 1)
+
+Weizmann and BAIR are decoded once into a uint8 clip store on the device (``load_weizmann_clips``, ``load_bair_clips``);
+``ClipBatches`` then cuts every batch out of it with one ``p2pvg_video_windows`` launch.
+
+    for x in ClipBatches(load_weizmann_clips(root, True, 18, 64), 128, "permutation", seq_len=(10, 18)):
+        losses = model(x, 0, len(x) - 1)
 """
 from __future__ import annotations
 
 import gzip
 import os
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -87,6 +94,173 @@ class MovingMNIST:
             draws = torch.randint(0, 2 ** 31 - 1, (B, nd, 5 + 4 * T), dtype=torch.int32, device=self.device, generator=self.generator)
             out = torch.empty(T, B, 1, S, S, dtype=torch.float32, device=self.device)
             self.K.moving_mnist(self.digits, draws, out, T, B, S, nd, self.deterministic)
+        return out
+
+
+class VideoClips:
+    """Clips decoded once: ``frames`` uint8 [F, 3, S, S], clip c = ``frames[clip_first[c]:clip_first[c] + clip_len[c]]``.
+
+    With ``paired_flips`` the dataset's entries are 2 * len(names): entry e is clip e >> 1, mirrored left-right when e is odd
+    (the order in which ``WeizmannDataset`` appends each clip and its flipped copy); otherwise entry e is clip e.
+    ``max_seq_len`` is the window length L every entry is cut to (each clip holds at least L frames)."""
+
+    def __init__(self, frames, clip_first, clip_len, names, paired_flips, max_seq_len):
+        self.frames, self.clip_first, self.clip_len = frames, clip_first, clip_len
+        self.names, self.paired_flips, self.max_seq_len = list(names), bool(paired_flips), int(max_seq_len)
+
+    def __len__(self):
+        return len(self.names) * (2 if self.paired_flips else 1)
+
+    def entry(self, e):
+        """(clip name, mirrored) of entry e."""
+        return (self.names[e >> 1], bool(e & 1)) if self.paired_flips else (self.names[e], False)
+
+    def to(self, device):
+        return VideoClips(self.frames.to(device), self.clip_first.to(device), self.clip_len.to(device), self.names,
+                          self.paired_flips, self.max_seq_len)
+
+
+def _read_frame(path, image_size):
+    """One frame as uint8 [3, S, S], what ``ToTensor`` gives the reference before / 255: an RGB frame as is, a mode-L frame
+    replicated to the three channels (the reference's broadcasting assignment into its [T, 3, S, S] buffer)."""
+    from PIL import Image
+    with Image.open(path) as im:
+        if im.size != (image_size, image_size):
+            raise ValueError(f"{path}: frame is {im.size[0]}x{im.size[1]}, expected {image_size}x{image_size}")
+        if im.mode == "RGB":
+            return np.asarray(im).transpose(2, 0, 1)
+        if im.mode == "L":
+            return np.broadcast_to(np.asarray(im), (3, image_size, image_size))
+        raise ValueError(f"{path}: image mode {im.mode!r}, expected 'RGB' or 'L'")
+
+
+def _decode_clips(clips, image_size, device, chunk_frames=4096):
+    """clips: [(name, [frame paths])] -> the uint8 store on ``device``, decoded by a thread pool (PIL releases the GIL while it
+    decodes) and copied over in chunks, so host memory holds one chunk, not the dataset."""
+    if not clips:
+        raise ValueError("no clip is long enough for the requested max_seq_len")
+    lens = [len(paths) for _, paths in clips]
+    paths = [p for _, ps in clips for p in ps]
+    S = image_size
+    frames = torch.empty((len(paths), 3, S, S), dtype=torch.uint8, device=device)
+    buf = np.empty((min(chunk_frames, len(paths)), 3, S, S), dtype=np.uint8)
+
+    def read(i, base):
+        buf[i - base] = _read_frame(paths[i], S)
+
+    with ThreadPoolExecutor(max_workers=min(32, os.cpu_count() or 1)) as pool:
+        for base in range(0, len(paths), len(buf)):
+            n = min(len(buf), len(paths) - base)
+            list(pool.map(read, range(base, base + n), [base] * n))
+            frames[base:base + n].copy_(torch.from_numpy(buf[:n]))
+    first = np.concatenate([[0], np.cumsum(lens)[:-1]])
+    return frames, torch.tensor(first, dtype=torch.int64, device=device), torch.tensor(lens, dtype=torch.int32, device=device)
+
+
+def load_weizmann_clips(data_root, train, max_seq_len, image_size, device="cuda"):
+    """``WeizmannDataset`` (data/weizmann.py:34-88) as a ``VideoClips``: identities are the subdirectories of
+    ``<data_root>/weizmann``, actions and frames are taken in ``sorted()`` name order, train is frames [0, n * 2 // 3) of each
+    action and test the rest, and a split shorter than ``max_seq_len`` is dropped.  Flipped copies are not stored: the kernel
+    mirrors odd entries.  Known deviation: the reference takes identities in raw ``os.listdir`` order, which depends on the
+    filesystem; here they are sorted, so entry numbers can differ from the reference's while the set of entries is the same.
+    Frames must be ``image_size`` square, RGB or L (ValueError naming the file otherwise)."""
+    root = os.path.join(data_root, "weizmann")
+    clips = []
+    for ident in sorted(d for d in os.listdir(root) if os.path.isdir(os.path.join(root, d))):
+        for act in sorted(os.listdir(os.path.join(root, ident))):
+            names = sorted(os.listdir(os.path.join(root, ident, act)))
+            num_train = len(names) * 2 // 3
+            lo, hi = (0, num_train) if train else (num_train, len(names))
+            if hi - lo < max_seq_len:
+                continue
+            clips.append((f"{ident}/{act}", [os.path.join(root, ident, act, f) for f in names[lo:hi]]))
+    store = _decode_clips(clips, image_size, device)
+    return VideoClips(*store, [c[0] for c in clips], paired_flips=True, max_seq_len=max_seq_len)
+
+
+def load_bair_clips(data_root, train, max_seq_len, image_size, device="cuda"):
+    """``BairRobotPush`` (data/bair.py:22-31, 61-69) as a ``VideoClips``: one clip per trajectory directory
+    ``<data_root>/bair/processed_data/{train,test}/<d1>/<d2>``, frames ``0.png .. <max_seq_len - 1>.png``.  Known deviation:
+    the reference lists d1 and d2 in raw ``os.listdir`` order, which depends on the filesystem; here both are sorted.  Frames
+    are not resized: they must already be ``image_size`` square (the reference hard-codes 64 x 64), RGB or L."""
+    data_dir = os.path.join(data_root, "bair", "processed_data", "train" if train else "test")
+    clips = []
+    for d1 in sorted(os.listdir(data_dir)):
+        for d2 in sorted(os.listdir(os.path.join(data_dir, d1))):
+            traj = os.path.join(data_dir, d1, d2)
+            clips.append((f"{d1}/{d2}", [os.path.join(traj, f"{i}.png") for i in range(max_seq_len)]))
+    store = _decode_clips(clips, image_size, device)
+    return VideoClips(*store, [c[0] for c in clips], paired_flips=False, max_seq_len=max_seq_len)
+
+
+# BairRobotPush.__len__: a DataLoader epoch over it is 10000 // batch_size batches
+BAIR_EPOCH_ITEMS = 10000
+SAMPLING = ("permutation", "uniform", "ordered")
+
+
+def ordered_schedule(n_entries, batch_size, epoch_items=BAIR_EPOCH_ITEMS):
+    """The entries of one epoch of ``ordered`` sampling, batch after batch (int64 [epoch_items // batch_size * batch_size]).
+    ``BairRobotPush.get_seq`` walks its trajectories in order and wraps at the end, whatever index it is asked for; each epoch
+    of the reference's DataLoader runs in a fresh worker holding a fresh copy of the dataset, so the walk restarts at 0."""
+    return torch.arange(epoch_items // batch_size * batch_size) % n_entries
+
+
+class ClipBatches:
+    """Endless iterator of fp32 [T, B, 3, S, S] device batches cut from ``clips`` (``p2pvg_video_windows``), time-major like
+    the reference's ``get_generator`` after ``.permute(1, 0, 2, 3, 4).cuda()[:seq_len]`` (data/data_utils.py:112-122).
+
+    Per batch, ``T = np.random.randint(lo, hi + 1)`` is drawn from NumPy's global stream, where ``get_generator`` calls
+    ``get_seq_len()``.  ``sampling`` picks the entries:
+      permutation  ``DataLoader(shuffle=True, drop_last=True)`` over the entries (Weizmann): a device ``randperm`` per epoch,
+                   ``len(clips) // B`` batches per epoch, each row's window start drawn on the device (``randint``)
+      uniform      entries drawn with replacement, windows start at frame 0 (BAIR train, bair.py:59)
+      ordered      entries in order, wrapping at the end, restarting at entry 0 every ``10000 // B`` batches: each epoch's
+                   loader worker starts from a fresh copy of the dataset (BAIR test, bair.py:52-57)
+    Random draws come from ``generator`` (a CUDA generator) instead of the reference's worker-process NumPy stream: the same
+    distributions, other values.  Each batch is a fresh tensor, never written again."""
+
+    def __init__(self, clips, batch_size, sampling, seq_len, device="cuda", generator=None):
+        from ._lib import kernels_for
+        if sampling not in SAMPLING:
+            raise ValueError(f"sampling = {sampling!r}, expected one of {SAMPLING}")
+        lo, hi = (int(v) for v in seq_len)
+        if not 1 <= lo <= hi <= clips.max_seq_len:
+            raise ValueError(f"seq_len = ({lo}, {hi}): needs 1 <= lo <= hi <= max_seq_len = {clips.max_seq_len}")
+        B, n = int(batch_size), len(clips)
+        if B < 1:
+            raise ValueError(f"batch_size = {B}")
+        epoch = {"permutation": n, "uniform": B, "ordered": BAIR_EPOCH_ITEMS}[sampling] // B
+        if epoch == 0:
+            raise ValueError(f"batch_size = {B} exceeds the {n if sampling == 'permutation' else BAIR_EPOCH_ITEMS} items of an "
+                             "epoch: the reference's drop_last loader would yield no batch")
+        self.K = kernels_for(device)
+        self.device = self.K.device
+        self.clips = clips.to(self.device)
+        self.batch_size, self.sampling, self.seq_len, self.generator = B, sampling, (lo, hi), generator
+        self.epoch_batches, self.k = epoch, 0
+        self.order = None
+        if sampling == "ordered":
+            self.order = ordered_schedule(n, B).to(self.device, torch.int32)
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        T = int(np.random.randint(self.seq_len[0], self.seq_len[1] + 1))
+        B, k, c = self.batch_size, self.k, self.clips
+        with torch.cuda.device(self.device):
+            draws = None
+            if self.sampling == "permutation":
+                if k == 0:
+                    self.order = torch.randperm(len(c), dtype=torch.int32, device=self.device, generator=self.generator)
+                draws = torch.randint(0, 2 ** 31 - 1, (B,), dtype=torch.int32, device=self.device, generator=self.generator)
+            if self.sampling == "uniform":
+                entries = torch.randint(0, len(c), (B,), dtype=torch.int32, device=self.device, generator=self.generator)
+            else:
+                entries = self.order[k * B:(k + 1) * B]
+            out = torch.empty((T, B) + tuple(c.frames.shape[1:]), dtype=torch.float32, device=self.device)
+            self.K.video_windows(c.frames, c.clip_first, c.clip_len, entries, draws, c.paired_flips, c.max_seq_len, out)
+        self.k = (k + 1) % self.epoch_batches
         return out
 
 
