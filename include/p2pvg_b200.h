@@ -247,6 +247,48 @@ typedef struct p2pvg_lstm_step_module {
   float* logvar;
 } p2pvg_lstm_step_module;
 int p2pvg_lstm_step(const p2pvg_lstm_step_module* modules /*host array*/, int n_modules, int rows, int R, void* stream);
+/* One whole call of the h36m pose encoder or decoder (models/h36m_mlp.py:28-95; no BatchNorm, so eval == train) in ONE launch.
+ *   residual_linear(nin, nout):  LayerNorm(relu(shortcut(x)) + relu(L3(relu(L2(relu(L1(x))))))), long-path width nin / 2,
+ *                                LayerNorm eps 1e-5 (the nn.LayerNorm default)
+ *   encoder (decoder = 0): fc1 = residual_linear(51, g), fc2 = residual_linear(g, g), out = tanh(fc3(h2)) [rows][g];
+ *                          h1 / h2 [rows][g] (the skips) written when non-NULL
+ *   decoder (decoder = 1): d1 = fc1(x) with fc1 = residual_linear(g, g), d2 = fc2([d1 | skip2]) with residual_linear(2g, g),
+ *                          out = fc3([d2 | skip1]) [rows][51] (Linear 2g -> 51, no activation); output row r reads skip row
+ *                          r % nsrc of skip1 / skip2 [nsrc][g] (skips encoded at B rows shared by nsample * B rows)
+ *   input row b = src[(src_idx[0] * rows + b) * in_dim + 0 : in_dim] (in_dim 51 / g; src_idx is a device pointer read at run time,
+ *                 NULL = frame 0)
+ * Clusters of 8 CTAs per slab of 8 rows, each CTA owning 1/8 of every Linear's output units (uneven for 25 / 51); stage outputs
+ * are pushed to every CTA of the cluster through distributed shared memory; weights stream from L2; exact fp32 FFMA.
+ * P2PVG_ERR_BAD_ARG: NULL pointers, g < 8, nsrc < 1.  P2PVG_ERR_UNSUPPORTED: the slab does not fit in shared memory. */
+typedef struct p2pvg_pose_residual {
+  const float* w_sc;   /* shortcut Linear [nout][nin], bias [nout] */
+  const float* b_sc;
+  const float* w1;     /* long path: [nin/2][nin], [nin/2][nin/2], [nout][nin/2] and their biases */
+  const float* b1;
+  const float* w2;
+  const float* b2;
+  const float* w3;
+  const float* b3;
+  const float* gamma;  /* LayerNorm(nout) */
+  const float* beta;
+} p2pvg_pose_residual;
+typedef struct p2pvg_pose_mlp_args {
+  int decoder;
+  int g;
+  const float* src;
+  const int* src_idx;
+  p2pvg_pose_residual fc1;
+  p2pvg_pose_residual fc2;
+  const float* w3;     /* fc3: encoder [g][g], decoder [51][2g] */
+  const float* b3;
+  const float* skip1;  /* decoder only */
+  const float* skip2;
+  int nsrc;
+  float* out;
+  float* h1;           /* encoder only */
+  float* h2;
+} p2pvg_pose_mlp_args;
+int p2pvg_pose_mlp(const p2pvg_pose_mlp_args* args /*host*/, int rows, void* stream);
 /* gaussian_lstm.reparameterize (models/lstm.py:76-81) for posterior and prior + KLCriterion.forward
  * (misc/criterion.py:10-15) summed over all elements (division by opt.batch_size happens in finalize_losses). */
 int p2pvg_reparam_kl_fwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,

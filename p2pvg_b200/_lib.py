@@ -77,6 +77,26 @@ class LstmStepModule(ctypes.Structure):
 LSTM_HEAD_LINEAR_TANH, LSTM_HEAD_GAUSSIAN = 0, 1
 
 
+class PoseResidual(ctypes.Structure):
+    """p2pvg_pose_residual (include/p2pvg_b200.h): the parameters of one residual_linear block."""
+    _fields_ = [(k, ctypes.c_void_p) for k in ("w_sc", "b_sc", "w1", "b1", "w2", "b2", "w3", "b3", "gamma", "beta")]
+
+
+class PoseMlpArgs(ctypes.Structure):
+    """p2pvg_pose_mlp_args (include/p2pvg_b200.h)."""
+    _fields_ = [("decoder", ctypes.c_int), ("g", ctypes.c_int), ("src", ctypes.c_void_p), ("src_idx", ctypes.c_void_p),
+                ("fc1", PoseResidual), ("fc2", PoseResidual), ("w3", ctypes.c_void_p), ("b3", ctypes.c_void_p),
+                ("skip1", ctypes.c_void_p), ("skip2", ctypes.c_void_p), ("nsrc", ctypes.c_int), ("out", ctypes.c_void_p),
+                ("h1", ctypes.c_void_p), ("h2", ctypes.c_void_p)]
+
+
+def pose_residual(rl):
+    """PoseResidual of a models.h36m_mlp.residual_linear module (pointers to its live parameters)."""
+    lins = (rl.shortcut[0], rl.long_path[0], rl.long_path[2], rl.long_path[4])
+    ptrs = [t.data_ptr() for lin in lins for t in (lin.weight, lin.bias)] + [rl.norm.weight.data_ptr(), rl.norm.bias.data_ptr()]
+    return PoseResidual(*ptrs)
+
+
 class _Workspaces:
     """Scratch buffers of one device, shared by every CudaKernels view of it.  ``gen`` counts re-allocations: a captured
     CUDA graph that used a workspace is stale once it moved (TrainEngine.graph_generation)."""
@@ -309,6 +329,18 @@ class CudaKernels:
             for k, v in m.items():
                 setattr(arr[i], k, v if isinstance(v, int) else (v.data_ptr() if v is not None else None))
         self._ck(self.lib.p2pvg_lstm_step(arr, _i(len(modules)), _i(rows), _i(R), self._stream()))
+
+    def pose_mlp(self, mod, decoder, src, out, rows, src_idx=None, skips=None, nsrc=0, h1=None, h2=None):
+        """p2pvg_pose_mlp: one call of a models.h36m_mlp encoder (decoder=False; h1 / h2 receive the skips when given) or
+        decoder (decoder=True; skips = [h1, h2] of an encoder call on nsrc rows) on `rows` rows of src[src_idx[0]]."""
+        s1, s2 = skips if skips is not None else (None, None)
+        a = PoseMlpArgs(decoder=int(decoder), g=mod.fc1.norm.normalized_shape[0], src=src.data_ptr(),
+                        src_idx=src_idx.data_ptr() if src_idx is not None else None, fc1=pose_residual(mod.fc1),
+                        fc2=pose_residual(mod.fc2), w3=mod.fc3.weight.data_ptr(), b3=mod.fc3.bias.data_ptr(),
+                        skip1=s1.data_ptr() if s1 is not None else None, skip2=s2.data_ptr() if s2 is not None else None,
+                        nsrc=int(nsrc), out=out.data_ptr(), h1=h1.data_ptr() if h1 is not None else None,
+                        h2=h2.data_ptr() if h2 is not None else None)
+        self._ck(self.lib.p2pvg_pose_mlp(ctypes.byref(a), _i(rows), self._stream()))
 
     def reparam_kl_fwd(self, mu, lv, mu_p, lv_p, eps, eps_p, z, z_p, n, kl_sum):
         self._ck(self.lib.p2pvg_reparam_kl_fwd(_p(mu), _p(lv), _p(mu_p), _p(lv_p), _p(eps), _p(eps_p), _p(z), _p(z_p), _i(n),

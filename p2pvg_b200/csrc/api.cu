@@ -79,6 +79,7 @@ int p2pvg_lstm_cluster512_bwd_impl(const float*, const float*, const float*, con
 int p2pvg_lstm_cluster512_max_clusters_impl(int);
 int p2pvg_lstm_cluster_max_clusters_impl(int);
 int p2pvg_lstm_step_impl(const p2pvg_lstm_step_module*, int, int, int, cudaStream_t);
+int p2pvg_pose_mlp_impl(const p2pvg_pose_mlp_args*, int, cudaStream_t);
 int p2pvg_reparam_kl_fwd_impl(const float*, const float*, const float*, const float*, const float*, const float*, float*, float*, int,
                               float*, cudaStream_t);
 int p2pvg_reparam_kl_bwd_impl(const float*, const float*, const float*, const float*, const float*, const float*, const float*,
@@ -262,6 +263,7 @@ int p2pvg_lstm_cluster_max_clusters(int which) { return p2pvg_lstm_cluster_max_c
 int p2pvg_lstm_step(const p2pvg_lstm_step_module* modules, int n_modules, int rows, int R, void* stream) {
   return p2pvg_lstm_step_impl(modules, n_modules, rows, R, ST);
 }
+int p2pvg_pose_mlp(const p2pvg_pose_mlp_args* args, int rows, void* stream) { return p2pvg_pose_mlp_impl(args, rows, ST); }
 int p2pvg_reparam_kl_fwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
                          const float* eps_p, float* z, float* z_p, int n, float* kl_sum, void* stream) {
   return p2pvg_reparam_kl_fwd_impl(mu, lv, mu_p, lv_p, eps, eps_p, z, z_p, n, kl_sum, ST);

@@ -8,6 +8,7 @@
 // fp32 FFMA, the same arithmetic class as the CUDA-core GEMMs of the eager generation path.  blockIdx.y = module.
 #include <cooperative_groups.h>
 
+#include "cluster_rows.cuh"
 #include "common.cuh"
 #include "../../include/p2pvg_b200.h"
 
@@ -26,23 +27,6 @@ __device__ __forceinline__ float in_elem(const p2pvg_lstm_step_module& m, int ro
   k -= m.ga;
   if (k < m.gb) return m.seg_b[((long long)m.idx_b[0] * rows + b) * m.gb + k];
   return k == m.gb ? m.tuc[0] : m.dt[0];
-}
-
-// acc[b] = sum_k w[k] * x[b * ldx + k] over the warp (lanes along k), result in every lane
-__device__ __forceinline__ void warp_dot(const float* __restrict__ w, const float* x, int ldx, int K, int nrows, int lane,
-                                         float (&acc)[SLAB]) {
-#pragma unroll
-  for (int b = 0; b < SLAB; b++) acc[b] = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    const float wk = __ldg(w + k);
-#pragma unroll
-    for (int b = 0; b < SLAB; b++)
-      if (b < nrows) acc[b] = fmaf(wk, x[b * ldx + k], acc[b]);
-  }
-#pragma unroll
-  for (int b = 0; b < SLAB; b++)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc[b] += __shfl_xor_sync(0xffffffffu, acc[b], o);
 }
 
 // full[b][R] <- the slices [b][U] of all CTAs of the cluster

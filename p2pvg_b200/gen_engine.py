@@ -1,4 +1,8 @@
-"""Graph-captured point-to-point generation for the dcgan backbones (reference models/p2p_model.py:80-183).
+"""Graph-captured point-to-point generation for the dcgan and h36m_mlp backbones (reference models/p2p_model.py:80-183).
+
+The recurrent part and all host logic below are shared; the backbone-specific parts (weight preparation, encode, skip
+halves, decode, the frame shape) are methods that ``PoseGenerateEngine`` (at the end of this file) overrides: there every
+encoder and decoder call is one p2pvg_pose_mlp launch, so an executed autoregressive step is at most four launches.
 
 ``GenerateEngine`` computes what ``infer.p2p_generate`` / ``infer.p2p_generate_samples`` compute, with every call one
 replay of a CUDA graph captured per signature (rows, sequence lengths, executed steps, model_mode, n_past,
@@ -64,7 +68,23 @@ def check_supported(model):
     """ValueError unless the model is a dcgan_64 / dcgan_128 P2PModel with every module in eval mode."""
     from .models.backbone import DcganDecoder, DcganEncoder
     if getattr(model, "is_pose", False) or not isinstance(model.encoder, DcganEncoder) or not isinstance(model.decoder, DcganDecoder):
-        raise ValueError("p2p_generate_graphed supports the dcgan_64 / dcgan_128 backbones only; use p2p_generate for this model")
+        raise ValueError("p2p_generate_graphed supports the dcgan_64 / dcgan_128 and h36m_mlp backbones only; use p2p_generate for "
+                         "this model")
+    _check_eval(model)
+
+
+def check_supported_pose(model):
+    """ValueError unless the model is an h36m_mlp P2PModel in eval mode whose LSTMs p2pvg_lstm_step runs."""
+    from .models.h36m_mlp import decoder, encoder
+    if not getattr(model, "is_pose", False) or not isinstance(model.encoder, encoder) or not isinstance(model.decoder, decoder):
+        raise ValueError("PoseGenerateEngine runs the h36m_mlp backbone only; use p2p_generate for this model")
+    _check_eval(model)
+    R = int(model.rnn_size)
+    if not (64 <= R <= 512 and R % 8 == 0):
+        raise ValueError(f"p2p_generate_graphed runs rnn_size 64..512 in multiples of 8 (got {R}); use p2p_generate")
+
+
+def _check_eval(model):
     for m in ("encoder", "decoder", "frame_predictor", "posterior", "prior"):
         if any(mod.training for mod in getattr(model, m).modules()):
             raise ValueError(f"p2p_generate_graphed needs every module in eval mode ({m} is in training mode); "
@@ -88,8 +108,8 @@ class GenerateEngine:
     def generate(self, x, len_output, eval_cp_ix, model_mode="full", skip_frame=False, init_hidden=True, nsample=1):
         from . import infer
         model = self.model
-        check_supported(model)
-        if isinstance(x, tuple):
+        self._check_model()
+        if isinstance(x, tuple):   # h36m: (pose_2d, pose_3d, camera_view) -> pose_3d (models/p2p_model.py:96-103)
             x = x[1]
         if model_mode not in ("full", "posterior", "prior"):
             raise ValueError(f"unknown model_mode {model_mode!r}")
@@ -97,10 +117,8 @@ class GenerateEngine:
             raise ValueError("nsample must be >= 1")
         opt = model.opt
         T = len(x)
-        B, C, H, W = (int(v) for v in x[0].shape)
-        if H != model.encoder.image_width or W != H or C != model.encoder.nc:
-            raise ValueError(f"frames of shape {tuple(x[0].shape)} do not fit the {model.encoder.image_width}-pixel, "
-                             f"{model.encoder.nc}-channel backbone")
+        fshape = self._frame_shape(x[0])
+        B = int(x[0].shape[0])
         n_past = int(opt.n_past)
         if n_past < 1 or T < min(n_past, len_output):
             raise ValueError("p2p_generate_graphed needs n_past >= 1 and at least min(n_past, len_output) input frames")
@@ -114,14 +132,14 @@ class GenerateEngine:
         adt = infer._act_dtype()
         K = infer.kernels_for(dev)
         ptrs = tuple(p.data_ptr() for p in model.parameters()) + tuple(b.data_ptr() for b in model.buffers())
-        sig = (rows, B, T, C, H, len_output, S, model_mode, n_past, lfs, str(adt), ptrs)
+        sig = (rows, B, T, fshape, len_output, S, model_mode, n_past, lfs, str(adt), ptrs)
         G = self._graphs.get(sig)
         if G is not None and G.ws_gen != K.ws_gen:
             del self._graphs[sig]
             G = None
         n_tf = min(n_past - 1, len_output - 1)
-        cfg = dict(rows=rows, B=B, T=T, C=C, W=H, S=S, n_tf=n_tf, mode=model_mode, n_past=n_past, lfs=lfs, adt=adt,
-                   ns=nsample, dev=dev)
+        cfg = dict(rows=rows, B=B, T=T, fshape=fshape, C=fshape[0], W=fshape[-1], S=S, n_tf=n_tf, mode=model_mode, n_past=n_past,
+                   lfs=lfs, adt=adt, ns=nsample, dev=dev)
         if not init_hidden:
             for m in ("posterior", "prior", "frame_predictor"):
                 mod = getattr(model, m)
@@ -191,7 +209,7 @@ class GenerateEngine:
                 frames.append(out[j])
                 j += 1
         seq = [x[0]] + frames
-        zeros = torch.zeros((rows, C, H, W), device=dev, dtype=x[0].dtype)
+        zeros = torch.zeros((rows, *fshape), device=dev, dtype=x[0].dtype)
         if nsample == 1:
             return [f if f is not None else zeros.clone() for f in seq]
         res = [[] for _ in range(nsample)]
@@ -203,6 +221,17 @@ class GenerateEngine:
             for s in range(nsample):
                 res[s].append(f[s * B:(s + 1) * B])
         return res
+
+    # ------------------------------------------------------------------ backbone hooks
+    def _check_model(self):
+        check_supported(self.model)
+
+    def _frame_shape(self, f):
+        """The per-row shape of an input frame; ValueError when the backbone cannot take it."""
+        enc = self.model.encoder
+        if f.dim() != 4 or tuple(f.shape[1:]) != (enc.nc, enc.image_width, enc.image_width):
+            raise ValueError(f"frames of shape {tuple(f.shape)} do not fit the {enc.image_width}-pixel, {enc.nc}-channel backbone")
+        return tuple(int(v) for v in f.shape[1:])
 
     def memory_bytes(self):
         """Device memory held by the cached graphs' buffers (the graphs' private pools come on top)."""
@@ -217,12 +246,12 @@ class GenerateEngine:
         c, model = G.cfg, self.model
         dev, S, rows = c["dev"], c["S"], c["rows"]
         b = G.bufs
-        b["x"] = torch.zeros(c["T"] * c["B"], c["C"], c["W"] * c["W"], device=dev)
+        b["x"] = torch.zeros(c["T"] * c["B"], *c["fshape"], device=dev)
         b["tab_int"] = torch.zeros(3 * S + 1, dtype=torch.int32, device=dev)
         b["tab_f"] = torch.zeros(max(2 * S, 1), device=dev)
         b["eps"] = torch.zeros(max(S, 1), 2, rows, model.z_dim, device=dev)
         n_dec = max(S - c["n_tf"], 0)
-        b["out"] = torch.zeros(max(n_dec, 1), rows, c["C"], c["W"], c["W"], device=dev)[:n_dec]
+        b["out"] = torch.zeros(max(n_dec, 1), rows, *c["fshape"], device=dev)[:n_dec]
         for m in ("posterior", "prior", "frame_predictor"):
             mod = getattr(model, m)
             for k in ("h", "c"):
@@ -241,22 +270,17 @@ class GenerateEngine:
         c, model = G.cfg, self.model
         K = infer.kernels_for(c["dev"])
         self.K, self.G = K, G
-        adt, rows, B, T, S, n_tf = c["adt"], c["rows"], c["B"], c["T"], c["S"], c["n_tf"]
+        rows, B, T, S, n_tf = c["rows"], c["B"], c["T"], c["S"], c["n_tf"]
         g, z = model.g_dim, model.z_dim
-        self.chans = infer._stages(model.encoder)
         self._prepare_weights()
         # ground truth: one time-batched encode at B rows, tiled to the nsample*B rows of the recurrent part
         N = T * B
-        hw, nc, W = c["W"] * c["W"], c["C"], c["W"]
-        a = self._buf(G, "gt_in", N * hw * nc, adt)
-        nchw_to_nhwc(K, G.bufs["x"], a, N, hw, nc)
         h_gt = self._buf(G, "gt_h", N * g)
-        gt_skips = self._encode("gt", a, N, h_gt)
+        gt_skips = self._encode("gt", G.bufs["x"], N, h_gt)
         Hsrc = self._buf(G, "Hsrc", (T + 1) * rows * g)     # [T + 1][rows][g]: ground truth frames, then this step's h
         K.permute4(h_gt, Hsrc, (T, c["ns"], B * g, 1), (B * g, 0, 1, 0))
         h_cur = Hsrc[T * rows * g:]
-        gsrc_b = self._buf(G, "grp_zero", max(c["ns"], 1), torch.int32)   # source image n % B for every sample
-        n = len(self.chans)
+        self._buf(G, "grp_zero", max(c["ns"], 1), torch.int32)   # source image n % B for every sample
 
         def gt_skip(f):
             return [s[f * B * s.numel() // N:(f + 1) * B * s.numel() // N] for s in gt_skips]
@@ -273,9 +297,7 @@ class GenerateEngine:
             tuc, dt = tf[s:s + 1], tf[S + s:S + s + 1]
             skips_cur = None
             if s > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
-                xin = self._buf(G, "step_in", rows * hw * nc, adt)
-                nchw_to_nhwc(K, prev_frame, xin, rows, hw, nc)
-                skips_cur = self._encode("step", xin, rows, h_cur)
+                skips_cur = self._encode("step", prev_frame, rows, h_cur)
             glob = ti[3 * S:3 * S + 1]
             # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
             K.lstm_step([self._module("posterior", Hsrc, ti[s:s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 0], out=zbuf[:rows * z]),
@@ -293,9 +315,11 @@ class GenerateEngine:
 
     # ------------------------------------------------------------------ weights
     def _prepare_weights(self):
+        from . import infer
         K, G, model = self.K, self.G, self.model
         adt = G.cfg["adt"]
         enc, dec = model.encoder, model.decoder
+        self.chans = infer._stages(enc)
         chans, n, g = self.chans, len(self.chans), model.g_dim
         self.wp, self.bn = {}, {}
 
@@ -335,12 +359,14 @@ class GenerateEngine:
                 coeffs(f"dec{k}", blk.main[1])
 
     # ------------------------------------------------------------------ encoder / decoder
-    def _encode(self, tag, a, N, h_out):
-        """a: NHWC frames [N, W, W, nc] in the activation dtype -> h_out fp32 [N, g]; returns the skip maps (NHWC)."""
+    def _encode(self, tag, frames, N, h_out):
+        """frames: fp32 NCHW [N, nc, W, W] -> h_out fp32 [N, g]; returns the skip maps (NHWC)."""
         K, G, model = self.K, self.G, self.model
         adt = G.cfg["adt"]
         enc = model.encoder
         H, cin = G.cfg["W"], enc.nc
+        a = self._buf(G, f"{tag}_in", N * H * H * cin, adt)
+        nchw_to_nhwc(K, frames, a, N, H * H, cin)
         skips = []
         for l, cout in enumerate(self.chans):
             conv = getattr(enc, f"c{l + 1}").main[0]
@@ -465,3 +491,35 @@ class GenerateEngine:
         else:
             d.update(head=LSTM_HEAD_LINEAR_TANH, out_dim=mod.output_size, w_out=mod.output[0].weight, b_out=mod.output[0].bias)
         return d
+
+
+class PoseGenerateEngine(GenerateEngine):
+    """p2p_generate_graphed for the h36m_mlp pose backbone (models/h36m_mlp.py): the planner, tables, eps, LSTM state and
+    output assembly of GenerateEngine; every encoder and decoder call is ONE p2pvg_pose_mlp launch reading the live
+    parameters (exact fp32 in both P2PVG_PRECISION modes, as the eager pose path).  The ground-truth encode keeps its skips
+    h1 / h2 at B rows; the decoder reads skip row r % B for output row r."""
+
+    def _check_model(self):
+        check_supported_pose(self.model)
+
+    def _frame_shape(self, f):
+        if f.dim() != 3 or tuple(f.shape[1:]) != (17, 3):
+            raise ValueError(f"p2p_generate_graphed takes [B, 17, 3] poses for the h36m_mlp backbone (got frames of shape "
+                             f"{tuple(f.shape)}); use p2p_generate")
+        return (17, 3)
+
+    def _prepare_weights(self):
+        pass   # the kernel reads the parameters in place; their addresses are part of the graph's signature
+
+    def _encode(self, tag, frames, N, h_out):
+        G, g = self.G, self.model.g_dim
+        h1, h2 = self._buf(G, f"{tag}_h1", N * g), self._buf(G, f"{tag}_h2", N * g)
+        self.K.pose_mlp(self.model.encoder, False, frames, h_out, N, h1=h1, h2=h2)
+        return [h1, h2]
+
+    def _skip_halves(self, tag, skips, nsrc):
+        return skips, nsrc
+
+    def _decode(self, h_pred, halves, frame_out):
+        skips, nsrc = halves
+        self.K.pose_mlp(self.model.decoder, True, h_pred, frame_out, self.G.cfg["rows"], skips=skips, nsrc=nsrc)

@@ -197,10 +197,11 @@ class P2PModel(nn.Module):
 
     def p2p_generate_graphed(self, x, len_output, eval_cp_ix, model_mode='full', skip_frame=False, init_hidden=True, nsample=1):
         """p2p_generate (nsample=1) or p2p_generate_samples (nsample>1) as one CUDA-graph replay per call (an addition to the
-        reference API; see gen_engine.py).  dcgan_64 / dcgan_128 in eval mode only: anything else raises ValueError."""
-        from ..gen_engine import GenerateEngine
+        reference API; see gen_engine.py).  dcgan_64 / dcgan_128 and h36m_mlp in eval mode only: anything else raises
+        ValueError.  Pose input: the (pose_2d, pose_3d, camera_view) tuple, a [T, B, 17, 3] tensor or a list of [B, 17, 3]."""
+        from ..gen_engine import GenerateEngine, PoseGenerateEngine
         if getattr(self, "_gen_engine", None) is None:
-            self._gen_engine = GenerateEngine(self)
+            self._gen_engine = (PoseGenerateEngine if self.is_pose else GenerateEngine)(self)
         return self._gen_engine.generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
                                          init_hidden=init_hidden, nsample=nsample)
 

@@ -6,6 +6,10 @@ callers make (dcgan backbones, eval-mode BatchNorm, randomly initialised weights
   (b) misc/visualize.py:135    dcgan_64,  C=1, B=100, 30 frames, 20 samples  eager: 20 looped calls and p2p_generate_samples
                                                                              graphed: 20 looped calls and nsample=20
   (c)                          dcgan_128, C=3, B=64,  30 frames, 1 sample
+  (d) misc/visualize.py:135    h36m_mlp, rnn_size 512, B=10, 30 frames, 20 samples   (as (b))
+  (e) generate.py:115-116      h36m_mlp, rnn_size 512, B=1,  30 frames, 5 samples    (as (a))
+
+The pose workloads (d) / (e) run exact fp32 in both P2PVG_PRECISION modes and use the fp32 parity bound.
 
 Eager and graphed calls alternate; every time is a host clock around calls that end in a device synchronise (median of
 --reps).  Before timing, each pair of paths is fed the same eps draws and compared at the timed size.  Prints the card
@@ -24,10 +28,12 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from p2pvg_b200.infer import eps_stream  # noqa: E402
-from p2pvg_b200.models import dcgan_64, dcgan_128  # noqa: E402
+from p2pvg_b200.models import dcgan_64, dcgan_128, h36m_mlp  # noqa: E402
 from p2pvg_b200.models.p2p_model import P2PModel  # noqa: E402
 
-TOL = {"fp32": (2e-4, 2e-5), "bf16": (4e-2, 6e-3)}
+TOL = {"fp32": (2e-4, 2e-5), "bf16": (4e-2, 6e-3), "pose": (3e-4, 3e-5)}
+WORKLOADS = (("a_generate_py", 64, 1, 1, 5), ("b_vis_seq", 64, 1, 100, 20), ("c_d128_rgb", 128, 3, 64, 1),
+             ("d_pose_vis_seq", "pose", 0, 10, 20), ("e_pose_generate_py", "pose", 0, 1, 5))
 
 
 def card():
@@ -37,11 +43,12 @@ def card():
 
 
 def make_model(width, C, B):
-    net = dcgan_64 if width == 64 else dcgan_128
-    opt = types.SimpleNamespace(dataset="mnist", backbone_net=net, lr=1e-3, beta1=0.9, beta=1e-4, weight_cpc=100.0,
-                                weight_align=0.5, skip_prob=0.5, n_past=1, last_frame_skip=False, batch_size=B)
+    pose = width == "pose"
+    net = h36m_mlp if pose else dcgan_64 if width == 64 else dcgan_128
+    opt = types.SimpleNamespace(dataset="h36m" if pose else "mnist", backbone_net=net, lr=1e-3, beta1=0.9, beta=1e-4,
+                                weight_cpc=100.0, weight_align=0.5, skip_prob=0.5, n_past=1, last_frame_skip=False, batch_size=B)
     torch.manual_seed(1)
-    return P2PModel(B, C, 128, 10, 256, 1, 1, 2, opt=opt).cuda().eval()
+    return P2PModel(B, max(C, 1), 128, 10, 512 if pose else 256, 1, 1, 2, opt=opt).cuda().eval()
 
 
 def timed(fn, reps):
@@ -80,6 +87,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    ap.add_argument("--only", default="abcde", help="workload letters to run")
     args = ap.parse_args()
     prec = os.environ.get("P2PVG_PRECISION", "bf16")
     info = card()
@@ -87,9 +95,16 @@ def main():
     T = L = 30
     cp = L - 1
     lines = []
-    for name, width, C, B, ns in (("a_generate_py", 64, 1, 1, 5), ("b_vis_seq", 64, 1, 100, 20), ("c_d128_rgb", 128, 3, 64, 1)):
+    for name, width, C, B, ns in WORKLOADS:
+        if name[0] not in args.only:
+            continue
         model = make_model(width, C, B)
-        x = torch.rand(T, B, C, width, width, device="cuda", generator=torch.Generator(device="cuda").manual_seed(2))
+        gen = torch.Generator(device="cuda").manual_seed(2)
+        if width == "pose":   # poses standardised to std 3 (the h36m loader)
+            x = 3 * torch.randn(T, B, 17, 3, device="cuda", generator=gen)
+        else:
+            x = torch.rand(T, B, C, width, width, device="cuda", generator=gen)
+        tol = "pose" if width == "pose" else prec
         xs = list(x)
         steps = L - 1   # skip_frame=False: every step executes
         variants = {
@@ -100,10 +115,10 @@ def main():
             variants["eager_samples"] = lambda: model.p2p_generate_samples(xs, ns, L, cp)
             variants["graphed_nsample"] = lambda: model.p2p_generate_graphed(xs, L, cp, nsample=ns)
         parity = {"looped_call": check(lambda: model.p2p_generate(xs, L, cp), lambda: model.p2p_generate_graphed(xs, L, cp),
-                                       B, steps, prec)}
+                                       B, steps, tol)}
         if ns > 1:
             parity["nsample"] = check(lambda: model.p2p_generate_samples(xs, ns, L, cp),
-                                      lambda: model.p2p_generate_graphed(xs, L, cp, nsample=ns), ns * B, steps, prec)
+                                      lambda: model.p2p_generate_graphed(xs, L, cp, nsample=ns), ns * B, steps, tol)
         for fn in variants.values():   # warm-up: module loads, graph capture
             fn()
         times = {k: [] for k in variants}
