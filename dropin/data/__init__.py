@@ -1,5 +1,5 @@
-"""Shadow of the reference's ``data`` package: ``data.data_utils`` comes from here (Moving MNIST, Weizmann and BAIR batches
-made on the GPU), every other submodule (``data.moving_mnist``, ``data.weizmann``, ``data.bair``, ...) keeps resolving to the
+"""Shadow of the reference's ``data`` package: ``data.data_utils`` comes from here (Moving MNIST, Weizmann, BAIR and
+Human3.6M batches made on the GPU), every other submodule (``data.moving_mnist``, ``data.weizmann``, ``data.bair``, ...) keeps resolving to the
 reference checkout named by $P2PVG_REF (or any later ``data`` directory on sys.path)."""
 import os
 import sys

@@ -376,6 +376,24 @@ int p2pvg_video_windows(const uint8_t* frames, const int64_t* clip_first, const 
                         const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H, int W,
                         float* out, void* stream);
 
+/* Human3.6M training batches gathered from device-resident pose stores: the windows Human36mDataset.__getitem__
+ * (data/human36m/human36m.py:67-107, constant-speed branch) returns, time-major and truncated to T frames, for both outputs in
+ * one launch.
+ *   pose2d     [F][J][2] fp32, pose3d [F][J][3] fp32: sequence s is frames seq_first[s] .. seq_first[s] + seq_len[s) of both
+ *   entries    [B] int32: the sequence of batch row b
+ *   draws      [2][B] int32: row b starts at start = (unsigned)draws[b] % (seq_len[e] - speed_hi * L + 1) and steps by
+ *              speed = speed_lo + (unsigned)draws[B + b] % (speed_hi - speed_lo + 1), i.e. the reference's
+ *              np.random.randint(lo, hi) calls as lo + r % (hi - lo)
+ *   out2d      [T][B][J][2] fp32, out3d [T][B][J][3] fp32: out[t, b] = pose[seq_first[e] + start + t * speed], a copy of the
+ *              store's values.  T <= L: the first T frames of the L-frame window.
+ * Precondition (not checked on the device): every entry lies in [0, n_seq) and every sequence an entry names has
+ * seq_len >= speed_hi * L; p2pvg_b200.data.PoseClips and PoseBatches build stores, entries and draws that way.
+ * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers (fp32 / int32 4-byte, seq_first 8-byte), n_seq < 1, J < 1, B < 0, T < 0,
+ * T > L, L < 1, speed_lo < 1, speed_lo > speed_hi.  P2PVG_ERR_UNSUPPORTED: speed_hi * L >= 2^31 or T * B * J * 5 >= 2^31. */
+int p2pvg_pose_windows(const float* pose2d, const float* pose3d, int J, const int64_t* seq_first, const int32_t* seq_len, int n_seq,
+                       const int32_t* entries, const int32_t* draws, int B, int speed_lo, int speed_hi, int L, int T, float* out2d,
+                       float* out3d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

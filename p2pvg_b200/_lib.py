@@ -432,3 +432,17 @@ class CudaKernels:
         self._ck(self.lib.p2pvg_video_windows(_p(frames), _p(clip_first), _p(clip_len), _i(len(clip_len)), _p(entries), _p(draws),
                                               _i(int(paired_flips)), _i(B), _i(L), _i(T), _i(C), _i(H), _i(W), _p(out),
                                               self._stream()))
+
+    def pose_windows(self, pose_2d, pose_3d, seq_first, seq_len, entries, draws, speed_range, L, out_2d, out_3d):
+        """pose_2d fp32 [F,J,2], pose_3d fp32 [F,J,3], seq_first int64 / seq_len int32 [n_seq], entries int32 [B], draws int32
+        [2,B], out_2d fp32 [T,B,J,2], out_3d fp32 [T,B,J,3] (p2pvg_pose_windows)."""
+        assert pose_2d.dtype == pose_3d.dtype == out_2d.dtype == out_3d.dtype == torch.float32
+        assert seq_first.dtype == torch.int64 and seq_len.dtype == entries.dtype == draws.dtype == torch.int32
+        assert all(t.is_contiguous() for t in (pose_2d, pose_3d, seq_first, seq_len, entries, draws, out_2d, out_3d))
+        T, B, J, _ = out_2d.shape
+        F = pose_2d.shape[0]
+        assert tuple(pose_2d.shape) == (F, J, 2) and tuple(pose_3d.shape) == (F, J, 3) and tuple(out_3d.shape) == (T, B, J, 3)
+        assert len(seq_len) == len(seq_first) and len(entries) == B and tuple(draws.shape) == (2, B)
+        self._ck(self.lib.p2pvg_pose_windows(_p(pose_2d), _p(pose_3d), _i(J), _p(seq_first), _p(seq_len), _i(len(seq_len)),
+                                             _p(entries), _p(draws), _i(B), _i(speed_range[0]), _i(speed_range[1]), _i(L), _i(T),
+                                             _p(out_2d), _p(out_3d), self._stream()))

@@ -102,6 +102,8 @@ int p2pvg_scale_impl(float*, long long, float, cudaStream_t);
 int p2pvg_moving_mnist_impl(const uint8_t*, int, const int32_t*, int, float*, int, int, int, int, int, cudaStream_t);
 int p2pvg_video_windows_impl(const uint8_t*, const int64_t*, const int32_t*, int, const int32_t*, const int32_t*, int, int, int, int,
                              int, int, int, float*, cudaStream_t);
+int p2pvg_pose_windows_impl(const float*, const float*, int, const int64_t*, const int32_t*, int, const int32_t*, const int32_t*, int, int,
+                            int, int, int, float*, float*, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -335,6 +337,12 @@ int p2pvg_video_windows(const uint8_t* frames, const int64_t* clip_first, const 
                         const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H, int W,
                         float* out, void* stream) {
   return p2pvg_video_windows_impl(frames, clip_first, clip_len, n_clips, entries, draws, paired_flips, B, L, T, C, H, W, out, ST);
+}
+int p2pvg_pose_windows(const float* pose2d, const float* pose3d, int J, const int64_t* seq_first, const int32_t* seq_len, int n_seq,
+                       const int32_t* entries, const int32_t* draws, int B, int speed_lo, int speed_hi, int L, int T, float* out2d,
+                       float* out3d, void* stream) {
+  return p2pvg_pose_windows_impl(pose2d, pose3d, J, seq_first, seq_len, n_seq, entries, draws, B, speed_lo, speed_hi, L, T, out2d,
+                                 out3d, ST);
 }
 
 }  // extern "C"

@@ -19,6 +19,12 @@ Weizmann and BAIR are decoded once into a uint8 clip store on the device (``load
 
     for x in ClipBatches(load_weizmann_clips(root, True, 18, 64), 128, "permutation", seq_len=(10, 18)):
         losses = model(x, 0, len(x) - 1)
+
+Human3.6M poses are uploaded once from the reference dataset's own normalised lists into fp32 stores on the device
+(``PoseClips``); ``PoseBatches`` then gathers both outputs of every batch with one ``p2pvg_pose_windows`` launch.
+
+    for x in PoseBatches(PoseClips(d["pose"]["2d"], d["pose"]["3d"], d["camera_view"], 30, 6), 256, (20, 30), (6, 6)):
+        losses = model(x, 0, len(x[1]) - 1)
 """
 from __future__ import annotations
 
@@ -198,6 +204,33 @@ BAIR_EPOCH_ITEMS = 10000
 SAMPLING = ("permutation", "uniform", "ordered")
 
 
+class _EpochBatches:
+    """What the device batch iterators share with the reference's loop (data/data_utils.py:94-137): per batch,
+    ``T = np.random.randint(lo, hi + 1)`` from NumPy's global stream, where the generator calls ``get_seq_len()``; epochs of
+    ``epoch_items // batch_size`` batches (drop_last), ``k`` the batch within the current epoch."""
+
+    def __init__(self, batch_size, seq_len, max_seq_len, epoch_items):
+        lo, hi = (int(v) for v in seq_len)
+        if not 1 <= lo <= hi <= max_seq_len:
+            raise ValueError(f"seq_len = ({lo}, {hi}): needs 1 <= lo <= hi <= max_seq_len = {max_seq_len}")
+        B = int(batch_size)
+        if B < 1:
+            raise ValueError(f"batch_size = {B}")
+        if epoch_items // B == 0:
+            raise ValueError(f"batch_size = {B} exceeds the {epoch_items} items of an epoch: the reference's drop_last loader "
+                             "would yield no batch")
+        self.batch_size, self.seq_len, self.epoch_batches, self.k = B, (lo, hi), epoch_items // B, 0
+
+    def __iter__(self):
+        return self
+
+    def _draw_seq_len(self):
+        return int(np.random.randint(self.seq_len[0], self.seq_len[1] + 1))
+
+    def _advance(self):
+        self.k = (self.k + 1) % self.epoch_batches
+
+
 def ordered_schedule(n_entries, batch_size, epoch_items=BAIR_EPOCH_ITEMS):
     """The entries of one epoch of ``ordered`` sampling, batch after batch (int64 [epoch_items // batch_size * batch_size]).
     ``BairRobotPush.get_seq`` walks its trajectories in order and wraps at the end, whatever index it is asked for; each epoch
@@ -205,7 +238,7 @@ def ordered_schedule(n_entries, batch_size, epoch_items=BAIR_EPOCH_ITEMS):
     return torch.arange(epoch_items // batch_size * batch_size) % n_entries
 
 
-class ClipBatches:
+class ClipBatches(_EpochBatches):
     """Endless iterator of fp32 [T, B, 3, S, S] device batches cut from ``clips`` (``p2pvg_video_windows``), time-major like
     the reference's ``get_generator`` after ``.permute(1, 0, 2, 3, 4).cuda()[:seq_len]`` (data/data_utils.py:112-122).
 
@@ -223,30 +256,20 @@ class ClipBatches:
         from ._lib import kernels_for
         if sampling not in SAMPLING:
             raise ValueError(f"sampling = {sampling!r}, expected one of {SAMPLING}")
-        lo, hi = (int(v) for v in seq_len)
-        if not 1 <= lo <= hi <= clips.max_seq_len:
-            raise ValueError(f"seq_len = ({lo}, {hi}): needs 1 <= lo <= hi <= max_seq_len = {clips.max_seq_len}")
-        B, n = int(batch_size), len(clips)
-        if B < 1:
-            raise ValueError(f"batch_size = {B}")
-        epoch = {"permutation": n, "uniform": B, "ordered": BAIR_EPOCH_ITEMS}[sampling] // B
-        if epoch == 0:
-            raise ValueError(f"batch_size = {B} exceeds the {n if sampling == 'permutation' else BAIR_EPOCH_ITEMS} items of an "
-                             "epoch: the reference's drop_last loader would yield no batch")
+        n = len(clips)
+        # a uniform "epoch" is one batch: nothing is drawn per epoch
+        items = {"permutation": n, "uniform": int(batch_size), "ordered": BAIR_EPOCH_ITEMS}[sampling]
+        super().__init__(batch_size, seq_len, clips.max_seq_len, items)
         self.K = kernels_for(device)
         self.device = self.K.device
         self.clips = clips.to(self.device)
-        self.batch_size, self.sampling, self.seq_len, self.generator = B, sampling, (lo, hi), generator
-        self.epoch_batches, self.k = epoch, 0
+        self.sampling, self.generator = sampling, generator
         self.order = None
         if sampling == "ordered":
-            self.order = ordered_schedule(n, B).to(self.device, torch.int32)
-
-    def __iter__(self):
-        return self
+            self.order = ordered_schedule(n, self.batch_size).to(self.device, torch.int32)
 
     def __next__(self):
-        T = int(np.random.randint(self.seq_len[0], self.seq_len[1] + 1))
+        T = self._draw_seq_len()
         B, k, c = self.batch_size, self.k, self.clips
         with torch.cuda.device(self.device):
             draws = None
@@ -260,8 +283,115 @@ class ClipBatches:
                 entries = self.order[k * B:(k + 1) * B]
             out = torch.empty((T, B) + tuple(c.frames.shape[1:]), dtype=torch.float32, device=self.device)
             self.K.video_windows(c.frames, c.clip_first, c.clip_len, entries, draws, c.paired_flips, c.max_seq_len, out)
-        self.k = (k + 1) % self.epoch_batches
+        self._advance()
         return out
+
+
+def _check_pose_lengths(lengths, need):
+    short = next((e for e, n in enumerate(lengths) if n < need), None)
+    if short is not None:
+        raise ValueError(f"entry {short}: {lengths[short]} frames, fewer than speed_hi * max_seq_len = {need}: the reference "
+                         "would raise from np.random.randint when it draws this entry")
+
+
+class PoseClips:
+    """Human3.6M pose sequences held on the device: ``pose_2d`` fp32 [F, J, 2] and ``pose_3d`` fp32 [F, J, 3]; entry e is
+    frames ``seq_first[e] .. seq_first[e] + seq_len[e]`` of both (``lengths``: the same lengths on the host).
+    ``camera_view`` (CPU int64) is the dataset's camera-view list, and entry e reports ``camera_view[e]``. ``max_seq_len`` is
+    the window length L.
+
+    Built from ``Human36mDataset``'s own normalised float64 lists ``data['pose']['2d' | '3d']`` and ``data['camera_view']``
+    (data/human36m/human36m.py:26-65) by a casting upload.  Each value is rounded to fp32 exactly as the reference's
+    ``.float()`` of its collated float64 batch rounds it.  The camera-view list is taken as the dataset holds it:
+    ``reformat_data`` appends [0, 1, 2, 3] per annotation but keeps one view of the poses, and the length filter does not
+    touch it, so it is longer than the entries, and ``__getitem__(e)`` reports its e-th value.
+
+    Raises ValueError naming the entry for arrays that are not [n, J, 2] / [n, J, 3] with one J, for 2d and 3d lengths that
+    differ, and for an entry shorter than ``speed_hi * max_seq_len``.  Known deviation: the reference accepts such a short
+    entry and raises from ``np.random.randint`` only when it draws it."""
+
+    def __init__(self, pose_2d, pose_3d, camera_view, max_seq_len, speed_hi=1, device="cuda"):
+        if len(pose_2d) != len(pose_3d):
+            raise ValueError(f"{len(pose_2d)} 2d entries but {len(pose_3d)} 3d entries")
+        if len(pose_2d) == 0:
+            raise ValueError("no pose entries")
+        if len(camera_view) < len(pose_2d):
+            raise ValueError(f"{len(camera_view)} camera views for {len(pose_2d)} entries")
+        pose_2d, pose_3d = [np.asarray(a) for a in pose_2d], [np.asarray(a) for a in pose_3d]
+        J = pose_2d[0].shape[1] if pose_2d[0].ndim == 3 else None
+        for e, (a, b) in enumerate(zip(pose_2d, pose_3d)):
+            if a.ndim != 3 or b.ndim != 3 or a.shape[1:] != (J, 2) or b.shape[1:] != (J, 3):
+                raise ValueError(f"entry {e}: pose arrays {a.shape} and {b.shape}, expected [n, {J}, 2] and [n, {J}, 3]")
+            if len(a) != len(b):
+                raise ValueError(f"entry {e}: {len(a)} 2d frames but {len(b)} 3d frames")
+        self.lengths = [len(a) for a in pose_2d]
+        _check_pose_lengths(self.lengths, int(speed_hi) * int(max_seq_len))
+        F = sum(self.lengths)
+        first = np.concatenate([[0], np.cumsum(self.lengths)[:-1]])
+        host_2d, host_3d = torch.empty(F, J, 2), torch.empty(F, J, 3)
+        for a, b, f, n in zip(pose_2d, pose_3d, first, self.lengths):
+            host_2d[f:f + n] = torch.from_numpy(np.ascontiguousarray(a))     # float64 -> fp32, round to nearest
+            host_3d[f:f + n] = torch.from_numpy(np.ascontiguousarray(b))
+        self.pose_2d, self.pose_3d = host_2d.to(device), host_3d.to(device)
+        self.seq_first = torch.tensor(first, dtype=torch.int64, device=device)
+        self.seq_len = torch.tensor(self.lengths, dtype=torch.int32, device=device)
+        self.camera_view = torch.as_tensor(np.asarray(camera_view), dtype=torch.int64)
+        self.max_seq_len = int(max_seq_len)
+
+    def __len__(self):
+        return len(self.lengths)
+
+    def to(self, device):
+        out = object.__new__(PoseClips)
+        out.__dict__.update(self.__dict__)
+        for k in ("pose_2d", "pose_3d", "seq_first", "seq_len"):
+            setattr(out, k, getattr(self, k).to(device))
+        return out
+
+
+class PoseBatches(_EpochBatches):
+    """Endless iterator of Human3.6M batches ``(pose_2d, pose_3d, camera_view)`` gathered from ``clips``
+    (``p2pvg_pose_windows``): fp32 [T, B, J, 2] and [T, B, J, 3] on the device, time-major, and the CPU int64 [B] camera views
+    of the rows' entries. This is what the reference's ``get_h36m_generator`` yields (data/data_utils.py:94-109).
+
+    Per batch, ``T = np.random.randint(lo, hi + 1)`` is drawn from NumPy's global stream where ``get_h36m_generator`` calls
+    ``get_seq_len()``.  The entries follow ``DataLoader(shuffle=True, drop_last=True)``: a fresh permutation every epoch of
+    ``len(clips) // B`` batches.  It is drawn on the host with torch's global CPU generator, from which the reference's
+    sampler also seeds itself once per epoch, and uploaded once per epoch, so the camera views are read on the host.  Each
+    row's window start and speed are drawn on the device from ``generator`` (a CUDA generator), in place of the reference's
+    worker-process NumPy stream: the same distributions, other values.  ``next()`` never waits for the device.  Only the
+    constant-speed crop is implemented: the breakpoint / acceleration branch of ``__getitem__`` is never enabled by
+    ``load_dataset``.  Each batch is a fresh pair of tensors, never written again."""
+
+    def __init__(self, clips, batch_size, seq_len, speed_range, device="cuda", generator=None):
+        from ._lib import kernels_for
+        lo, hi = (int(v) for v in speed_range)
+        if not 1 <= lo <= hi:
+            raise ValueError(f"speed_range = ({lo}, {hi}): needs 1 <= speed_lo <= speed_hi")
+        super().__init__(batch_size, seq_len, clips.max_seq_len, len(clips))
+        _check_pose_lengths(clips.lengths, hi * clips.max_seq_len)
+        self.K = kernels_for(device)
+        self.device = self.K.device
+        self.clips = clips.to(self.device)
+        self.speed_range, self.generator = (lo, hi), generator
+        self.order = self.order_host = None
+
+    def __next__(self):
+        T = self._draw_seq_len()
+        B, k, c = self.batch_size, self.k, self.clips
+        J = c.pose_2d.shape[1]
+        with torch.cuda.device(self.device):
+            if k == 0:
+                self.order_host = torch.randperm(len(c))[:self.epoch_batches * B]
+                self.order = self.order_host.to(torch.int32).pin_memory().to(self.device, non_blocking=True)
+            draws = torch.randint(0, 2 ** 31 - 1, (2, B), dtype=torch.int32, device=self.device, generator=self.generator)
+            out_2d = torch.empty((T, B, J, 2), dtype=torch.float32, device=self.device)
+            out_3d = torch.empty((T, B, J, 3), dtype=torch.float32, device=self.device)
+            self.K.pose_windows(c.pose_2d, c.pose_3d, c.seq_first, c.seq_len, self.order[k * B:(k + 1) * B], draws,
+                                self.speed_range, c.max_seq_len, out_2d, out_3d)
+        camera_view = c.camera_view[self.order_host[k * B:(k + 1) * B]]
+        self._advance()
+        return out_2d, out_3d, camera_view
 
 
 def _chain_front(first, rest):
