@@ -220,7 +220,7 @@ def alpha_for(K, tf32=False):
     return acc + (2.0 ** -9 if tf32 else 0.0)
 
 
-def assert_within(got, ref, absref, K, out_dtype, name="", locate=None, alpha=None):
+def assert_within(got, ref, absref, K, out_dtype, name="", locate=None, alpha=None, quiet=False):
     """|got - ref| <= alpha * absref + beta * |ref|: alpha covers the fp32 accumulation (alpha_for), beta the rounding of the
     stored output.  On failure: the worst ratio, its index and (via `locate(index) -> str`) its tile.  Returns the worst ratio."""
     a = alpha_for(K) if alpha is None else alpha
@@ -236,5 +236,6 @@ def assert_within(got, ref, absref, K, out_dtype, name="", locate=None, alpha=No
         where = locate(idx) if locate is not None else ""
         raise AssertionError(f"{name}: {bad}/{ratio.numel()} elements out of bound, worst ratio {worst:.3g} at {idx} "
                              f"(got {got[idx].item():.6g}, ref {ref[idx].item():.6g}, bound {bound[idx].item():.3g}) {where}")
-    print(f"[bound] {name}: worst error/bound {worst:.3g}")
+    if not quiet:
+        print(f"[bound] {name}: worst error/bound {worst:.3g}")
     return worst
