@@ -100,7 +100,7 @@ int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c
  *                     row block mt and phase ph is row mt*phases + ph; reduce per group with p2pvg_bn_fwd_finalize_tiles
  *                     (rows of one BatchNorm group must be a multiple of 128).
  *   addend_dtype      the skip-half addend may be stored in bf16 (it is the output of another p2pvg_conv_gemm call).
- *   eval_scale/shift  kinds 0 and 2: nn.BatchNorm2d in eval mode + activation applied in the epilogue (generation,
+ *   eval_scale/shift  kinds 0, 2 and 3: nn.BatchNorm2d in eval mode + activation applied in the epilogue (generation,
  *                     models/p2p_model.py:80-183 with running statistics): the stored output is
  *                     y = act(eval_scale[c] * (acc + bias[c] + addend) + eval_shift[c]), act = P2PVG_ACT_LRELU | P2PVG_ACT_TANH,
  *                     coefficients as p2pvg_bn_eval_coeffs writes them.  NULL: no such epilogue.  Not combinable with
@@ -128,6 +128,21 @@ int p2pvg_maxpool2_bwd(const void* x, const void* dy, void* dx, int dtype, int N
 int p2pvg_upsample2_fwd(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream);
 int p2pvg_upsample2_bwd(const void* dy, void* dx, int dtype, int N, int H, int W, int C, void* stream);
 int p2pvg_gather_add(void* dst, int dtype, const float* src, const int* grp_src, int G, int64_t n, void* stream);
+
+/* The two thin ends of the vgg stacks in eval mode (generation), each one launch on the CUDA cores.  Both read the fp32
+ * parameters in PyTorch's own layout, in place, and accumulate in fp32 FFMA in a fixed order (first: input channel, kh, kw;
+ * last: kh, kw, input channel); the activations are stored in `dtype` (f32 | bf16), rounded once.  nc = 1..4 image channels (else P2PVG_ERR_UNSUPPORTED).
+ *   vgg_first_eval: the first encoder layer vgg_layer(nc, 64) (models/vgg_64.py:22) with BatchNorm on running statistics:
+ *                   y[N,H,W,64] (NHWC) = LeakyReLU_0.2(scale[c] * (conv3x3_p1(x)[c] + bias[c]) + shift[c]) from fp32 NCHW frames
+ *                   x[N,nc,H,W]; w = Conv2d weight [64][nc][3][3], scale / shift as p2pvg_bn_eval_coeffs writes them.
+ *   vgg_last_eval:  the closing ConvTranspose2d(64, nc, 3, 1, 1) + Sigmoid (models/vgg_64.py:87-90):
+ *                   out[n,c,y,x] (fp32 NCHW) = sigmoid(bias[c] + sum_{ci,kh,kw} d[n, y+1-kh, x+1-kw, ci] * w[ci][c][kh][kw]) from
+ *                   d[N,H,W,64] (NHWC); w = ConvTranspose2d weight [64][nc][3][3].
+ * P2PVG_ERR_BAD_ARG: NULL pointers, N < 0, H or W < 1, a y / d base that is not 16-byte aligned. */
+int p2pvg_vgg_first_eval(const float* x, int nc, const float* w, const float* bias, const float* scale, const float* shift, void* y,
+                         int y_dtype, int N, int H, int W, void* stream);
+int p2pvg_vgg_last_eval(const void* d, int d_dtype, const float* w, const float* bias, float* out, int nc, int N, int H, int W,
+                        void* stream);
 
 /* 4x4 / stride 2 / pad 1 lowering (nn.Conv2d(nin,nout,4,2,1), models/dcgan_64.py:8; and the data-gradient of
  * nn.ConvTranspose2d(nin,nout,4,2,1), models/dcgan_64.py:20): x [N,H,W,C] -> col [N*H/2*W/2, 16*C], K order (kh,kw,c). */

@@ -203,7 +203,7 @@ class CudaKernels:
                   imgs_per_group=0, accumulate=False, stat_partial=None, eval_scale=None, eval_shift=None, act=ACT_NONE):
         """kind 0..5 of p2pvg_conv_gemm (see include/p2pvg_b200.h).  H, W: small-map size.  stat_partial: fp32 buffer of
         [tiles * phases, Cn, 2] receiving the BatchNorm forward statistics of the output (epilogue fusion).  eval_scale /
-        eval_shift (kinds 0, 2): eval-mode BatchNorm + `act` applied in the epilogue."""
+        eval_shift (kinds 0, 2, 3): eval-mode BatchNorm + `act` applied in the epilogue."""
         taps = 9 if kind >= 3 else 16
         if ldb is None:
             ldb = taps * Ck if kind in (0, 3, 5) else taps * Cn
@@ -248,6 +248,15 @@ class CudaKernels:
 
     def gather_add(self, dst, src, grp_src, G, n):
         self._ck(self.lib.p2pvg_gather_add(_p(dst), _i(_dt(dst)), _p(src), _p(grp_src), _i(G), _i64(n), self._stream()))
+
+    def vgg_first_eval(self, x, nc, w, bias, scale, shift, y, N, H, W):
+        """p2pvg_vgg_first_eval: fp32 NCHW frames x -> y[N,H,W,64] in y's dtype (first vgg layer, eval-mode BatchNorm)."""
+        self._ck(self.lib.p2pvg_vgg_first_eval(_p(x), _i(nc), _p(w), _p(bias), _p(scale), _p(shift), _p(y), _i(_dt(y)), _i(N), _i(H),
+                                               _i(W), self._stream()))
+
+    def vgg_last_eval(self, d, w, bias, out, nc, N, H, W):
+        """p2pvg_vgg_last_eval: d[N,H,W,64] -> fp32 NCHW frames out (closing ConvTranspose2d(64, nc, 3, 1, 1) + Sigmoid)."""
+        self._ck(self.lib.p2pvg_vgg_last_eval(_p(d), _i(_dt(d)), _p(w), _p(bias), _p(out), _i(nc), _i(N), _i(H), _i(W), self._stream()))
 
     def permute4(self, src, dst, dims, strides, accumulate=False):
         d = (_i * 4)(*dims)

@@ -50,6 +50,9 @@ int p2pvg_maxpool2_bwd_impl(const void*, const void*, void*, int, int, int, int,
 int p2pvg_upsample2_fwd_impl(const void*, void*, int, int, int, int, int, cudaStream_t);
 int p2pvg_upsample2_bwd_impl(const void*, void*, int, int, int, int, int, cudaStream_t);
 int p2pvg_gather_add_impl(void*, int, const float*, const int*, int, long long, cudaStream_t);
+int p2pvg_vgg_first_eval_impl(const float*, int, const float*, const float*, const float*, const float*, void*, int, int, int, int,
+                              cudaStream_t);
+int p2pvg_vgg_last_eval_impl(const void*, int, const float*, const float*, float*, int, int, int, int, cudaStream_t);
 int p2pvg_col2im_k4s2p1_impl(const void*, const void*, const int*, int, void*, int, int, int, int, int, const float*, int, cudaStream_t);
 int p2pvg_permute4_impl(const void*, int, void*, int, const int*, const long long*, int, cudaStream_t);
 int p2pvg_nchw_to_nhwc_dual_impl(const float*, float*, void*, int, long long, int, int, cudaStream_t);
@@ -197,6 +200,14 @@ int p2pvg_upsample2_bwd(const void* dy, void* dx, int dtype, int N, int H, int W
 }
 int p2pvg_gather_add(void* dst, int dtype, const float* src, const int* grp_src, int G, int64_t n, void* stream) {
   return p2pvg_gather_add_impl(dst, dtype, src, grp_src, G, n, ST);
+}
+int p2pvg_vgg_first_eval(const float* x, int nc, const float* w, const float* bias, const float* scale, const float* shift, void* y,
+                         int y_dtype, int N, int H, int W, void* stream) {
+  return p2pvg_vgg_first_eval_impl(x, nc, w, bias, scale, shift, y, y_dtype, N, H, W, ST);
+}
+int p2pvg_vgg_last_eval(const void* d, int d_dtype, const float* w, const float* bias, float* out, int nc, int N, int H, int W,
+                        void* stream) {
+  return p2pvg_vgg_last_eval_impl(d, d_dtype, w, bias, out, nc, N, H, W, ST);
 }
 int p2pvg_transpose_batched(const void* src, int src_dtype, void* dst, int dst_dtype, int A, int P, int Q, void* stream) {
   return p2pvg_transpose_batched_impl(src, src_dtype, dst, dst_dtype, A, P, Q, ST);

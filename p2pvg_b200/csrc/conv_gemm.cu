@@ -87,7 +87,8 @@ __device__ __forceinline__ void addend_add32(float (&f)[32], const float4 (&a4)[
   }
 }
 
-// EVAL: eval-mode BatchNorm + activation in the epilogue, y = act(eval_scale[c] * (acc + bias + addend) + eval_shift[c]) (kinds 0 / 2)
+// EVAL: eval-mode BatchNorm + activation in the epilogue, y = act(eval_scale[c] * (acc + bias + addend) + eval_shift[c]) (kinds 0 / 2;
+// kind 3 runs as kind 0)
 // BM = 256 (kind 2, BN = 64, no statistics or eval epilogue): 256-pixel tiles, twice the MMA work per filled K block
 template <int KIND, int BM, int BN, bool STAT, bool EVAL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -507,7 +508,7 @@ int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, 
   P2PVG_REQUIRE(driver().encode != nullptr, P2PVG_ERR_UNSUPPORTED, "conv_gemm: cuTensorMapEncodeTiled unavailable");
   P2PVG_REQUIRE(kind >= 0 && kind <= 5, P2PVG_ERR_BAD_ARG, "conv_gemm: bad kind %d", kind);
   if (eval_scale != nullptr) {
-    P2PVG_REQUIRE(kind == 0 || kind == 2, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue belongs to kinds 0 and 2");
+    P2PVG_REQUIRE(kind == 0 || kind == 2 || kind == 3, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue belongs to kinds 0, 2 and 3");
     P2PVG_REQUIRE(eval_shift != nullptr, P2PVG_ERR_BAD_ARG, "conv_gemm: eval_scale without eval_shift");
     P2PVG_REQUIRE(stat_partial == nullptr, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue excludes fwd_stat_partial");
     P2PVG_REQUIRE(!accumulate, P2PVG_ERR_BAD_ARG, "conv_gemm: the eval-BatchNorm epilogue does not accumulate");

@@ -1,8 +1,9 @@
-"""Graph-captured point-to-point generation for the dcgan and h36m_mlp backbones (reference models/p2p_model.py:80-183).
+"""Graph-captured point-to-point generation for the dcgan, vgg and h36m_mlp backbones (reference models/p2p_model.py:80-183).
 
-The recurrent part and all host logic below are shared; the backbone-specific parts (weight preparation, encode, skip
-halves, decode, the frame shape) are methods that ``PoseGenerateEngine`` (at the end of this file) overrides: there every
-encoder and decoder call is one p2pvg_pose_mlp launch, so an executed autoregressive step is at most four launches.
+The recurrent part and all host logic below are shared; the backbone-specific parts (model check, weight preparation,
+encode, skip halves, decode, the frame shape) are methods that ``PoseGenerateEngine`` (at the end of this file) and
+``gen_engine_vgg.VggGenerateEngine`` (vgg_64 / vgg_128) override.  For poses every encoder and decoder call is one
+p2pvg_pose_mlp launch, so an executed autoregressive step is at most four launches.
 
 ``GenerateEngine`` computes what ``infer.p2p_generate`` / ``infer.p2p_generate_samples`` compute, with every call one
 replay of a CUDA graph captured per signature (rows, sequence lengths, executed steps, model_mode, n_past,
@@ -68,8 +69,8 @@ def check_supported(model):
     """ValueError unless the model is a dcgan_64 / dcgan_128 P2PModel with every module in eval mode."""
     from .models.backbone import DcganDecoder, DcganEncoder
     if getattr(model, "is_pose", False) or not isinstance(model.encoder, DcganEncoder) or not isinstance(model.decoder, DcganDecoder):
-        raise ValueError("p2p_generate_graphed supports the dcgan_64 / dcgan_128 and h36m_mlp backbones only; use p2p_generate for "
-                         "this model")
+        raise ValueError("p2p_generate_graphed supports the dcgan_64 / dcgan_128, vgg_64 / vgg_128 and h36m_mlp backbones only; use "
+                         "p2p_generate for this model")
     _check_eval(model)
 
 

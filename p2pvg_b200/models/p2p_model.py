@@ -197,11 +197,15 @@ class P2PModel(nn.Module):
 
     def p2p_generate_graphed(self, x, len_output, eval_cp_ix, model_mode='full', skip_frame=False, init_hidden=True, nsample=1):
         """p2p_generate (nsample=1) or p2p_generate_samples (nsample>1) as one CUDA-graph replay per call (an addition to the
-        reference API; see gen_engine.py).  dcgan_64 / dcgan_128 and h36m_mlp in eval mode only: anything else raises
-        ValueError.  Pose input: the (pose_2d, pose_3d, camera_view) tuple, a [T, B, 17, 3] tensor or a list of [B, 17, 3]."""
+        reference API; see gen_engine.py and gen_engine_vgg.py).  dcgan_64 / dcgan_128, vgg_64 / vgg_128 (on a CUDA device)
+        and h36m_mlp in eval mode only: anything else raises ValueError.  Pose input: the (pose_2d, pose_3d, camera_view)
+        tuple, a [T, B, 17, 3] tensor or a list of [B, 17, 3]."""
         from ..gen_engine import GenerateEngine, PoseGenerateEngine
+        from ..gen_engine_vgg import VggGenerateEngine
+        from .vgg import VggEncoder
         if getattr(self, "_gen_engine", None) is None:
-            self._gen_engine = (PoseGenerateEngine if self.is_pose else GenerateEngine)(self)
+            cls = PoseGenerateEngine if self.is_pose else VggGenerateEngine if isinstance(self.encoder, VggEncoder) else GenerateEngine
+            self._gen_engine = cls(self)
         return self._gen_engine.generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
                                          init_hidden=init_hidden, nsample=nsample)
 

@@ -8,8 +8,12 @@ callers make (dcgan backbones, eval-mode BatchNorm, randomly initialised weights
   (c)                          dcgan_128, C=3, B=64,  30 frames, 1 sample
   (d) misc/visualize.py:135    h36m_mlp, rnn_size 512, B=10, 30 frames, 20 samples   (as (b))
   (e) generate.py:115-116      h36m_mlp, rnn_size 512, B=1,  30 frames, 5 samples    (as (a))
+  (f) generate.py:115-116      vgg_64,   C=3, B=1,   30 frames, 5 samples   (as (a))
+  (g) misc/visualize.py:135    vgg_64,   C=3, B=128, 30 frames, 20 samples  (as (b); the C3 training batch)
+  (h)                          vgg_128,  C=3, B=16,  30 frames, 1 sample
 
-The pose workloads (d) / (e) run exact fp32 in both P2PVG_PRECISION modes and use the fp32 parity bound.
+The pose workloads (d) / (e) run exact fp32 in both P2PVG_PRECISION modes and use the fp32 parity bound.  Each JSON line also gives the graph buffers' device memory (GenerateEngine.memory_bytes()) of
+one looped call's and one nsample call's signature, each cached alone.
 
 Eager and graphed calls alternate; every time is a host clock around calls that end in a device synchronise (median of
 --reps).  Before timing, each pair of paths is fed the same eps draws and compared at the timed size.  Prints the card
@@ -28,12 +32,14 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from p2pvg_b200.infer import eps_stream  # noqa: E402
-from p2pvg_b200.models import dcgan_64, dcgan_128, h36m_mlp  # noqa: E402
+from p2pvg_b200.models import dcgan_64, dcgan_128, h36m_mlp, vgg_64, vgg_128  # noqa: E402
 from p2pvg_b200.models.p2p_model import P2PModel  # noqa: E402
 
 TOL = {"fp32": (2e-4, 2e-5), "bf16": (4e-2, 6e-3), "pose": (3e-4, 3e-5)}
 WORKLOADS = (("a_generate_py", 64, 1, 1, 5), ("b_vis_seq", 64, 1, 100, 20), ("c_d128_rgb", 128, 3, 64, 1),
-             ("d_pose_vis_seq", "pose", 0, 10, 20), ("e_pose_generate_py", "pose", 0, 1, 5))
+             ("d_pose_vis_seq", "pose", 0, 10, 20), ("e_pose_generate_py", "pose", 0, 1, 5),
+             ("f_vgg64_generate_py", "vgg64", 3, 1, 5), ("g_vgg64_vis_seq", "vgg64", 3, 128, 20), ("h_vgg128_rgb", "vgg128", 3, 16, 1))
+SIDE = {"vgg64": 64, "vgg128": 128}
 
 
 def card():
@@ -44,7 +50,7 @@ def card():
 
 def make_model(width, C, B):
     pose = width == "pose"
-    net = h36m_mlp if pose else dcgan_64 if width == 64 else dcgan_128
+    net = h36m_mlp if pose else {64: dcgan_64, 128: dcgan_128, "vgg64": vgg_64, "vgg128": vgg_128}[width]
     opt = types.SimpleNamespace(dataset="h36m" if pose else "mnist", backbone_net=net, lr=1e-3, beta1=0.9, beta=1e-4,
                                 weight_cpc=100.0, weight_align=0.5, skip_prob=0.5, n_past=1, last_frame_skip=False, batch_size=B)
     torch.manual_seed(1)
@@ -103,7 +109,8 @@ def main():
         if width == "pose":   # poses standardised to std 3 (the h36m loader)
             x = 3 * torch.randn(T, B, 17, 3, device="cuda", generator=gen)
         else:
-            x = torch.rand(T, B, C, width, width, device="cuda", generator=gen)
+            side = SIDE.get(width, width)
+            x = torch.rand(T, B, C, side, side, device="cuda", generator=gen)
         tol = "pose" if width == "pose" else prec
         xs = list(x)
         steps = L - 1   # skip_frame=False: every step executes
@@ -125,9 +132,18 @@ def main():
         for _ in range(args.reps):     # alternate the paths
             for k, fn in variants.items():
                 times[k].append(timed(fn, 1))
+        eng = model._gen_engine
+        memory = {}
+        for k, fn in (("looped_call", lambda: model.p2p_generate_graphed(xs, L, cp)),
+                      ("nsample", lambda: model.p2p_generate_graphed(xs, L, cp, nsample=ns))):
+            if k == "nsample" and ns == 1:
+                continue
+            eng.clear()
+            fn()
+            memory[k] = eng.memory_bytes()
         frames = ns * B * (L - 1)
         res = dict(workload=name, image_width=width, channels=C, B=B, samples=ns, len_output=L, precision=prec, card=info,
-                   parity=parity)
+                   parity=parity, graph_memory_bytes=memory)
         for k, ts in times.items():
             ms = statistics.median(ts)
             calls = ns if k.endswith("looped") else 1
