@@ -409,6 +409,35 @@ int p2pvg_pose_windows(const float* pose2d, const float* pose3d, int J, const in
                        const int32_t* entries, const int32_t* draws, int B, int speed_lo, int speed_hi, int L, int T, float* out2d,
                        float* out3d, void* stream);
 
+/* Scores of generated frames against ground-truth frames, one result row per pair.
+ *   pred       [N][C][H][W] fp32, 16-byte aligned; gt [M][C][H][W] fp32, 16-byte aligned
+ *   pairs      [n_pairs][2] int32, 4-byte aligned: pair p scores pred frame pairs[p][0] against gt frame pairs[p][1]
+ *   out        [n_pairs][3] fp64, 8-byte aligned: mse, psnr, ssim of each pair, with R = data_range:
+ *              mse  = sum (P - G)^2 / (C H W)
+ *              psnr = 10 log10(R^2 / mse), +inf when mse == 0
+ *              ssim = the mean over channels of the mean of S over the (H - 6)(W - 6) 7x7 windows inside the frame, with
+ *                     window means ux, uy, sample (ddof 1) variances vx, vy and covariance vxy,
+ *                     S = (2 ux uy + C1)(2 vxy + C2) / ((ux^2 + uy^2 + C1)(vx + vy + C2)), C1 = (0.01 R)^2, C2 = (0.03 R)^2
+ *                     (skimage.metrics.structural_similarity at its defaults, data_range = R, channels averaged)
+ * One pass: each element of a pair's two frames is read once; per-pixel arithmetic is fp32, the per-pair sums fp64 in a
+ * fixed order, so a pair's row is bit-identical whichever other pairs share the launch.  Pairs that share a gt frame are
+ * best placed next to each other: the repeats of that frame are then served from L2.
+ * Precondition (not checked on the device): 0 <= pairs[p][0] < N and 0 <= pairs[p][1] < M; p2pvg_b200.metrics checks it.
+ * n_pairs == 0 returns P2PVG_OK without a launch (pairs and out may then be NULL, as empty arrays' storage often is).
+ * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, C < 1, H < 7, W < 8, W % 4 != 0, n_pairs < 0, data_range not finite and
+ * positive.  P2PVG_ERR_UNSUPPORTED: W > 128 (the width the shared-memory tiles cover) or C * H * W >= 2^31. */
+int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int C, int H, int W,
+                        float data_range, double* out, void* stream);
+
+/* Scores of generated poses against ground-truth poses, one result row per pair.
+ *   pred [N][J][3] fp32, gt [M][J][3] fp32 (4-byte aligned); pairs [n_pairs][2] int32 (4-byte aligned) as for
+ *   p2pvg_frame_metrics; out [n_pairs][2] fp64 (8-byte aligned): mse = the mean of the 3J squared differences,
+ *   mpjpe = (1/J) sum_j ||P_j - G_j||_2.  fp64 throughout, a fixed summation order.
+ * Precondition (not checked on the device): pair indices in range.  n_pairs == 0 returns P2PVG_OK without a launch (pairs
+ * and out may then be NULL).
+ * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, J < 1, n_pairs < 0. */
+int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -455,3 +455,14 @@ class CudaKernels:
         self._ck(self.lib.p2pvg_pose_windows(_p(pose_2d), _p(pose_3d), _i(J), _p(seq_first), _p(seq_len), _i(len(seq_len)),
                                              _p(entries), _p(draws), _i(B), _i(speed_range[0]), _i(speed_range[1]), _i(L), _i(T),
                                              _p(out_2d), _p(out_3d), self._stream()))
+
+    # -- metrics ---------------------------------------------------------------------------
+    def frame_metrics(self, pred, gt, pairs, n_pairs, C, H, W, data_range, out):
+        """p2pvg_frame_metrics: out fp64 [n_pairs, 3] = mse, psnr, ssim of pred[pairs[p, 0]] against gt[pairs[p, 1]]
+        (fp32 [.., C, H, W] stores, int32 pairs; checked by p2pvg_b200.metrics)."""
+        self._ck(self.lib.p2pvg_frame_metrics(_p(pred), _p(gt), _p(pairs), _i(n_pairs), _i(C), _i(H), _i(W), _f(data_range), _p(out),
+                                              self._stream()))
+
+    def pose_metrics(self, pred, gt, pairs, n_pairs, J, out):
+        """p2pvg_pose_metrics: out fp64 [n_pairs, 2] = mse, mpjpe of pred[pairs[p, 0]] against gt[pairs[p, 1]] ([.., J, 3])."""
+        self._ck(self.lib.p2pvg_pose_metrics(_p(pred), _p(gt), _p(pairs), _i(n_pairs), _i(J), _p(out), self._stream()))

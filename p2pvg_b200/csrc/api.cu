@@ -107,6 +107,8 @@ int p2pvg_video_windows_impl(const uint8_t*, const int64_t*, const int32_t*, int
                              int, int, int, float*, cudaStream_t);
 int p2pvg_pose_windows_impl(const float*, const float*, int, const int64_t*, const int32_t*, int, const int32_t*, const int32_t*, int, int,
                             int, int, int, float*, float*, cudaStream_t);
+int p2pvg_frame_metrics_impl(const float*, const float*, const int32_t*, int, int, int, int, float, double*, cudaStream_t);
+int p2pvg_pose_metrics_impl(const float*, const float*, const int32_t*, int, int, double*, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -354,6 +356,13 @@ int p2pvg_pose_windows(const float* pose2d, const float* pose3d, int J, const in
                        float* out3d, void* stream) {
   return p2pvg_pose_windows_impl(pose2d, pose3d, J, seq_first, seq_len, n_seq, entries, draws, B, speed_lo, speed_hi, L, T, out2d,
                                  out3d, ST);
+}
+int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int C, int H, int W,
+                        float data_range, double* out, void* stream) {
+  return p2pvg_frame_metrics_impl(pred, gt, pairs, n_pairs, C, H, W, data_range, out, ST);
+}
+int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream) {
+  return p2pvg_pose_metrics_impl(pred, gt, pairs, n_pairs, J, out, ST);
 }
 
 }  // extern "C"

@@ -29,6 +29,10 @@ Layer dispatch (bf16 mode): the 4x4/s2 convolutions with >= 64 channels on both 
 (im2col / col2im + GEMM), the 4x4-valid GEMMs (encoder final, decoder first) and all of the fp32 mode use the explicit
 lowering followed by p2pvg_bn_act, as infer.py does (the training engine lowers the thin ends the same way).
 
+``evaluate`` (P2PModel.p2p_evaluate) runs the replay of a generate call and, instead of assembling the output list, scores the
+decoded frames in the graph's output buffer against the ground truth in its input buffer with one metrics launch
+(metrics.plan_pairs names the rows).
+
 Memory: every cached signature (at most MAX_GRAPHS, least recently used evicted) owns its buffers; the ground-truth encode
 covers all len(x) frames of the call.  ``GenerateEngine.memory_bytes()`` reports the total, ``clear()`` frees it.
 
@@ -107,11 +111,49 @@ class GenerateEngine:
     # ------------------------------------------------------------------ public entry
     @torch.no_grad()
     def generate(self, x, len_output, eval_cp_ix, model_mode="full", skip_frame=False, init_hidden=True, nsample=1):
+        if isinstance(x, tuple):   # h36m: (pose_2d, pose_3d, camera_view) -> pose_3d (models/p2p_model.py:96-103)
+            x = x[1]
+        G, slots = self._replay(x, len_output, eval_cp_ix, model_mode, skip_frame, init_hidden, nsample)
+        return self._assemble(G, x, slots, len_output)
+
+    @torch.no_grad()
+    def evaluate(self, x, nsample=1, len_output=None, model_mode="full", data_range=1.0):
+        """generate(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) with L = len_output or len(x), scored by ONE
+        metrics launch on the graph's own output and input buffers (metrics.plan_pairs): see P2PModel.p2p_evaluate."""
+        from . import metrics
+        if isinstance(x, tuple):
+            x = x[1]
+        self._check_model()
+        T = len(x)
+        L = T if len_output is None else int(len_output)
+        n_past = int(self.model.opt.n_past)
+        if L <= n_past:
+            raise ValueError(f"p2p_evaluate: nothing is generated to score (len_output = {L} <= n_past = {n_past})")
+        metrics._check_range(data_range)
+        G, _ = self._replay(x, L, L - 1, model_mode, False, True, nsample)
+        c = G.cfg
+        B, fshape = c["B"], c["fshape"]
+        pairs = G.bufs.get("eval_pairs")
+        if pairs is None:   # the plan depends on nothing but the graph's signature
+            frames, pairs = metrics.plan_pairs(L, T, n_past, nsample, B)
+            pairs = G.bufs["eval_pairs"] = pairs.to(c["dev"])
+            G.eval_frames = frames
+        frames = G.eval_frames
+        out, xb = G.bufs["out"], G.bufs["x"]
+        if self.model.is_pose:
+            res, names = metrics.launch_pose_metrics(out, xb, pairs, fshape[0]), metrics.POSE_METRICS
+        else:
+            res, names = metrics.launch_frame_metrics(out, xb, pairs, fshape, data_range), metrics.FRAME_METRICS
+        res = res.view(len(frames), B, nsample, len(names)).permute(3, 2, 0, 1)   # [metric][sample][frame][b]
+        scores = {k: res[i].contiguous() for i, k in enumerate(names)}
+        return dict(frames=list(frames), **scores, best=metrics.best_of(scores, names))
+
+    def _replay(self, x, len_output, eval_cp_ix, model_mode, skip_frame, init_hidden, nsample):
+        """Steps (1)-(5) of a call: capture on first use of the signature, write this call's inputs, replay, and leave the
+        LSTM state in the modules' .hidden as the eager path does.  Returns the graph and the executed slots."""
         from . import infer
         model = self.model
         self._check_model()
-        if isinstance(x, tuple):   # h36m: (pose_2d, pose_3d, camera_view) -> pose_3d (models/p2p_model.py:96-103)
-            x = x[1]
         if model_mode not in ("full", "posterior", "prior"):
             raise ValueError(f"unknown model_mode {model_mode!r}")
         if nsample < 1:
@@ -191,13 +233,19 @@ class GenerateEngine:
                 for l, (h, c) in enumerate(getattr(model, m).hidden):
                     hs[l].copy_(h)
                     cs[l].copy_(c)
-        # (5) replay
+        # (5) replay, LSTM state written back as the eager path leaves it
         G.graph.replay()
-        # (6) fresh tensors out of the static buffers, LSTM state written back as the eager path leaves it
-        out = G.bufs["out"].clone()
         for m in ("posterior", "prior", "frame_predictor"):
             hs, cs = G.bufs[f"{m}_h"], G.bufs[f"{m}_c"]
             getattr(model, m).hidden = [(hs[l].clone(), cs[l].clone()) for l in range(hs.shape[0])]
+        return G, slots
+
+    def _assemble(self, G, x, slots, len_output):
+        """Steps (6)-(7): the generated sequence (or nsample sequences) as fresh tensors out of the graph's buffers."""
+        c = G.cfg
+        nsample, B, n_past, fshape, dev, rows = c["ns"], c["B"], c["n_past"], c["fshape"], c["dev"], c["rows"]
+        # (6) fresh tensors out of the static buffers
+        out = G.bufs["out"].clone()
         # (7) the returned list: ground truth while i < n_past, zeros for skipped frames
         executed = {i for (i, _, _, _) in slots}
         frames, j = [], 0

@@ -200,14 +200,32 @@ class P2PModel(nn.Module):
         reference API; see gen_engine.py and gen_engine_vgg.py).  dcgan_64 / dcgan_128, vgg_64 / vgg_128 (on a CUDA device)
         and h36m_mlp in eval mode only: anything else raises ValueError.  Pose input: the (pose_2d, pose_3d, camera_view)
         tuple, a [T, B, 17, 3] tensor or a list of [B, 17, 3]."""
+        return self._graphed_engine().generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
+                                               init_hidden=init_hidden, nsample=nsample)
+
+    def p2p_evaluate(self, x, nsample=1, len_output=None, model_mode='full', data_range=1.0):
+        """Generate and score in one call (an addition to the reference API): exactly what
+        p2p_generate_graphed(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) generates (same draws, same cached
+        graph, .hidden left the same way), with L = len_output or len(x) (len(pose_3d) for the pose tuple), then ONE metrics
+        launch (p2pvg_b200.metrics) on the generated frames.  Scored: every generated frame n_past .. L - 1 against x[i] when
+        L == len(x), else only the control point L - 1 against x[len(x) - 1].  The same models as p2p_generate_graphed.
+
+        Returns a dict: 'frames' (the scored indices), per metric a float64 [nsample, len(frames), B] tensor on the device --
+        mse, psnr, ssim for frames (data_range: the frames' value range), mse, mpjpe for poses; the last frame column is the
+        control point -- and 'best': per metric (index [B], curve [len(frames), B]) of the sample with the best mean over the
+        scored frames (highest ssim / psnr, lowest mse / mpjpe; the first on ties).  ValueError when L <= n_past or
+        data_range is not positive."""
+        return self._graphed_engine().evaluate(x, nsample=nsample, len_output=len_output, model_mode=model_mode,
+                                               data_range=data_range)
+
+    def _graphed_engine(self):
         from ..gen_engine import GenerateEngine, PoseGenerateEngine
         from ..gen_engine_vgg import VggGenerateEngine
         from .vgg import VggEncoder
         if getattr(self, "_gen_engine", None) is None:
             cls = PoseGenerateEngine if self.is_pose else VggGenerateEngine if isinstance(self.encoder, VggEncoder) else GenerateEngine
             self._gen_engine = cls(self)
-        return self._gen_engine.generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
-                                         init_hidden=init_hidden, nsample=nsample)
+        return self._gen_engine
 
     # ---- checkpoints (same dict layout as reference p2p_model.py:289-330) --------------------------
     def save(self, fname, epoch):
