@@ -29,9 +29,16 @@ Layer dispatch (bf16 mode): the 4x4/s2 convolutions with >= 64 channels on both 
 (im2col / col2im + GEMM), the 4x4-valid GEMMs (encoder final, decoder first) and all of the fp32 mode use the explicit
 lowering followed by p2pvg_bn_act, as infer.py does (the training engine lowers the thin ends the same way).
 
-``evaluate`` (P2PModel.p2p_evaluate) runs the replay of a generate call and, instead of assembling the output list, scores the
-decoded frames in the graph's output buffer against the ground truth in its input buffer with one metrics launch
-(metrics.plan_pairs names the rows).
+``generate_multi_cp`` (P2PModel.p2p_generate_multi_cp) replays a chain of segments x[cp_ixs[k] : cp_ixs[k + 1] + 1], each
+what one call with init_hidden=False after the first computes; a single call is the one-segment chain.  The per-slot tables
+(plan_segments) index clip frames, so every slot reads its segment's ground truth, global descriptor (a per-slot tab_int
+entry) and counters; the LSTM state stays in the graph's buffers across segments.  A chain's ground-truth encode covers the
+clip followed by a copy of each segment's skip source frame, so that the skip halves of all segments are one batched launch
+per stage, of which each decode reads its segment's B images.
+
+``evaluate`` (P2PModel.p2p_evaluate) runs the replay of a generate call (or chain) and, instead of assembling the output list,
+scores the decoded frames in the graph's output buffer against the ground truth in its input buffer with one metrics launch
+(metrics.plan_pairs / plan_pairs_multi_cp name the rows).
 
 Memory: every cached signature (at most MAX_GRAPHS, least recently used evicted) owns its buffers; the ground-truth encode
 covers all len(x) frames of the call.  ``GenerateEngine.memory_bytes()`` reports the total, ``clear()`` frees it.
@@ -42,6 +49,7 @@ draws are consumed in the reference's order (posterior, then prior, per executed
 """
 from __future__ import annotations
 
+import gc
 from collections import OrderedDict
 
 import numpy as np
@@ -67,6 +75,61 @@ def plan_slots(len_output, len_x, probs, skip_prob, n_past, skip_frame, eval_cp_
         out.append((i, (eval_cp_ix - i + 1) / eval_cp_ix, (i - prev_i) / eval_cp_ix, i if i < len_x else -1))
         prev_i = i
     return out
+
+
+def plan_segments(segs, T, probs, skip_prob, n_past, skip_frame, model_mode):
+    """Executed steps and per-slot tables of a chain of generate calls whose inputs are slices of one clip.
+
+    segs: per segment (offset, T_k, L_k, eval_cp_ix_k): the call p2p_generate(x[offset : offset + T_k], L_k, eval_cp_ix_k);
+    probs: each segment's NumPy skip draw; T: the clip's frame count, which is also the index of the row that holds the
+    autoregressive encode in the engine's h source.  The slots of all segments are numbered in chain order.
+
+    Returns (slots, ints, floats): plan_slots of each segment; the int32 table [tab_i | tab_h | tab_z | tab_g] of 4 * S
+    entries (clip frame of the posterior target, clip frame or T of the encoder input h, 0 / 1 for the predictor's z from
+    the posterior / prior, clip frame of the global descriptor); the float table [time_until_cp | delta_time] of 2 * S."""
+    slots, tab_i, tab_h, tab_z, tab_g, tuc, dt = [], [], [], [], [], [], []
+    for (o, Tk, Lk, cp), pr in zip(segs, probs):
+        sl = plan_slots(Lk, Tk, pr, skip_prob, n_past, skip_frame, cp)
+        n_tf = min(n_past - 1, Lk - 1)
+        slots.append(sl)
+        for j, (_, t, d, tgt) in enumerate(sl):
+            h = o + j if j <= n_tf else T                  # ground truth until the segment's first decode
+            tab_h.append(h)
+            tab_i.append(o + tgt if tgt >= 0 else h)       # posterior: x_k[i], or h_cpaw's h when x_k has no frame i
+            tab_z.append(0 if (model_mode == "posterior" or (j < n_tf and model_mode == "full")) else 1)
+            tab_g.append(o + Tk - 1)                       # global descriptor: the segment's control point
+            tuc.append(t)
+            dt.append(d)
+    return slots, tab_i + tab_h + tab_z + tab_g, tuc + dt
+
+
+def check_cp_ixs(cp_ixs, T, len_outputs, n_past):
+    """The segments (offset, T_k, L_k, L_k - 1) of a multi-control-point call on a clip of T frames; ValueError for a
+    malformed cp_ixs or len_outputs, or a segment with fewer than min(n_past, L_k) frames."""
+    try:
+        cps = [int(v) for v in cp_ixs]
+    except (TypeError, ValueError):
+        raise ValueError(f"cp_ixs must be a sequence of ints (got {cp_ixs!r})") from None
+    if any(isinstance(v, bool) or int(v) != v for v in cp_ixs):
+        raise ValueError(f"cp_ixs must be a sequence of ints (got {cp_ixs!r})")
+    if len(cps) < 2 or cps[0] != 0 or any(b <= a for a, b in zip(cps, cps[1:])) or cps[-1] > T - 1:
+        raise ValueError(f"cp_ixs must start at 0, increase strictly, have at least 2 entries and end at or before the last "
+                         f"input frame {T - 1} (got {cps})")
+    Ts = [b - a + 1 for a, b in zip(cps, cps[1:])]
+    if len_outputs is None:
+        Ls = Ts
+    else:
+        Ls = list(len_outputs)
+        if len(Ls) != len(Ts):
+            raise ValueError(f"len_outputs needs one entry per segment ({len(Ts)}), got {len(Ls)}")
+        if any(isinstance(v, bool) or int(v) != v or v < 2 for v in Ls):
+            raise ValueError(f"every len_outputs entry must be an int >= 2 (got {Ls})")
+        Ls = [int(v) for v in Ls]
+    for k, (Tk, Lk) in enumerate(zip(Ts, Ls)):
+        if n_past < 1 or Tk < min(n_past, Lk):
+            raise ValueError(f"segment {k} has {Tk} frames; it needs n_past >= 1 and at least min(n_past, len_output) = "
+                             f"{min(n_past, Lk)}")
+    return [(o, Tk, Lk, Lk - 1) for o, Tk, Lk in zip(cps, Ts, Ls)]
 
 
 def check_supported(model):
@@ -114,28 +177,57 @@ class GenerateEngine:
         if isinstance(x, tuple):   # h36m: (pose_2d, pose_3d, camera_view) -> pose_3d (models/p2p_model.py:96-103)
             x = x[1]
         G, slots = self._replay(x, len_output, eval_cp_ix, model_mode, skip_frame, init_hidden, nsample)
-        return self._assemble(G, x, slots, len_output)
+        return self._assemble(G, x, slots[0], len_output)
 
     @torch.no_grad()
-    def evaluate(self, x, nsample=1, len_output=None, model_mode="full", data_range=1.0):
-        """generate(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) with L = len_output or len(x), scored by ONE
-        metrics launch on the graph's own output and input buffers (metrics.plan_pairs): see P2PModel.p2p_evaluate."""
+    def generate_multi_cp(self, x, cp_ixs, len_outputs=None, model_mode="full", skip_frame=False, nsample=1):
+        """The chain generate(x_0, L_0, L_0 - 1, init_hidden=True), then generate(x_k, L_k, L_k - 1, init_hidden=False) for
+        k >= 1, with x_k = x[cp_ixs[k] : cp_ixs[k + 1] + 1], as ONE replay: see P2PModel.p2p_generate_multi_cp."""
+        if isinstance(x, tuple):
+            x = x[1]
+        G, slots, segs = self._replay_chain(x, cp_ixs, len_outputs, model_mode, skip_frame, nsample)
+        out, res, d = G.bufs["out"].clone(), [], 0
+        for (o, Tk, Lk, _), sl, (_, _, _, Sk, n_tf) in zip(segs, slots, G.cfg["segs"]):
+            n_dec = max(Sk - n_tf, 0)
+            res.append(self._assemble_seq(G.cfg, out[d:d + n_dec], x[o:o + Tk], sl, Lk))
+            d += n_dec
+        return res
+
+    @torch.no_grad()
+    def evaluate(self, x, nsample=1, len_output=None, model_mode="full", data_range=1.0, cp_ixs=None):
+        """generate(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) with L = len_output or len(x) (or, given cp_ixs,
+        generate_multi_cp(x, cp_ixs, None, model_mode, skip_frame=False, nsample=nsample)), scored by ONE metrics launch on the
+        graph's own output and input buffers (metrics.plan_pairs / plan_pairs_multi_cp): see P2PModel.p2p_evaluate."""
         from . import metrics
         if isinstance(x, tuple):
             x = x[1]
         self._check_model()
         T = len(x)
-        L = T if len_output is None else int(len_output)
         n_past = int(self.model.opt.n_past)
-        if L <= n_past:
-            raise ValueError(f"p2p_evaluate: nothing is generated to score (len_output = {L} <= n_past = {n_past})")
-        metrics._check_range(data_range)
-        G, _ = self._replay(x, L, L - 1, model_mode, False, True, nsample)
+        if cp_ixs is not None:
+            if len_output is not None:
+                raise ValueError("p2p_evaluate takes cp_ixs or len_output, not both (with cp_ixs every segment keeps the clip's "
+                                 "timing)")
+            segs = check_cp_ixs(cp_ixs, T, None, n_past)
+            for k, (_, _, Lk, _) in enumerate(segs):
+                if Lk <= n_past:
+                    raise ValueError(f"p2p_evaluate: segment {k} generates nothing to score ({Lk} frames <= n_past = {n_past})")
+            metrics._check_range(data_range)
+            G, _, _ = self._replay_chain(x, cp_ixs, None, model_mode, False, nsample)
+        else:
+            L = T if len_output is None else int(len_output)
+            if L <= n_past:
+                raise ValueError(f"p2p_evaluate: nothing is generated to score (len_output = {L} <= n_past = {n_past})")
+            metrics._check_range(data_range)
+            G, _ = self._replay(x, L, L - 1, model_mode, False, True, nsample)
         c = G.cfg
         B, fshape = c["B"], c["fshape"]
         pairs = G.bufs.get("eval_pairs")
         if pairs is None:   # the plan depends on nothing but the graph's signature
-            frames, pairs = metrics.plan_pairs(L, T, n_past, nsample, B)
+            if cp_ixs is not None:
+                frames, pairs = metrics.plan_pairs_multi_cp([o for (o, _, _, _, _) in c["segs"]] + [c["T"] - 1], n_past, nsample, B)
+            else:
+                frames, pairs = metrics.plan_pairs(L, T, n_past, nsample, B)
             pairs = G.bufs["eval_pairs"] = pairs.to(c["dev"])
             G.eval_frames = frames
         frames = G.eval_frames
@@ -149,8 +241,22 @@ class GenerateEngine:
         return dict(frames=list(frames), **scores, best=metrics.best_of(scores, names))
 
     def _replay(self, x, len_output, eval_cp_ix, model_mode, skip_frame, init_hidden, nsample):
-        """Steps (1)-(5) of a call: capture on first use of the signature, write this call's inputs, replay, and leave the
-        LSTM state in the modules' .hidden as the eager path does.  Returns the graph and the executed slots."""
+        """One call: the one-segment chain over all len(x) frames.  Returns the graph and [executed slots]."""
+        return self._run(x, len(x), [(0, len(x), len_output, eval_cp_ix)], model_mode, skip_frame, init_hidden, nsample)
+
+    def _replay_chain(self, x, cp_ixs, len_outputs, model_mode, skip_frame, nsample):
+        """A multi-control-point call: checks before any draw or launch, then the chain of segments (offset, T_k, L_k,
+        L_k - 1) over the clip's first cp_ixs[-1] + 1 frames.  Returns the graph, the slots per segment and the segments."""
+        self._check_model()
+        segs = check_cp_ixs(cp_ixs, len(x), len_outputs, int(self.model.opt.n_past))
+        T = segs[-1][0] + segs[-1][1]
+        G, slots = self._run(x, T, segs, model_mode, skip_frame, True, nsample)
+        return G, slots, segs
+
+    def _run(self, x, T, segs, model_mode, skip_frame, init_hidden, nsample):
+        """Steps (1)-(5) of a chain of segments (offset, T_k, L_k, eval_cp_ix_k) on the clip x[:T]: capture on first use of
+        the signature, write this call's inputs, replay, and leave the LSTM state in the modules' .hidden as the eager path
+        does.  Returns the graph and the executed slots of each segment."""
         from . import infer
         model = self.model
         self._check_model()
@@ -159,30 +265,37 @@ class GenerateEngine:
         if nsample < 1:
             raise ValueError("nsample must be >= 1")
         opt = model.opt
-        T = len(x)
         fshape = self._frame_shape(x[0])
         B = int(x[0].shape[0])
         n_past = int(opt.n_past)
-        if n_past < 1 or T < min(n_past, len_output):
+        if n_past < 1 or any(Tk < min(n_past, Lk) for (_, Tk, Lk, _) in segs):
             raise ValueError("p2p_generate_graphed needs n_past >= 1 and at least min(n_past, len_output) input frames")
         rows = nsample * B
         dev = x[0].device
-        # (1) the reference's NumPy draw, made even when skip_frame is False (models/p2p_model.py:128)
-        probs = np.random.uniform(0, 1, len_output - 1)
-        slots = plan_slots(len_output, T, probs, float(opt.skip_prob), n_past, skip_frame, eval_cp_ix)
-        S = len(slots)
+        # (1) the reference's NumPy draw per segment, made even when skip_frame is False (models/p2p_model.py:128)
+        probs = [np.random.uniform(0, 1, Lk - 1) for (_, _, Lk, _) in segs]
+        slots, ints, fl = plan_segments(segs, T, probs, float(opt.skip_prob), n_past, skip_frame, model_mode)
+        Ss = [len(sl) for sl in slots]
+        S = sum(Ss)
         lfs = bool(opt.last_frame_skip)
         adt = infer._act_dtype()
         K = infer.kernels_for(dev)
         ptrs = tuple(p.data_ptr() for p in model.parameters()) + tuple(b.data_ptr() for b in model.buffers())
-        sig = (rows, B, T, fshape, len_output, S, model_mode, n_past, lfs, str(adt), ptrs)
+        # one segment: (len_output, executed steps), as for a single call; a chain: (T_k, L_k, S_k) per segment
+        seg_sig = (segs[0][2], S) if len(segs) == 1 else (tuple((Tk, Lk, Sk) for (_, Tk, Lk, _), Sk in zip(segs, Ss)),)
+        sig = (rows, B, T, fshape, *seg_sig, model_mode, n_past, lfs, str(adt), ptrs)
         G = self._graphs.get(sig)
         if G is not None and G.ws_gen != K.ws_gen:
             del self._graphs[sig]
             G = None
-        n_tf = min(n_past - 1, len_output - 1)
-        cfg = dict(rows=rows, B=B, T=T, fshape=fshape, C=fshape[0], W=fshape[-1], S=S, n_tf=n_tf, mode=model_mode, n_past=n_past,
-                   lfs=lfs, adt=adt, ns=nsample, dev=dev)
+        cseg = tuple((o, Tk, Lk, Sk, min(n_past - 1, Lk - 1)) for (o, Tk, Lk, _), Sk in zip(segs, Ss))
+        # the ground-truth frames whose skip maps give the decoders' skip halves, one per segment: x_k[max(n_past - 2, 0)],
+        # or with last_frame_skip the frame before the segment's first decode.  One segment reads it in place; a chain
+        # appends copies of them behind the clip, so that all segments' skip halves come from one batched launch per stage
+        src = [o + min(n_tf if lfs else max(n_past - 2, 0), Tk - 1) for (o, Tk, _, _, n_tf) in cseg]
+        cfg = dict(rows=rows, B=B, T=T, fshape=fshape, C=fshape[0], W=fshape[-1], S=S, segs=cseg, src=src,
+                   T_enc=T if len(segs) == 1 else T + len(segs), n_dec=sum(max(Sk - n_tf, 0) for (_, _, _, Sk, n_tf) in cseg),
+                   mode=model_mode, n_past=n_past, lfs=lfs, adt=adt, ns=nsample, dev=dev)
         if not init_hidden:
             for m in ("posterior", "prior", "frame_predictor"):
                 mod = getattr(model, m)
@@ -198,8 +311,16 @@ class GenerateEngine:
             self._body(G)
             torch.cuda.current_stream(dev).synchronize()
             G.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(G.graph):
-                self._body(G)
+            # no garbage collection during the capture: a dropped model and its engine form a reference cycle, and a cached
+            # CUDA graph the collector destroys mid-capture invalidates this capture
+            gc_on = gc.isenabled()
+            gc.disable()
+            try:
+                with torch.cuda.graph(G.graph):
+                    self._body(G)
+            finally:
+                if gc_on:
+                    gc.enable()
             G.ws_gen = K.ws_gen
             self._graphs[sig] = G
             while len(self._graphs) > MAX_GRAPHS:
@@ -208,14 +329,12 @@ class GenerateEngine:
             self._graphs.move_to_end(sig)
         # (2)-(4) inputs of this call: frames, per-slot tables, eps, initial LSTM state
         xs = x if torch.is_tensor(x) else torch.stack(list(x))
-        G.bufs["x"].copy_(xs.reshape(G.bufs["x"].shape))
-        tab_h = [s if s <= n_tf else T for s in range(S)]                   # h source: ground truth until the first decode
-        tab_i = [t if t >= 0 else tab_h[s] for s, (_, _, _, t) in enumerate(slots)]   # posterior: x[i] or h_cpaw's h
-        tab_z = [0 if (model_mode == "posterior" or (s < n_tf and model_mode == "full")) else 1 for s in range(S)]
-        ints = torch.tensor(tab_i + tab_h + tab_z + [T - 1], dtype=torch.int32)
-        fl = torch.tensor([t for (_, t, _, _) in slots] + [d for (_, _, d, _) in slots], dtype=torch.float64).float()
-        G.bufs["tab_int"].copy_(ints, non_blocking=True)
-        G.bufs["tab_f"][:2 * S].copy_(fl, non_blocking=True)
+        xb = G.bufs["x"].view(cfg["T_enc"], B, *fshape)
+        xb[:T].copy_(xs[:T].reshape(T, B, *fshape))
+        if cfg["T_enc"] > T:
+            xb[T:].copy_(xs[src].reshape(len(src), B, *fshape))
+        G.bufs["tab_int"][:4 * S].copy_(torch.tensor(ints, dtype=torch.int32), non_blocking=True)
+        G.bufs["tab_f"][:2 * S].copy_(torch.tensor(fl, dtype=torch.float64).float(), non_blocking=True)
         if S:
             z = model.z_dim
             if infer._EPS_STREAM is not None:
@@ -241,12 +360,14 @@ class GenerateEngine:
         return G, slots
 
     def _assemble(self, G, x, slots, len_output):
-        """Steps (6)-(7): the generated sequence (or nsample sequences) as fresh tensors out of the graph's buffers."""
-        c = G.cfg
+        """Steps (6)-(7) of a one-segment call: the generated sequence (or nsample sequences) as fresh tensors out of the
+        graph's buffers."""
+        return self._assemble_seq(G.cfg, G.bufs["out"].clone(), x, slots, len_output)
+
+    def _assemble_seq(self, c, out, x, slots, len_output):
+        """The returned list of one segment from its decoded frames out (already out of graph memory): ground truth while
+        i < n_past, zeros for skipped frames."""
         nsample, B, n_past, fshape, dev, rows = c["ns"], c["B"], c["n_past"], c["fshape"], c["dev"], c["rows"]
-        # (6) fresh tensors out of the static buffers
-        out = G.bufs["out"].clone()
-        # (7) the returned list: ground truth while i < n_past, zeros for skipped frames
         executed = {i for (i, _, _, _) in slots}
         frames, j = [], 0
         for i in range(1, len_output):
@@ -295,11 +416,11 @@ class GenerateEngine:
         c, model = G.cfg, self.model
         dev, S, rows = c["dev"], c["S"], c["rows"]
         b = G.bufs
-        b["x"] = torch.zeros(c["T"] * c["B"], *c["fshape"], device=dev)
-        b["tab_int"] = torch.zeros(3 * S + 1, dtype=torch.int32, device=dev)
+        b["x"] = torch.zeros(c["T_enc"] * c["B"], *c["fshape"], device=dev)
+        b["tab_int"] = torch.zeros(max(4 * S, 1), dtype=torch.int32, device=dev)
         b["tab_f"] = torch.zeros(max(2 * S, 1), device=dev)
         b["eps"] = torch.zeros(max(S, 1), 2, rows, model.z_dim, device=dev)
-        n_dec = max(S - c["n_tf"], 0)
+        n_dec = c["n_dec"]
         b["out"] = torch.zeros(max(n_dec, 1), rows, *c["fshape"], device=dev)[:n_dec]
         for m in ("posterior", "prior", "frame_predictor"):
             mod = getattr(model, m)
@@ -319,11 +440,13 @@ class GenerateEngine:
         c, model = G.cfg, self.model
         K = infer.kernels_for(c["dev"])
         self.K, self.G = K, G
-        rows, B, T, S, n_tf = c["rows"], c["B"], c["T"], c["S"], c["n_tf"]
+        rows, B, T, S, segs = c["rows"], c["B"], c["T"], c["S"], c["segs"]
         g, z = model.g_dim, model.z_dim
+        nK = len(segs)
         self._prepare_weights()
-        # ground truth: one time-batched encode at B rows, tiled to the nsample*B rows of the recurrent part
-        N = T * B
+        # ground truth: one time-batched encode at B rows (the clip, then a chain's skip-source copies), tiled to the
+        # nsample*B rows of the recurrent part
+        N = c["T_enc"] * B
         h_gt = self._buf(G, "gt_h", N * g)
         gt_skips = self._encode("gt", G.bufs["x"], N, h_gt)
         Hsrc = self._buf(G, "Hsrc", (T + 1) * rows * g)     # [T + 1][rows][g]: ground truth frames, then this step's h
@@ -331,36 +454,50 @@ class GenerateEngine:
         h_cur = Hsrc[T * rows * g:]
         self._buf(G, "grp_zero", max(c["ns"], 1), torch.int32)   # source image n % B for every sample
 
-        def gt_skip(f):
-            return [s[f * B * s.numel() // N:(f + 1) * B * s.numel() // N] for s in gt_skips]
-
-        if S > n_tf and not c["lfs"]:
-            # models/p2p_model.py:143-144: the last skip set while i == 1 or i < n_past comes from x[max(n_past - 2, 0)]
-            halves = self._skip_halves("skip", gt_skip(max(c["n_past"] - 2, 0)), B)
+        # the skip sources of all segments: one frame in place (one segment), or the nK copies behind the clip (a chain)
+        f0 = c["src"][0] if nK == 1 else T
+        src_skips = [s[f0 * B * s.numel() // N:(f0 + nK) * B * s.numel() // N] for s in gt_skips]
+        halves0 = None
+        if any(Sk > n_tf for (_, _, _, Sk, n_tf) in segs) and not c["lfs"]:
+            # models/p2p_model.py:143-144: the last skip set while i == 1 or i < n_past comes from x_k[max(n_past - 2, 0)]
+            halves0 = self._skip_halves("skip", src_skips, nK * B)
         ti, tf = G.bufs["tab_int"], G.bufs["tab_f"]
         zbuf = self._buf(G, "Z", 2 * rows * z)
         h_pred = self._buf(G, "h_pred", rows * g)
         eps = G.bufs["eps"]
-        prev_frame = None
-        for s in range(S):
-            tuc, dt = tf[s:s + 1], tf[S + s:S + s + 1]
-            skips_cur = None
-            if s > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
-                skips_cur = self._encode("step", prev_frame, rows, h_cur)
-            glob = ti[3 * S:3 * S + 1]
-            # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
-            K.lstm_step([self._module("posterior", Hsrc, ti[s:s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 0], out=zbuf[:rows * z]),
-                         self._module("prior", Hsrc, ti[S + s:S + s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 1], out=zbuf[rows * z:])],
-                        rows, model.rnn_size)
-            K.lstm_step([self._module("frame_predictor", Hsrc, ti[S + s:S + s + 1], zbuf, ti[2 * S + s:2 * S + s + 1], z, tuc, dt,
-                                      out=h_pred)], rows, model.rnn_size)
-            if s < n_tf:
-                continue   # teacher-forced step: the predictor only advances its state (models/p2p_model.py:157-163)
-            if c["lfs"]:
-                src = gt_skip(s) if s == n_tf else skips_cur
-                halves = self._skip_halves("skip", src, B if s == n_tf else rows)
-            prev_frame = G.bufs["out"][s - n_tf]
-            self._decode(h_pred, halves, prev_frame)
+        s, d = 0, 0   # chain slot, decoded frame
+        for k, (_, _, _, Sk, n_tf) in enumerate(segs):
+            prev_frame = None
+            for j in range(Sk):
+                tuc, dt = tf[s:s + 1], tf[S + s:S + s + 1]
+                skips_cur = None
+                if j > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
+                    skips_cur = self._encode("step", prev_frame, rows, h_cur)
+                glob = ti[3 * S + s:3 * S + s + 1]
+                # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
+                K.lstm_step([self._module("posterior", Hsrc, ti[s:s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 0], out=zbuf[:rows * z]),
+                             self._module("prior", Hsrc, ti[S + s:S + s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 1],
+                                          out=zbuf[rows * z:])], rows, model.rnn_size)
+                K.lstm_step([self._module("frame_predictor", Hsrc, ti[S + s:S + s + 1], zbuf, ti[2 * S + s:2 * S + s + 1], z, tuc,
+                                          dt, out=h_pred)], rows, model.rnn_size)
+                s += 1
+                if j < n_tf:
+                    continue   # teacher-forced step: the predictor only advances its state (models/p2p_model.py:157-163)
+                if c["lfs"] and j > n_tf:
+                    halves = self._skip_halves("skip", skips_cur, rows)
+                else:
+                    if halves0 is None:   # last_frame_skip: every segment's first decode, batched at the chain's first
+                        halves0 = self._skip_halves("skip0", src_skips, nK * B)
+                    halves = self._segment_halves(halves0, k, nK)
+                prev_frame = G.bufs["out"][d]
+                d += 1
+                self._decode(h_pred, halves, prev_frame)
+
+    def _segment_halves(self, halves, k, nK):
+        """Segment k's part of skip halves computed for the nK segments' sources at once (B images each)."""
+        if nK == 1:
+            return halves
+        return [(t[k * t.numel() // nK:(k + 1) * t.numel() // nK], nsrc // nK) for t, nsrc in halves]
 
     # ------------------------------------------------------------------ weights
     def _prepare_weights(self):
@@ -568,6 +705,12 @@ class PoseGenerateEngine(GenerateEngine):
 
     def _skip_halves(self, tag, skips, nsrc):
         return skips, nsrc
+
+    def _segment_halves(self, halves, k, nK):
+        skips, nsrc = halves
+        if nK == 1:
+            return halves
+        return [s[k * s.numel() // nK:(k + 1) * s.numel() // nK] for s in skips], nsrc // nK
 
     def _decode(self, h_pred, halves, frame_out):
         skips, nsrc = halves

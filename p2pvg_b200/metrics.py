@@ -7,8 +7,9 @@ skimage.metrics.structural_similarity computes at its defaults with data_range=R
 mse over the J * 3 values and mpjpe, the mean over joints of the Euclidean joint error.
 
 ``frame_metrics`` / ``pose_metrics`` score any set of (pred index, gt index) pairs of two stores in one launch, so the
-generated frames of several samples can be scored against one copy of the ground truth.  ``plan_pairs`` is the pair list
-``P2PModel.p2p_evaluate`` scores inside the generation engine's buffers.
+generated frames of several samples can be scored against one copy of the ground truth.  ``plan_pairs`` (one call) and
+``plan_pairs_multi_cp`` (a chain through control points) are the pair lists ``P2PModel.p2p_evaluate`` scores inside the
+generation engine's buffers.
 """
 from __future__ import annotations
 
@@ -39,14 +40,35 @@ def plan_pairs(len_output, len_x, n_past, nsample, B):
         frames, gts = list(range(n_past, len_output)), list(range(n_past, len_output))
     else:
         frames, gts = [len_output - 1], [len_x - 1]
+    return frames, _pairs([f - n_past for f in frames], gts, nsample, B)
+
+
+def plan_pairs_multi_cp(cp_ixs, n_past, nsample, B):
+    """plan_pairs of a multi-control-point call with the clip's timing (P2PModel.p2p_evaluate with cp_ixs): segment k
+    generates frames n_past .. T_k - 1 of x[cp_ixs[k] : cp_ixs[k + 1] + 1] (T_k = cp_ixs[k + 1] - cp_ixs[k] + 1), decoded in
+    chain order into the output store, and each is scored against its clip frame cp_ixs[k] + i.  Returns (frames, pairs)
+    with frames the sorted clip indices; every control point cp_ixs[1:] is among them."""
+    frames, dec = [], []
+    for a, b in zip(cp_ixs, cp_ixs[1:]):
+        if b - a + 1 <= n_past:
+            raise ValueError(f"nothing is generated to score in segment [{a}, {b}]: {b - a + 1} frames <= n_past = {n_past}")
+        dec += [len(dec) + j for j in range(b - a + 1 - n_past)]
+        frames += [a + i for i in range(n_past, b - a + 1)]
+    return frames, _pairs(dec, frames, nsample, B)
+
+
+def _pairs(dec, gts, nsample, B):
+    """int32 [len(dec) * B * nsample, 2] pairs (output row, input row) of decoded frame dec[j], sample s, batch row b (row
+    (dec[j] * nsample + s) * B + b of the output store) against ground-truth frame gts[j] (row gts[j] * B + b), ordered
+    (frame, b, sample)."""
     rows = nsample * B
-    f = torch.tensor(frames, dtype=torch.int64).view(-1, 1, 1)
+    f = torch.tensor(dec, dtype=torch.int64).view(-1, 1, 1)
     t = torch.tensor(gts, dtype=torch.int64).view(-1, 1, 1)
     b = torch.arange(B).view(1, -1, 1)
     s = torch.arange(nsample).view(1, 1, -1)
-    pred = (f - n_past) * rows + s * B + b
+    pred = f * rows + s * B + b
     gt = (t * B + b).expand_as(pred)
-    return frames, torch.stack([pred.reshape(-1), gt.reshape(-1)], 1).to(torch.int32)
+    return torch.stack([pred.reshape(-1), gt.reshape(-1)], 1).to(torch.int32)
 
 
 def _check_store(name, t, tail_dims):

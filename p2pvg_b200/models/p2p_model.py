@@ -203,12 +203,34 @@ class P2PModel(nn.Module):
         return self._graphed_engine().generate(x, len_output, eval_cp_ix, model_mode=model_mode, skip_frame=skip_frame,
                                                init_hidden=init_hidden, nsample=nsample)
 
-    def p2p_evaluate(self, x, nsample=1, len_output=None, model_mode='full', data_range=1.0):
+    def p2p_generate_multi_cp(self, x, cp_ixs, len_outputs=None, model_mode='full', skip_frame=False, nsample=1):
+        """Generation through several control points as ONE CUDA-graph replay (an addition to the reference API; see
+        gen_engine.py).  Segment k is x_k = x[cp_ixs[k] : cp_ixs[k + 1] + 1], generated with L_k = len_outputs[k] frames
+        (default: len(x_k), the clip's timing; any L_k >= 2).  The result is what the looped calls
+
+            [p2p_generate_graphed(x_0, L_0, L_0 - 1, model_mode, skip_frame, init_hidden=True, nsample=nsample)] +
+            [p2p_generate_graphed(x_k, L_k, L_k - 1, model_mode, skip_frame, init_hidden=False, nsample=nsample) for k >= 1]
+
+        return -- a list of one such result per segment -- with the same NumPy draws (one per segment, in order), the same eps
+        consumption under infer.eps_stream and the same final LSTM state in .hidden.  Segment k > 0 starts from its given
+        control point x_k[0].  cp_ixs: strictly increasing ints, at least 2, cp_ixs[0] == 0, cp_ixs[-1] <= len(x) - 1; to
+        generate from control points only pass the stacked control points and cp_ixs = range(K + 1).  x: what
+        p2p_generate_graphed takes (for the pose tuple only pose_3d is read).  The same models as p2p_generate_graphed;
+        ValueError before any launch for a malformed cp_ixs or len_outputs, or a segment shorter than min(n_past, L_k)."""
+        return self._graphed_engine().generate_multi_cp(x, cp_ixs, len_outputs=len_outputs, model_mode=model_mode,
+                                                        skip_frame=skip_frame, nsample=nsample)
+
+    def p2p_evaluate(self, x, nsample=1, len_output=None, model_mode='full', data_range=1.0, cp_ixs=None):
         """Generate and score in one call (an addition to the reference API): exactly what
         p2p_generate_graphed(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) generates (same draws, same cached
         graph, .hidden left the same way), with L = len_output or len(x) (len(pose_3d) for the pose tuple), then ONE metrics
         launch (p2pvg_b200.metrics) on the generated frames.  Scored: every generated frame n_past .. L - 1 against x[i] when
         L == len(x), else only the control point L - 1 against x[len(x) - 1].  The same models as p2p_generate_graphed.
+
+        cp_ixs: score a generation through control points instead -- exactly what p2p_generate_multi_cp(x, cp_ixs,
+        model_mode=model_mode, nsample=nsample) generates (the clip's timing, skip_frame=False) -- with every generated frame
+        n_past .. T_k - 1 of every segment scored against x[cp_ixs[k] + i]; 'frames' then holds the sorted clip indices, which
+        include every control point cp_ixs[1:].  ValueError with len_output, or when a segment has no more than n_past frames.
 
         Returns a dict: 'frames' (the scored indices), per metric a float64 [nsample, len(frames), B] tensor on the device --
         mse, psnr, ssim for frames (data_range: the frames' value range), mse, mpjpe for poses; the last frame column is the
@@ -216,7 +238,7 @@ class P2PModel(nn.Module):
         scored frames (highest ssim / psnr, lowest mse / mpjpe; the first on ties).  ValueError when L <= n_past or
         data_range is not positive."""
         return self._graphed_engine().evaluate(x, nsample=nsample, len_output=len_output, model_mode=model_mode,
-                                               data_range=data_range)
+                                               data_range=data_range, cp_ixs=cp_ixs)
 
     def _graphed_engine(self):
         from ..gen_engine import GenerateEngine, PoseGenerateEngine
