@@ -181,6 +181,29 @@ int p2pvg_bn_act(const void* x, void* y, int dtype, const float* scale, const fl
 int p2pvg_bn_bwd(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
                  const float* gamma, int G, int64_t R, int C, int act, void* ws, size_t ws_bytes, void* dx, float* sum_dz,
                  float* sum_dzx, const float* scale, const float* shift, void* stream);
+/* p2pvg_bn_bwd for bf16 activations and LeakyReLU (y omitted: the slope comes from sign(x*scale+shift)), whose apply pass
+ * also writes dx_sum[f] = sum over the groups g with grp_src[g] == f of dx[g] (f < F; R*C bf16 elements each), summed in
+ * fp32 in increasing g and rounded once: bit-identical to p2pvg_group_sum of the dx that p2pvg_bn_bwd writes.  A source
+ * no group maps to comes out as zeros; a group whose grp_src is outside [0, F) is left untouched.  dx may alias dy.
+ * dout != NULL (C = 64): the layer's output y = bf16(lrelu(x*scale+shift)) feeds a 4x4 / stride-2 / pad-1 ConvTranspose2d(64,
+ * 1) whose output-map gradient is dout [G * R / Ho^2][2 Ho][2 Ho] (bf16, Ho a power of two); the reduce pass then also writes that
+ * convolution's weight gradient dw[c][kh * 4 + kw] = sum over rows of y[c] * dout[tap] (the [64][tap] packed layout),
+ * through wpart as p2pvg_bn_bwd_wgrad_c1 does.  dout == NULL: Ho, wpart, wpart_bytes and dw are ignored. */
+int p2pvg_bn_bwd_group_sum(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                           int64_t R, int C, void* ws, size_t ws_bytes, void* dx, float* sum_dz, float* sum_dzx,
+                           const float* scale, const float* shift, const int* grp_src, int F, void* dx_sum, const void* dout,
+                           int Ho, float* wpart, size_t wpart_bytes, float* dw, void* stream);
+/* p2pvg_bn_bwd for bf16 activations, LeakyReLU (y omitted) and C = 64, where x is the output of a 4x4 / stride-2 / pad-1
+ * convolution of the 1-channel bf16 map cin [G * R / Ho^2][2 Ho][2 Ho] (R = rows per group = images per group * Ho^2,
+ * Ho a power of two).
+ * dx is not stored: its weight gradient dw[c][kh * 4 + kw] = sum over rows of bf16(dx[c]) * cin[tap] (PyTorch's
+ * [64][1][4][4] layout) is written instead, accumulated in fp32 per block into wpart (p2pvg_bn_wgrad_c1_partial_bytes(G)
+ * bytes) and combined in fp64 in a fixed order (deterministic). */
+size_t p2pvg_bn_wgrad_c1_partial_bytes(int G);
+int p2pvg_bn_bwd_wgrad_c1(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                          int64_t R, void* ws, size_t ws_bytes, float* sum_dz, float* sum_dzx, const float* scale,
+                          const float* shift, const void* cin, int Ho, float* wpart, size_t wpart_bytes, float* dw,
+                          void* stream);
 /* The forward statistics when their per-tile column sums were produced by a GEMM epilogue (p2pvg_conv_fusion):
  * partial is float2 [G * parts_per_group][ldp]; channel c of group g sums the group's partial rows over the `fold` column
  * groups f*C + c (a GEMM row may hold several pixels / filter taps of one channel).  R = elements per (group, channel).

@@ -33,6 +33,7 @@ def load_library():
         _lib = ctypes.CDLL(LIB_PATH)
         _lib.p2pvg_last_error.restype = ctypes.c_char_p
         _lib.p2pvg_bn_workspace_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_bn_wgrad_c1_partial_bytes.restype = ctypes.c_size_t
     return _lib
 
 
@@ -303,6 +304,30 @@ class CudaKernels:
         self._ck(self.lib.p2pvg_bn_bwd(_p(dy), _p(x), _p(y), _i(_dt(x)), _p(mean), _p(invstd), _p(gamma), _i(G), _i64(R), _i(C),
                                        _i(act), _p(ws), _sz(ws.numel()), _p(dx), _p(sum_dz), _p(sum_dzx), _p(scale), _p(shift),
                                        self._stream()))
+
+    def bn_bwd_group_sum(self, dy, x, mean, invstd, gamma, G, R, C, dx, sum_dz, sum_dzx, scale, shift, grp_src, F, dx_sum,
+                         dout=None, Ho=0, wpart=None, dw=None):
+        """bn_bwd (bf16, LeakyReLU from sign(x*scale+shift)) whose apply pass also writes dx_sum[f] = the sum of dx over the
+        groups g with grp_src[g] == f, bit-identical to group_sum of the stored dx.  dout (C = 64): the gradient of the
+        1-channel output map of the 4x4 / stride-2 ConvTranspose that reads this layer's output; its weight gradient [64][16]
+        is then written to dw (wpart: bn_wgrad_c1_partial_numel(G) floats of scratch)."""
+        ws = self.bn_workspace(G, C)
+        wpb = wpart.numel() * wpart.element_size() if wpart is not None else 0
+        self._ck(self.lib.p2pvg_bn_bwd_group_sum(_p(dy), _p(x), _p(mean), _p(invstd), _p(gamma), _i(G), _i64(R), _i(C), _p(ws),
+                                                 _sz(ws.numel()), _p(dx), _p(sum_dz), _p(sum_dzx), _p(scale), _p(shift), _p(grp_src),
+                                                 _i(F), _p(dx_sum), _p(dout), _i(Ho), _p(wpart), _sz(wpb), _p(dw), self._stream()))
+
+    def bn_wgrad_c1_partial_numel(self, G):
+        """fp32 elements of the per-block weight-gradient partials bn_bwd_wgrad_c1 needs for G groups."""
+        return int(self.lib.p2pvg_bn_wgrad_c1_partial_bytes(_i(G))) // 4
+
+    def bn_bwd_wgrad_c1(self, dy, x, mean, invstd, gamma, G, R, sum_dz, sum_dzx, scale, shift, cin, Ho, wpart, dw):
+        """bn_bwd (bf16, LeakyReLU, C = 64) of the output of a 4x4 / stride-2 conv of the 1-channel map cin: writes that conv's
+        weight gradient dw [64][16] instead of dx."""
+        ws = self.bn_workspace(G, 64)
+        self._ck(self.lib.p2pvg_bn_bwd_wgrad_c1(_p(dy), _p(x), _p(mean), _p(invstd), _p(gamma), _i(G), _i64(R), _p(ws), _sz(ws.numel()),
+                                                _p(sum_dz), _p(sum_dzx), _p(scale), _p(shift), _p(cin), _i(Ho), _p(wpart),
+                                                _sz(wpart.numel() * wpart.element_size()), _p(dw), self._stream()))
 
     def bn_param_grad(self, sum_dz, sum_dzx, G, C, dgamma, dbeta):
         self._ck(self.lib.p2pvg_bn_param_grad(_p(sum_dz), _p(sum_dzx), _i(G), _i(C), _p(dgamma), _p(dbeta), self._stream()))

@@ -64,6 +64,12 @@ size_t p2pvg_bn_workspace_bytes_impl(int, int);
 int p2pvg_bn_fwd_stats_impl(const void*, int, int, long long, int, const float*, const float*, float, void*, size_t, float*, float*,
                             float*, float*, float*, cudaStream_t);
 int p2pvg_bn_act_impl(const void*, void*, int, const float*, const float*, int, long long, int, int, cudaStream_t);
+int p2pvg_bn_bwd_group_sum_impl(const void*, const void*, const float*, const float*, const float*, int, long long, int, void*, size_t,
+                                void*, float*, float*, const float*, const float*, const int*, int, void*, const void*, int, float*,
+                                size_t, float*, cudaStream_t);
+size_t p2pvg_bn_wgrad_c1_partial_bytes_impl(int);
+int p2pvg_bn_bwd_wgrad_c1_impl(const void*, const void*, const float*, const float*, const float*, int, long long, void*, size_t, float*,
+                               float*, const float*, const float*, const void*, int, float*, size_t, float*, cudaStream_t);
 int p2pvg_bn_bwd_impl(const void*, const void*, const void*, int, const float*, const float*, const float*, int, long long, int, int,
                       void*, size_t, void*, float*, float*, const float*, const float*, cudaStream_t);
 int p2pvg_bn_param_grad_impl(const float*, const float*, int, int, float*, float*, cudaStream_t);
@@ -234,6 +240,21 @@ int p2pvg_bn_bwd(const void* dy, const void* x, const void* y, int dtype, const 
                  const float* gamma, int G, int64_t R, int C, int act, void* ws, size_t ws_bytes, void* dx, float* sum_dz,
                  float* sum_dzx, const float* scale, const float* shift, void* stream) {
   return p2pvg_bn_bwd_impl(dy, x, y, dtype, mean, invstd, gamma, G, R, C, act, ws, ws_bytes, dx, sum_dz, sum_dzx, scale, shift, ST);
+}
+int p2pvg_bn_bwd_group_sum(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                           int64_t R, int C, void* ws, size_t ws_bytes, void* dx, float* sum_dz, float* sum_dzx,
+                           const float* scale, const float* shift, const int* grp_src, int F, void* dx_sum, const void* dout,
+                           int Ho, float* wpart, size_t wpart_bytes, float* dw, void* stream) {
+  return p2pvg_bn_bwd_group_sum_impl(dy, x, mean, invstd, gamma, G, R, C, ws, ws_bytes, dx, sum_dz, sum_dzx, scale, shift, grp_src, F,
+                                     dx_sum, dout, Ho, wpart, wpart_bytes, dw, ST);
+}
+size_t p2pvg_bn_wgrad_c1_partial_bytes(int G) { return p2pvg_bn_wgrad_c1_partial_bytes_impl(G); }
+int p2pvg_bn_bwd_wgrad_c1(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                          int64_t R, void* ws, size_t ws_bytes, float* sum_dz, float* sum_dzx, const float* scale,
+                          const float* shift, const void* cin, int Ho, float* wpart, size_t wpart_bytes, float* dw,
+                          void* stream) {
+  return p2pvg_bn_bwd_wgrad_c1_impl(dy, x, mean, invstd, gamma, G, R, ws, ws_bytes, sum_dz, sum_dzx, scale, shift, cin, Ho, wpart,
+                                    wpart_bytes, dw, ST);
 }
 int p2pvg_bn_fwd_finalize_tiles(const void* partial, int parts_per_group, int ldp, int fold, int G, int64_t R, int C,
                                 const float* gamma, const float* beta, float eps, float* mean, float* invstd, float* var_unbiased,

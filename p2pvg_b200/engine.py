@@ -193,6 +193,11 @@ class TrainEngine:
         self.fuse_stats = self.implicit
         # 1- / 3-channel stacks: tap gather + sigmoid + MSE of the last decoder layer as one kernel (no raw-output tensor)
         self.fuse_last = hasattr(kernels, "convt_c1_loss") and act_dtype == torch.bfloat16
+        # bf16 BatchNorm-backward passes that also finish the work of the next launch on the tensors they stream: the
+        # decoder's skip-frame sums of dx (and, in the stage before a 64 -> 1 last layer, that layer's weight gradient), and
+        # the weight gradient of a 1-channel first encoder layer (whose dx is then not stored)
+        self.bn_skip_sums = hasattr(kernels, "bn_bwd_group_sum") and act_dtype == torch.bfloat16
+        self.bn_wgrad_c1 = hasattr(kernels, "bn_bwd_wgrad_c1") and act_dtype == torch.bfloat16
         # independent chains of small kernels (the three LSTMs, backward #2) run on side streams inside the captured graph
         self.concurrent = getattr(kernels, "name", "") == "cuda" and act_dtype == torch.bfloat16 and os.environ.get("P2PVG_CONCURRENT", "1") != "0"
         self.streams, self._dirty, self._serial = {}, set(), False
@@ -893,6 +898,11 @@ class TrainEngine:
         nskip = self.last_plan.nskip
         E = self.nc * self.W0 * self.W0
         dy = self.d_rawout[g0 * B * E:g1 * B * E]
+        # a 64 -> 1 last layer's weight gradient (the half that reads the previous stage's output) is summed in that stage's
+        # BatchNorm reduce pass, which reads the same rows; until then its packed gradient waits here
+        wg_last = want_wgrad and want_skip and self.bn_skip_sums and n >= 2 and self.dec[n - 1]["cout"] == 1 \
+            and self.dec[n - 1]["cd"] == 64 and not self.dec[n - 1]["imp"] and self.dec[n - 2]["imp"]
+        deferred = None
         for k in range(n - 1, -1, -1):
             rec = self.dec[k]
             cd, cout, Hi = rec["cd"], rec["cout"], rec["Hi"]
@@ -900,11 +910,26 @@ class TrainEngine:
             cn, bn = self.dec_names(k)
             Ho = 2 * Hi
             rows_o = N * Ho * Ho
+            # skip gradient: dy summed over the calls that share a skip frame (group_sum, or the BatchNorm apply pass)
+            dyS = self.buf(f"scratch_dyS{k}", nskip * B * Ho * Ho * cout) if want_skip and rec["imp"] else None
+            fused_skip = dyS is not None and k < n - 1 and self.bn_skip_sums
             if k < n - 1:  # BatchNorm + LeakyReLU backward of this stage's output
                 st = rec["st"]
                 sl = slice(g0 * B * Ho * Ho * cout, g1 * B * Ho * Ho * cout)
                 c0, c1 = g0 * st["C"], g1 * st["C"]
-                self.bn_backward(dy, rec["raw"][sl], rec["d"][sl], st, c0, c1, Gn, B * Ho * Ho, cout, ACT_LRELU)
+                if fused_skip:
+                    wg = {}
+                    if deferred is not None:
+                        wg = dict(dout=deferred["dout"], Ho=Ho, wpart=self.fbuf("dec_wpart", K.bn_wgrad_c1_partial_numel(Gn)),
+                                  dw=deferred["dw"])
+                    K.bn_bwd_group_sum(dy, rec["raw"][sl], st["mean"][c0:c1], st["invstd"][c0:c1], st["gamma"], Gn, B * Ho * Ho, cout, dy,
+                                       st["sdz"][c0:c1], st["sdzx"][c0:c1], st["scale"][c0:c1], st["shift"][c0:c1],
+                                       self.ix["skip_src"][g0:g1], nskip, dyS, **wg)
+                    if deferred is not None:
+                        unpack_convt4(K, deferred["gw"], A.g[deferred["name"]])
+                        deferred = None
+                else:
+                    self.bn_backward(dy, rec["raw"][sl], rec["d"][sl], st, c0, c1, Gn, B * Ho * Ho, cout, ACT_LRELU)
                 if want_wgrad:
                     K.bn_param_grad(st["sdz"][c0:c1], st["sdzx"][c0:c1], Gn, cout, A.g[bn + ".weight"], A.g[bn + ".bias"])
                     A.g[cn + ".bias"].zero_()  # bias feeding a training-mode BatchNorm: gradient is exactly zero
@@ -923,8 +948,8 @@ class TrainEngine:
                 if want_wgrad:
                     K.conv_gemm(1, x_in, dy, gw[:cd * 16 * cout], N, Hi, Hi, 0, cout, Cm=cd)
                 if want_skip:
-                    dyS = self.buf(f"scratch_dyS{k}", nskip * B * Ho * Ho * cout)
-                    K.group_sum(dy, dyS, self.ix["skip_src"][g0:g1], Gn, nskip, B * Ho * Ho * cout)
+                    if not fused_skip:
+                        K.group_sum(dy, dyS, self.ix["skip_src"][g0:g1], Gn, nskip, B * Ho * Ho * cout)
                     dsk = self.buf(f"dskip{k}", Ms * cd)
                     K.conv_gemm(0, dyS, wS, dsk, nskip * B, Hi, Hi, cout, cd)
                     rec["dskip"] = dsk
@@ -941,7 +966,7 @@ class TrainEngine:
                     K.gemm(dcol, self._packed["dec_last.bdD"], dd, Md // 4, 4 * cd, 64 * cout)
                 else:
                     K.gemm(dcol, wD, dd, Md, cd, 16 * cout)
-                if want_wgrad:
+                if want_wgrad and not (wg_last and k == n - 1):
                     K.gemm(x_in, dcol, gw[:cd * 16 * cout], cd, 16 * cout, Md, a_mn=True, b_mn=True, lda=cd, ldb=16 * cout)
                 if want_skip:
                     dcolS = self.buf("scratch_dcolS", Ms * 16 * cout)
@@ -954,7 +979,9 @@ class TrainEngine:
                     rec["dskip"] = dsk
                     if want_wgrad:
                         K.gemm(rec["skip"], dcolS, gw[cd * 16 * cout:], cd, 16 * cout, Ms, a_mn=True, b_mn=True, lda=cd, ldb=16 * cout)
-                if want_wgrad:
+                if wg_last and k == n - 1:
+                    deferred = dict(gw=gw, dw=gw[:cd * 16 * cout], name=cn + ".weight", dout=dy)
+                elif want_wgrad:
                     unpack_convt4(K, gw, A.g[cn + ".weight"])
             dy = dd
         # upc1: BatchNorm + LeakyReLU, then the g -> 4x4xCtop GEMM
@@ -1148,6 +1175,14 @@ class TrainEngine:
                 K.add_indexed(gy, dsk, self.ix["skip_dst"], nskip, B * Ho * Ho * cout)
             cn, bn = self.enc_names(l)
             st = rec["st"]
+            if l == 0 and cin == 1 and cout == 64 and self.bn_wgrad_c1:
+                # the first layer has no data gradient: its weight gradient comes out of the BatchNorm apply pass
+                wpart = self.fbuf("enc0_wpart", K.bn_wgrad_c1_partial_numel(T))
+                K.bn_bwd_wgrad_c1(gy, rec["raw"], st["mean"], st["invstd"], st["gamma"], T, B * Ho * Ho, st["sdz"], st["sdzx"],
+                                  st["scale"], st["shift"], rec["inp"], Ho, wpart, A.g[cn + ".weight"])
+                K.bn_param_grad(st["sdz"], st["sdzx"], T, cout, A.g[bn + ".weight"], A.g[bn + ".bias"])
+                A.g[cn + ".bias"].zero_()
+                continue
             self.bn_backward(gy, rec["raw"], rec["y"], st, 0, T * cout, T, B * Ho * Ho, cout, ACT_LRELU)
             K.bn_param_grad(st["sdz"], st["sdzx"], T, cout, A.g[bn + ".weight"], A.g[bn + ".bias"])
             A.g[cn + ".bias"].zero_()
