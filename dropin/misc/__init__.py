@@ -1,6 +1,7 @@
-"""Shadow of the reference's ``misc`` package: ``misc.criterion`` comes from p2pvg_b200, every other submodule
-(``misc.utils``, ``misc.visualize``, ``misc.metrics``) keeps resolving to the reference checkout named by
-$P2PVG_REF (or any later ``misc`` directory on sys.path)."""
+"""Shadow of the reference's ``misc`` package: ``misc.criterion`` comes from p2pvg_b200, ``misc.visualize`` runs ``vis_seq`` on
+the graphed generator (every other name in it is the reference's), and every other submodule (``misc.utils``,
+``misc.metrics``) keeps resolving to the reference checkout named by $P2PVG_REF (or any later ``misc`` directory on
+sys.path)."""
 import os
 import sys
 

@@ -461,6 +461,23 @@ int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs
  * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, J < 1, n_pairs < 0. */
 int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream);
 
+/* The pictures of the reference's misc/visualize.py vis_seq (:176-261) from generated frames, in one launch.
+ *   store0 [n0][C][H][H], store1 [n1][C][H][H] fp32 frame stores (a generation graph's input and output buffers, or any
+ *              stacked store); C = 1 (replicated to 3 channels) or 3; square frames, 1 <= H <= 128
+ *   tiles_host [r_len][n_block][6][3] int32, HOST memory: per tile (frame t, row block i, row j) the store (0 / 1), the frame
+ *              in it (-1: an all-zero frame) and the border (0 none, 1 orange (1, 165/255, 0), 2 red (1, 0, 0), 3 pixels
+ *              wide); checked, then copied to tiles_dev (device, same size) on the stream before the launch
+ *   canvas     [3][n_block * 6 * H][r_len * H] fp32: tile (t, i, j) at rows (6 i + j) H, columns t H (the PNG)
+ *   video      [r_len][3][n_block * H][6 * H] fp32: tile (t, i, j) in frame t at rows i H, columns j H (add_video)
+ *   gif        [r_len][n_block * H][6 * H][3] uint8: video frame t, channels last, (uint8)truncf(v * 255.f) (the GIF frames,
+ *              the reference's (frame * 255).astype(np.uint8) for frames in [0, 1])
+ * Every output value is a copy of a frame value, a border constant or that truncation, so all three are bit-identical to
+ * the reference's composition of the same frames.
+ * P2PVG_ERR_BAD_ARG: NULL pointers, C not 1 or 3, H outside 1..128, r_len < 1, n_block < 1, a tile whose store is not 0 / 1,
+ * whose frame is not -1 .. n_store - 1 or whose border is not 0..2.  P2PVG_ERR_UNSUPPORTED: outputs of 2^31 values or more. */
+int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                     int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

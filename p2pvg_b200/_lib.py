@@ -491,3 +491,11 @@ class CudaKernels:
     def pose_metrics(self, pred, gt, pairs, n_pairs, J, out):
         """p2pvg_pose_metrics: out fp64 [n_pairs, 2] = mse, mpjpe of pred[pairs[p, 0]] against gt[pairs[p, 1]] ([.., J, 3])."""
         self._ck(self.lib.p2pvg_pose_metrics(_p(pred), _p(gt), _p(pairs), _i(n_pairs), _i(J), _p(out), self._stream()))
+
+    # -- qualitative pictures ----------------------------------------------------------------
+    def vis_canvas(self, store0, n0, store1, n1, C, H, tiles_host, tiles_dev, r_len, n_block, canvas, video, gif):
+        """p2pvg_vis_canvas: the PNG canvas, video tensor and GIF frames of misc/visualize.py vis_seq from fp32 frame stores
+        [n, C, H, H] and the int32 tile table [r_len, n_block, 6, 3] (tiles_host on the host, tiles_dev its device copy;
+        checked by the library before the launch)."""
+        self._ck(self.lib.p2pvg_vis_canvas(_p(store0), _i(n0), _p(store1), _i(n1), _i(C), _i(H), _vp(tiles_host.ctypes.data),
+                                           _p(tiles_dev), _i(r_len), _i(n_block), _p(canvas), _p(video), _p(gif), self._stream()))

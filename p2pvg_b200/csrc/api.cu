@@ -115,6 +115,8 @@ int p2pvg_pose_windows_impl(const float*, const float*, int, const int64_t*, con
                             int, int, int, float*, float*, cudaStream_t);
 int p2pvg_frame_metrics_impl(const float*, const float*, const int32_t*, int, int, int, int, float, double*, cudaStream_t);
 int p2pvg_pose_metrics_impl(const float*, const float*, const int32_t*, int, int, double*, cudaStream_t);
+int p2pvg_vis_canvas_impl(const float*, int, const float*, int, int, int, const int32_t*, int32_t*, int, int, float*, float*, uint8_t*,
+                          cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -384,6 +386,10 @@ int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs
 }
 int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream) {
   return p2pvg_pose_metrics_impl(pred, gt, pairs, n_pairs, J, out, ST);
+}
+int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                     int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream) {
+  return p2pvg_vis_canvas_impl(store0, n0, store1, n1, C, H, tiles_host, tiles_dev, r_len, n_block, canvas, video, gif, ST);
 }
 
 }  // extern "C"

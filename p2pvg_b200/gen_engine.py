@@ -240,6 +240,34 @@ class GenerateEngine:
         scores = {k: res[i].contiguous() for i, k in enumerate(names)}
         return dict(frames=list(frames), **scores, best=metrics.best_of(scores, names))
 
+    @torch.no_grad()
+    def vis_canvas(self, x, len_output, model_mode, nsample, plan):
+        """vis_seq's generation and composition (p2pvg_b200.visualize): the replay of generate(x, len_output, len_output - 1,
+        model_mode, skip_frame=False, nsample=nsample), then ONE p2pvg_vis_canvas launch that reads the graph's own input and
+        output buffers (no copy of the generated frames).  plan(gt_ref, sample_ref) returns the tile table (see
+        visualize.plan_tiles); gt_ref(t) and sample_ref(s, t) give (store, frame of row 0) of ground-truth frame t and of
+        sample s's frame t, sample_ref None for a skipped (zero) frame.  Returns visualize.compose's (canvas, video, gif)."""
+        from . import visualize
+        G, slots = self._replay(x, len_output, len_output - 1, model_mode, False, True, nsample)
+        c = G.cfg
+        B, rows, n_past = c["B"], c["rows"], c["n_past"]
+        dec, d = {}, 0
+        for (i, _, _, _) in slots[0]:
+            if i >= n_past:
+                dec[i] = d
+                d += 1
+        executed = {i for (i, _, _, _) in slots[0]}
+
+        def sample_ref(s, t):
+            if t == 0 or (t in executed and t < n_past):
+                return 0, t * B
+            if t not in executed:
+                return None
+            return 1, dec[t] * rows + s * B
+
+        tiles = plan(lambda t: (0, t * B), sample_ref)
+        return visualize.compose(G.bufs["x"], G.bufs["out"], tiles, c["fshape"][0], c["W"])
+
     def _replay(self, x, len_output, eval_cp_ix, model_mode, skip_frame, init_hidden, nsample):
         """One call: the one-segment chain over all len(x) frames.  Returns the graph and [executed slots]."""
         return self._run(x, len(x), [(0, len(x), len_output, eval_cp_ix)], model_mode, skip_frame, init_hidden, nsample)
@@ -696,6 +724,10 @@ class PoseGenerateEngine(GenerateEngine):
 
     def _prepare_weights(self):
         pass   # the kernel reads the parameters in place; their addresses are part of the graph's signature
+
+    def vis_canvas(self, *args, **kwargs):
+        raise ValueError("poses are rendered on the host before they are composed: p2pvg_b200.visualize.vis_seq composes "
+                         "the uploaded images")
 
     def _encode(self, tag, frames, N, h_out):
         G, g = self.G, self.model.g_dim
