@@ -32,6 +32,7 @@ struct p2pvg_conv_fusion;
 
 #define P2PVG_F32 0
 #define P2PVG_BF16 1
+#define P2PVG_F64 2 /* p2pvg_histograms segments only */
 
 #define P2PVG_ACT_NONE 0
 #define P2PVG_ACT_LRELU 1 /* LeakyReLU(0.2): models/dcgan_64.py:10,22 */
@@ -477,6 +478,31 @@ int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs,
  * whose frame is not -1 .. n_store - 1 or whose border is not 0..2.  P2PVG_ERR_UNSUPPORTED: outputs of 2^31 values or more. */
 int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
                      int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream);
+
+/* TensorBoard histograms (the reference's train.py:225-233 add_histogram calls) of many device ranges in one launch.
+ *   segs       [n_seg][3] int64, HOST memory: per segment the device address of a contiguous range, its element count
+ *              (>= 1) and its dtype (P2PVG_F32 or P2PVG_F64); the address is aligned to the element size
+ *   edges      [n_edges] fp64, HOST memory: strictly increasing finite bin edges, 2 <= n_edges <= 4096 (p2pvg_b200.tboard
+ *              DEFAULT_BINS holds TensorBoard's 1549 default edges)
+ *   workspace  p2pvg_histograms_workspace_bytes(segs, n_seg, n_edges) bytes, 16-byte aligned: the edge and segment tables
+ *              (staged on the host and copied on the stream before the launch) and fp64 partials of every chunk of
+ *              P2PVG_HIST_CHUNK elements, i.e. 32 * sum_s ceil(count_s / 16384) bytes plus the tables
+ *   counts     [n_seg][n_edges - 1] int64 (8-byte aligned): np.histogram(values.astype(np.float64), bins=edges) -- bins
+ *              [e_k, e_k+1), the last one closed; values below e_0 or above e_last and NaN are not counted; -0.0 counts
+ *              as 0.0.  fp32 values are widened to fp64 exactly (the library is built without -ftz or fast math).
+ *   stats      [n_seg][5] fp64 (8-byte aligned): min, max (numpy's: NaN if any value is NaN, +-inf kept), num (the element
+ *              count), sum and sum of squares of the fp64 values
+ * sum and sum of squares are summed in a fixed order of fixed-size chunks of the segment, so each segment's results are
+ * bit-identical whatever else shares the launch and from run to run; the order is not numpy's, so they match
+ * values.sum() / values.dot(values) to rounding, and exactly when every partial sum is representable.
+ * n_seg == 0 returns P2PVG_OK without a launch (every pointer may then be NULL).
+ * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, n_seg < 0, n_edges < 2, an edge not finite or not above the previous one,
+ * a segment dtype other than F32 / F64, a count < 1.  P2PVG_ERR_UNSUPPORTED: n_edges > 4096, a count >= 2^40.
+ * P2PVG_ERR_WORKSPACE: workspace smaller than the query. */
+#define P2PVG_HIST_CHUNK 16384
+size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_edges);
+int p2pvg_histograms(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* workspace, size_t ws_bytes,
+                     int64_t* counts, double* stats, void* stream);
 
 #ifdef __cplusplus
 }

@@ -34,6 +34,7 @@ def load_library():
         _lib.p2pvg_last_error.restype = ctypes.c_char_p
         _lib.p2pvg_bn_workspace_bytes.restype = ctypes.c_size_t
         _lib.p2pvg_bn_wgrad_c1_partial_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_histograms_workspace_bytes.restype = ctypes.c_size_t
     return _lib
 
 
@@ -499,3 +500,16 @@ class CudaKernels:
         checked by the library before the launch)."""
         self._ck(self.lib.p2pvg_vis_canvas(_p(store0), _i(n0), _p(store1), _i(n1), _i(C), _i(H), _vp(tiles_host.ctypes.data),
                                            _p(tiles_dev), _i(r_len), _i(n_block), _p(canvas), _p(video), _p(gif), self._stream()))
+
+    # -- TensorBoard histograms ------------------------------------------------------------
+    def histograms_workspace_bytes(self, segs_host, n_edges):
+        """Bytes of workspace p2pvg_histograms needs for the int64 host segment table segs_host [n_seg, 3]."""
+        return int(self.lib.p2pvg_histograms_workspace_bytes(_vp(segs_host.ctypes.data), _i(len(segs_host)), _i(n_edges)))
+
+    def histograms(self, segs_host, edges_host, workspace, counts, stats):
+        """p2pvg_histograms: counts int64 [n_seg, n_edges - 1] and stats fp64 [n_seg, 5] (min, max, num, sum, sum_squares) of
+        the segments of segs_host (int64 [n_seg, 3] on the host: address, count, P2PVG_F32 / P2PVG_F64) over the fp64 host
+        edge table edges_host (both checked by the library before the launch)."""
+        self._ck(self.lib.p2pvg_histograms(_vp(segs_host.ctypes.data), _i(len(segs_host)), _vp(edges_host.ctypes.data),
+                                           _i(len(edges_host)), _p(workspace), _sz(workspace.numel() * workspace.element_size()),
+                                           _p(counts), _p(stats), self._stream()))

@@ -117,6 +117,8 @@ int p2pvg_frame_metrics_impl(const float*, const float*, const int32_t*, int, in
 int p2pvg_pose_metrics_impl(const float*, const float*, const int32_t*, int, int, double*, cudaStream_t);
 int p2pvg_vis_canvas_impl(const float*, int, const float*, int, int, int, const int32_t*, int32_t*, int, int, float*, float*, uint8_t*,
                           cudaStream_t);
+size_t p2pvg_histograms_workspace_bytes_impl(const int64_t*, int, int);
+int p2pvg_histograms_impl(const int64_t*, int, const double*, int, void*, size_t, int64_t*, double*, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -390,6 +392,13 @@ int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs,
 int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
                      int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream) {
   return p2pvg_vis_canvas_impl(store0, n0, store1, n1, C, H, tiles_host, tiles_dev, r_len, n_block, canvas, video, gif, ST);
+}
+size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_edges) {
+  return p2pvg_histograms_workspace_bytes_impl(segs, n_seg, n_edges);
+}
+int p2pvg_histograms(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* workspace, size_t ws_bytes,
+                     int64_t* counts, double* stats, void* stream) {
+  return p2pvg_histograms_impl(segs, n_seg, edges, n_edges, workspace, ws_bytes, counts, stats, ST);
 }
 
 }  // extern "C"

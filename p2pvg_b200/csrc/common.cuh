@@ -13,6 +13,7 @@
 
 #define P2PVG_F32 0
 #define P2PVG_BF16 1
+#define P2PVG_F64 2   // only the histogram segments take fp64
 
 #define P2PVG_ACT_NONE 0
 #define P2PVG_ACT_LRELU 1
