@@ -257,7 +257,9 @@ int p2pvg_lstm_cluster_max_clusters(int which);
  *                c_out == c_in is allowed: the state may be updated in place)
  *   head         P2PVG_LSTM_HEAD_LINEAR_TANH: out[rows][out_dim] = tanh(h W_out^T + b_out)
  *                P2PVG_LSTM_HEAD_GAUSSIAN:    mu = h W_out^T + b_out, logvar = h W_out2^T + b_out2, out = eps * exp(logvar / 2) + mu
- *                                             (mu / logvar written when non-NULL)  */
+ *                                             (mu / logvar written when non-NULL)
+ *   counter_rows 0: tuc[0] and dt[0] are the time counters of every row; > 0: row b reads tuc[b / counter_rows] and
+ *                dt[b / counter_rows] (groups of counter_rows rows, e.g. one output length each); negative: P2PVG_ERR_BAD_ARG  */
 #define P2PVG_LSTM_HEAD_LINEAR_TANH 0
 #define P2PVG_LSTM_HEAD_GAUSSIAN 1
 typedef struct p2pvg_lstm_step_module {
@@ -284,6 +286,7 @@ typedef struct p2pvg_lstm_step_module {
   float* out;
   float* mu;
   float* logvar;
+  int counter_rows;
 } p2pvg_lstm_step_module;
 int p2pvg_lstm_step(const p2pvg_lstm_step_module* modules /*host array*/, int n_modules, int rows, int R, void* stream);
 /* One whole call of the h36m pose encoder or decoder (models/h36m_mlp.py:28-95; no BatchNorm, so eval == train) in ONE launch.
@@ -478,6 +481,24 @@ int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs,
  * whose frame is not -1 .. n_store - 1 or whose border is not 0..2.  P2PVG_ERR_UNSUPPORTED: outputs of 2^31 values or more. */
 int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
                      int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream);
+
+/* The pictures of the reference's generate.py (:117-163) for every output length, in one launch: tiles of frames, each with
+ * its control-point border, written into destination images.
+ *   store0 [n0][C][H][H], store1 [n1][C][H][H] fp32 frame stores; C = 1 (replicated to 3 channels) or 3; 1 <= H <= 128
+ *   images_host [n_images][4] int64, HOST memory: per destination image (offset, kind, h, w): kind 0 is fp32 [3][h][w] at
+ *              out_f + offset, kind 1 uint8 [h][w][3] at out_u8 + offset
+ *   tiles_host [n_tiles][6] int32, HOST memory: (store 0 / 1, frame or -1 for zeros, border 0 none / 1 orange / 2 red,
+ *              image, y, x): the H x H frame written at rows y.., columns x.. of the image, channels c -> c (C = 3) or 0
+ *              (C = 1); border pixels (3 wide) are (1, 165 / 255, 0) or (1, 0, 0); uint8 values are (uint8)truncf(v * 255.f)
+ *   tables_dev device workspace, 8-byte aligned, of 32 n_images + 24 n_tiles bytes: the checked tables are copied there on
+ *              the stream before the launch
+ *   out_f      n_f fp32 values, out_u8 n_u8 bytes (either may be NULL when its count is 0)
+ * P2PVG_ERR_BAD_ARG: NULL or misaligned tables, C not 1 or 3, H outside 1..128, n_images < 1, an image of 2^20 rows or
+ * columns or more, or one that does not fit its output, a tile whose store, frame, border or image is out of range or which does not fit its image.  Nothing is copied or
+ * launched then.  n_tiles == 0 returns P2PVG_OK without a launch. */
+int p2pvg_vis_tiles(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                    int n_tiles, const int64_t* images_host, int n_images, void* tables_dev, float* out_f, long long n_f,
+                    uint8_t* out_u8, long long n_u8, void* stream);
 
 /* TensorBoard histograms (the reference's train.py:225-233 add_histogram calls) of many device ranges in one launch.
  *   segs       [n_seg][3] int64, HOST memory: per segment the device address of a contiguous range, its element count

@@ -73,7 +73,7 @@ class LstmStepModule(ctypes.Structure):
                 ("w_embed", ctypes.c_void_p), ("b_embed", ctypes.c_void_p), ("layers", ctypes.c_int), ("layer_w", ctypes.c_void_p),
                 ("state", ctypes.c_void_p), ("head", ctypes.c_int), ("out_dim", ctypes.c_int), ("w_out", ctypes.c_void_p),
                 ("b_out", ctypes.c_void_p), ("w_out2", ctypes.c_void_p), ("b_out2", ctypes.c_void_p), ("eps", ctypes.c_void_p),
-                ("out", ctypes.c_void_p), ("mu", ctypes.c_void_p), ("logvar", ctypes.c_void_p)]
+                ("out", ctypes.c_void_p), ("mu", ctypes.c_void_p), ("logvar", ctypes.c_void_p), ("counter_rows", ctypes.c_int)]
 
 
 LSTM_HEAD_LINEAR_TANH, LSTM_HEAD_GAUSSIAN = 0, 1
@@ -500,6 +500,15 @@ class CudaKernels:
         checked by the library before the launch)."""
         self._ck(self.lib.p2pvg_vis_canvas(_p(store0), _i(n0), _p(store1), _i(n1), _i(C), _i(H), _vp(tiles_host.ctypes.data),
                                            _p(tiles_dev), _i(r_len), _i(n_block), _p(canvas), _p(video), _p(gif), self._stream()))
+
+    def vis_tiles(self, store0, n0, store1, n1, C, H, tiles_host, images_host, tables_dev, out_f, out_u8):
+        """p2pvg_vis_tiles: the tiles of the int32 host table tiles_host [n, 6] (store, frame, border, image, y, x) written into
+        the destination images of the int64 host table images_host [m, 4] (offset, kind, h, w) in out_f (fp32) / out_u8
+        (uint8); tables_dev: a device workspace of 32 m + 24 n bytes.  Checked by the library before the launch."""
+        self._ck(self.lib.p2pvg_vis_tiles(_p(store0), _i(n0), _p(store1), _i(n1), _i(C), _i(H), _vp(tiles_host.ctypes.data),
+                                          _i(len(tiles_host)), _vp(images_host.ctypes.data), _i(len(images_host)), _p(tables_dev),
+                                          _p(out_f), ctypes.c_longlong(0 if out_f is None else out_f.numel()), _p(out_u8),
+                                          ctypes.c_longlong(0 if out_u8 is None else out_u8.numel()), self._stream()))
 
     # -- TensorBoard histograms ------------------------------------------------------------
     def histograms_workspace_bytes(self, segs_host, n_edges):

@@ -117,6 +117,8 @@ int p2pvg_frame_metrics_impl(const float*, const float*, const int32_t*, int, in
 int p2pvg_pose_metrics_impl(const float*, const float*, const int32_t*, int, int, double*, cudaStream_t);
 int p2pvg_vis_canvas_impl(const float*, int, const float*, int, int, int, const int32_t*, int32_t*, int, int, float*, float*, uint8_t*,
                           cudaStream_t);
+int p2pvg_vis_tiles_impl(const float*, int, const float*, int, int, int, const int32_t*, int, const int64_t*, int, void*, float*,
+                         long long, uint8_t*, long long, cudaStream_t);
 size_t p2pvg_histograms_workspace_bytes_impl(const int64_t*, int, int);
 int p2pvg_histograms_impl(const int64_t*, int, const double*, int, void*, size_t, int64_t*, double*, cudaStream_t);
 
@@ -392,6 +394,12 @@ int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs,
 int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
                      int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream) {
   return p2pvg_vis_canvas_impl(store0, n0, store1, n1, C, H, tiles_host, tiles_dev, r_len, n_block, canvas, video, gif, ST);
+}
+int p2pvg_vis_tiles(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                    int n_tiles, const int64_t* images_host, int n_images, void* tables_dev, float* out_f, long long n_f,
+                    uint8_t* out_u8, long long n_u8, void* stream) {
+  return p2pvg_vis_tiles_impl(store0, n0, store1, n1, C, H, tiles_host, n_tiles, images_host, n_images, tables_dev, out_f, n_f,
+                              out_u8, n_u8, ST);
 }
 size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_edges) {
   return p2pvg_histograms_workspace_bytes_impl(segs, n_seg, n_edges);

@@ -21,12 +21,13 @@ constexpr int SLAB = 8;      // batch rows per cluster
 constexpr int NT = 256;      // threads per CTA
 constexpr int NW = NT / 32;
 
-// the module input row b: [ A[ia * rows + b, 0:ga] | Bm[ib * rows + b, 0:gb] | tuc | dt ]
+// the module input row b: [ A[ia * rows + b, 0:ga] | Bm[ib * rows + b, 0:gb] | tuc | dt ], the counters of row b's group
 __device__ __forceinline__ float in_elem(const p2pvg_lstm_step_module& m, int rows, int b, int k) {
   if (k < m.ga) return m.seg_a[((long long)m.idx_a[0] * rows + b) * m.ga + k];
   k -= m.ga;
   if (k < m.gb) return m.seg_b[((long long)m.idx_b[0] * rows + b) * m.gb + k];
-  return k == m.gb ? m.tuc[0] : m.dt[0];
+  const int grp = m.counter_rows > 0 ? b / m.counter_rows : 0;
+  return k == m.gb ? m.tuc[grp] : m.dt[grp];
 }
 
 // full[b][R] <- the slices [b][U] of all CTAs of the cluster
@@ -136,6 +137,7 @@ int p2pvg_lstm_step_impl(const p2pvg_lstm_step_module* mods, int n_mods, int row
                   "lstm_step: module %d input segments", i);
     P2PVG_REQUIRE(m.head == P2PVG_LSTM_HEAD_LINEAR_TANH || (m.head == P2PVG_LSTM_HEAD_GAUSSIAN && m.w_out2 && m.b_out2 && m.eps),
                   P2PVG_ERR_BAD_ARG, "lstm_step: module %d head", i);
+    P2PVG_REQUIRE(m.counter_rows >= 0, P2PVG_ERR_BAD_ARG, "lstm_step: module %d counter_rows %d (needs >= 0)", i, m.counter_rows);
     in_max = max(in_max, m.ga + m.gb + 2);
   }
   if (rows <= 0) return P2PVG_OK;

@@ -4,11 +4,10 @@
 // truncation of v * 255 in fp32, so the three outputs are bit-identical to the reference's torch / NumPy composition of the
 // same frames.
 #include "common.cuh"
+#include "vis_common.cuh"
 
 #define VIS_THREADS 256
 #define VIS_ROWS 6          // rows per block: the ground truth and five samples (misc/visualize.py:105)
-#define VIS_PAD 3           // border width (misc/visualize.py:13, 55)
-#define VIS_MAX_W 128
 
 namespace {
 
@@ -21,7 +20,7 @@ __global__ void __launch_bounds__(VIS_THREADS) vis_canvas_kernel(const float* __
   const int src = tiles[3 * tile], idx = tiles[3 * tile + 1], border = tiles[3 * tile + 2];
   const int W = H, HW = H * W;
   const float* f = idx < 0 ? nullptr : (src == 0 ? s0 : s1) + (size_t)idx * C * HW;
-  const float bc[3] = {1.f, border == 1 ? (float)(165.0 / 255.0) : 0.f, 0.f};
+  const float bc[3] = {vis_border_value(border, 0), vis_border_value(border, 1), vis_border_value(border, 2)};
   const size_t cw = (size_t)r_len * W, ch = (size_t)n_block * VIS_ROWS * H;   // PNG canvas [3][ch][cw]
   const size_t vw = (size_t)VIS_ROWS * W, vh = (size_t)n_block * H;           // video / GIF frame [3][vh][vw]
   float* cv = canvas + (size_t)(i * VIS_ROWS + j) * H * cw + (size_t)t * W;
@@ -29,14 +28,13 @@ __global__ void __launch_bounds__(VIS_THREADS) vis_canvas_kernel(const float* __
   uint8_t* gf = gif + ((size_t)t * vh * vw + (size_t)i * H * vw + (size_t)j * W) * 3;
   for (int p = threadIdx.x; p < HW; p += VIS_THREADS) {
     const int y = p / W, x = p - y * W;
-    const bool edge = border != 0 && !(y >= VIS_PAD && y < W - VIS_PAD && x >= VIS_PAD && x < W - VIS_PAD);
+    const bool edge = vis_is_edge(border, y, x, W);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float v = edge ? bc[c] : (f ? f[(C == 1 ? 0 : c) * HW + p] : 0.f);
       cv[c * ch * cw + (size_t)y * cw + x] = v;
       vd[c * vh * vw + (size_t)y * vw + x] = v;
-      // (v * 255).astype(np.uint8): fp32 product, truncated toward zero, low byte
-      gf[((size_t)y * vw + x) * 3 + c] = (uint8_t)(int)truncf(v * 255.f);
+      gf[((size_t)y * vw + x) * 3 + c] = vis_to_u8(v);
     }
   }
 }

@@ -36,6 +36,13 @@ entry) and counters; the LSTM state stays in the graph's buffers across segments
 clip followed by a copy of each segment's skip source frame, so that the skip halves of all segments are one batched launch
 per stage, of which each decode reads its segment's B images.
 
+``generate_lengths`` (P2PModel.p2p_generate_lengths) replays one call per output length as ONE graph: each length owns a
+group of nsample * B rows, the groups sorted longest first (plan_lengths), so that the rows still generating at step i are a
+prefix of the batch and every launch of step i runs on that prefix only.  A length changes only the time counters (one
+tab_f entry per slot and group, read per row through p2pvg_lstm_step's counter_rows) and the step where its rows stop; the
+other tables are the longest length's.  The module inputs are indexed with the step's row count as stride, so the ground
+truth h source is kept once per distinct active row count; every other buffer is allocated at its first, largest use.
+
 ``evaluate`` (P2PModel.p2p_evaluate) runs the replay of a generate call (or chain) and, instead of assembling the output list,
 scores the decoded frames in the graph's output buffer against the ground truth in its input buffer with one metrics launch
 (metrics.plan_pairs / plan_pairs_multi_cp name the rows).
@@ -132,6 +139,46 @@ def check_cp_ixs(cp_ixs, T, len_outputs, n_past):
     return [(o, Tk, Lk, Lk - 1) for o, Tk, Lk in zip(cps, Ts, Ls)]
 
 
+def check_lengths(len_outputs, T, n_past):
+    """The output lengths of a generate_lengths call on a clip of T frames as a list of ints; ValueError for an empty or
+    malformed len_outputs, a length below 2, or a length L with T < min(n_past, L)."""
+    try:
+        Ls = list(len_outputs)
+        bad = not Ls or any(isinstance(v, bool) or int(v) != v or v < 2 for v in Ls)
+    except (TypeError, ValueError):
+        bad = True
+    if bad:
+        raise ValueError(f"len_outputs must be a non-empty sequence of ints >= 2 (got {len_outputs!r})")
+    Ls = [int(v) for v in Ls]
+    for L in Ls:
+        if n_past < 1 or T < min(n_past, L):
+            raise ValueError(f"len_output {L} needs n_past >= 1 and at least min(n_past, len_output) = {min(n_past, L)} input "
+                             f"frames (got {T})")
+    return Ls
+
+
+def lengths_order(lens):
+    """The row groups of generate_lengths: caller indices sorted by length, longest first, ties in caller order."""
+    return sorted(range(len(lens)), key=lambda k: -lens[k])
+
+
+def plan_lengths(lens, len_x, probs, skip_prob, n_past, group_rows):
+    """The ragged rows of generate_lengths: output length lens[k] is row group order.index(k) (lengths_order) of group_rows
+    rows.  Step i (slot i - 1) runs on the groups whose length is greater than i, which are a prefix of the rows.
+
+    Returns (order, active, floats): the caller index of every group; the active row count of every slot; the float table
+    [time_until_cp | delta_time] of 2 * S * G entries, slot-major, with group g's counters at slot s * G + g (plan_slots'
+    doubles for its own length; zero once the group has stopped)."""
+    order = lengths_order(lens)
+    nG, S = len(lens), max(lens) - 1
+    active = [group_rows * sum(1 for L in lens if L > i) for i in range(1, S + 1)]
+    tuc, dt = [0.0] * (S * nG), [0.0] * (S * nG)
+    for g, k in enumerate(order):
+        for s, (_, t, d, _) in enumerate(plan_slots(lens[k], len_x, probs[k], skip_prob, n_past, False, lens[k] - 1)):
+            tuc[s * nG + g], dt[s * nG + g] = t, d
+    return order, active, tuc + dt
+
+
 def check_supported(model):
     """ValueError unless the model is a dcgan_64 / dcgan_128 P2PModel with every module in eval mode."""
     from .models.backbone import DcganDecoder, DcganEncoder
@@ -191,6 +238,21 @@ class GenerateEngine:
             n_dec = max(Sk - n_tf, 0)
             res.append(self._assemble_seq(G.cfg, out[d:d + n_dec], x[o:o + Tk], sl, Lk))
             d += n_dec
+        return res
+
+    @torch.no_grad()
+    def generate_lengths(self, x, len_outputs, model_mode="full", nsample=1):
+        """generate(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) for every L in len_outputs, in order, as ONE
+        replay: see P2PModel.p2p_generate_lengths."""
+        if isinstance(x, tuple):
+            x = x[1]
+        G, slots, lens, order = self._replay_lengths(x, len_outputs, model_mode, nsample)
+        c = G.cfg
+        out, gr = G.bufs["out"].clone(), c["grows"]
+        res = []
+        for k, L in enumerate(lens):
+            g = order.index(k)
+            res.append(self._assemble_seq(dict(c, rows=gr), out[:, g * gr:(g + 1) * gr], x, slots[0][:L - 1], L))
         return res
 
     @torch.no_grad()
@@ -272,6 +334,16 @@ class GenerateEngine:
         """One call: the one-segment chain over all len(x) frames.  Returns the graph and [executed slots]."""
         return self._run(x, len(x), [(0, len(x), len_output, eval_cp_ix)], model_mode, skip_frame, init_hidden, nsample)
 
+    def _replay_lengths(self, x, len_outputs, model_mode, nsample):
+        """A generate_lengths call: checks before any draw or launch, then the one-segment plan of the longest length over
+        row groups of every length.  Returns the graph, [executed slots of the longest length], the lengths and the group
+        order (lengths_order)."""
+        self._check_model()
+        lens = check_lengths(len_outputs, len(x), int(self.model.opt.n_past))
+        Lmax = max(lens)
+        G, slots = self._run(x, len(x), [(0, len(x), Lmax, Lmax - 1)], model_mode, False, True, nsample, lens=lens)
+        return G, slots, lens, lengths_order(lens)
+
     def _replay_chain(self, x, cp_ixs, len_outputs, model_mode, skip_frame, nsample):
         """A multi-control-point call: checks before any draw or launch, then the chain of segments (offset, T_k, L_k,
         L_k - 1) over the clip's first cp_ixs[-1] + 1 frames.  Returns the graph, the slots per segment and the segments."""
@@ -281,10 +353,14 @@ class GenerateEngine:
         G, slots = self._run(x, T, segs, model_mode, skip_frame, True, nsample)
         return G, slots, segs
 
-    def _run(self, x, T, segs, model_mode, skip_frame, init_hidden, nsample):
+    def _run(self, x, T, segs, model_mode, skip_frame, init_hidden, nsample, lens=None):
         """Steps (1)-(5) of a chain of segments (offset, T_k, L_k, eval_cp_ix_k) on the clip x[:T]: capture on first use of
         the signature, write this call's inputs, replay, and leave the LSTM state in the modules' .hidden as the eager path
-        does.  Returns the graph and the executed slots of each segment."""
+        does.  Returns the graph and the executed slots of each segment.
+
+        lens (generate_lengths; one segment of the longest length, skip_frame False): one row group of nsample * B rows per
+        output length (plan_lengths), each with its own NumPy draw, counters and eps; .hidden is left holding the group of
+        lens[-1]."""
         from . import infer
         model = self.model
         self._check_model()
@@ -298,19 +374,35 @@ class GenerateEngine:
         n_past = int(opt.n_past)
         if n_past < 1 or any(Tk < min(n_past, Lk) for (_, Tk, Lk, _) in segs):
             raise ValueError("p2p_generate_graphed needs n_past >= 1 and at least min(n_past, len_output) input frames")
-        rows = nsample * B
+        nG = 1 if lens is None else len(lens)
+        grows = nsample * B   # rows of one output length
+        rows = nG * grows
         dev = x[0].device
-        # (1) the reference's NumPy draw per segment, made even when skip_frame is False (models/p2p_model.py:128)
-        probs = [np.random.uniform(0, 1, Lk - 1) for (_, _, Lk, _) in segs]
-        slots, ints, fl = plan_segments(segs, T, probs, float(opt.skip_prob), n_past, skip_frame, model_mode)
+        # (1) the reference's NumPy draw per segment (per output length), made even when skip_frame is False
+        # (models/p2p_model.py:128)
+        if lens is None:
+            probs = [np.random.uniform(0, 1, Lk - 1) for (_, _, Lk, _) in segs]
+            slots, ints, fl = plan_segments(segs, T, probs, float(opt.skip_prob), n_past, skip_frame, model_mode)
+            order, feed = [0], None
+        else:
+            probs = [np.random.uniform(0, 1, L - 1) for L in lens]
+            order, active, fl = plan_lengths(lens, T, probs, float(opt.skip_prob), n_past, grows)
+            # the tables the groups share (targets, encoder inputs, z source, global descriptor): the longest length's
+            slots, ints, _ = plan_segments(segs, T, [probs[order[0]]], float(opt.skip_prob), n_past, False, model_mode)
+            feed = [(order.index(k), L - 1) for k, L in enumerate(lens)]   # (group, executed steps) in caller order
         Ss = [len(sl) for sl in slots]
         S = sum(Ss)
+        if lens is None or nG == 1:
+            active = [rows] * S
+        feed = feed or [(0, S)]
         lfs = bool(opt.last_frame_skip)
         adt = infer._act_dtype()
         K = infer.kernels_for(dev)
         ptrs = tuple(p.data_ptr() for p in model.parameters()) + tuple(b.data_ptr() for b in model.buffers())
         # one segment: (len_output, executed steps), as for a single call; a chain: (T_k, L_k, S_k) per segment
         seg_sig = (segs[0][2], S) if len(segs) == 1 else (tuple((Tk, Lk, Sk) for (_, Tk, Lk, _), Sk in zip(segs, Ss)),)
+        if nG > 1:   # generate_lengths: the graph depends on the lengths in group order
+            seg_sig += (tuple(lens[k] for k in order),)
         sig = (rows, B, T, fshape, *seg_sig, model_mode, n_past, lfs, str(adt), ptrs)
         G = self._graphs.get(sig)
         if G is not None and G.ws_gen != K.ws_gen:
@@ -321,7 +413,7 @@ class GenerateEngine:
         # or with last_frame_skip the frame before the segment's first decode.  One segment reads it in place; a chain
         # appends copies of them behind the clip, so that all segments' skip halves come from one batched launch per stage
         src = [o + min(n_tf if lfs else max(n_past - 2, 0), Tk - 1) for (o, Tk, _, _, n_tf) in cseg]
-        cfg = dict(rows=rows, B=B, T=T, fshape=fshape, C=fshape[0], W=fshape[-1], S=S, segs=cseg, src=src,
+        cfg = dict(rows=rows, grows=grows, nG=nG, active=tuple(active), B=B, T=T, fshape=fshape, C=fshape[0], W=fshape[-1], S=S, segs=cseg, src=src,
                    T_enc=T if len(segs) == 1 else T + len(segs), n_dec=sum(max(Sk - n_tf, 0) for (_, _, _, Sk, n_tf) in cseg),
                    mode=model_mode, n_past=n_past, lfs=lfs, adt=adt, ns=nsample, dev=dev)
         if not init_hidden:
@@ -362,13 +454,15 @@ class GenerateEngine:
         if cfg["T_enc"] > T:
             xb[T:].copy_(xs[src].reshape(len(src), B, *fshape))
         G.bufs["tab_int"][:4 * S].copy_(torch.tensor(ints, dtype=torch.int32), non_blocking=True)
-        G.bufs["tab_f"][:2 * S].copy_(torch.tensor(fl, dtype=torch.float64).float(), non_blocking=True)
+        G.bufs["tab_f"][:2 * S * nG].copy_(torch.tensor(fl, dtype=torch.float64).float(), non_blocking=True)
         if S:
             z = model.z_dim
             if infer._EPS_STREAM is not None:
-                for s in range(S):
-                    for j in (0, 1):
-                        G.bufs["eps"][s, j].copy_(infer._EPS_STREAM.pop(0).to(device=dev, dtype=torch.float32).reshape(rows, z))
+                for g, Sg in feed:
+                    for s in range(Sg):
+                        for j in (0, 1):
+                            G.bufs["eps"][s, j, g * grows:(g + 1) * grows].copy_(
+                                infer._EPS_STREAM.pop(0).to(device=dev, dtype=torch.float32).reshape(grows, z))
             else:
                 torch.randn(S, 2, rows, z, device=dev, out=G.bufs["eps"])
         for m in ("posterior", "prior", "frame_predictor"):
@@ -380,11 +474,13 @@ class GenerateEngine:
                 for l, (h, c) in enumerate(getattr(model, m).hidden):
                     hs[l].copy_(h)
                     cs[l].copy_(c)
-        # (5) replay, LSTM state written back as the eager path leaves it
+        # (5) replay, LSTM state written back as the eager path leaves it (the rows of the last output length)
         G.graph.replay()
+        r0 = 0 if lens is None else order.index(len(lens) - 1) * grows
+        r1 = r0 + (rows if lens is None else grows)
         for m in ("posterior", "prior", "frame_predictor"):
             hs, cs = G.bufs[f"{m}_h"], G.bufs[f"{m}_c"]
-            getattr(model, m).hidden = [(hs[l].clone(), cs[l].clone()) for l in range(hs.shape[0])]
+            getattr(model, m).hidden = [(hs[l, r0:r1].clone(), cs[l, r0:r1].clone()) for l in range(hs.shape[0])]
         return G, slots
 
     def _assemble(self, G, x, slots, len_output):
@@ -446,7 +542,7 @@ class GenerateEngine:
         b = G.bufs
         b["x"] = torch.zeros(c["T_enc"] * c["B"], *c["fshape"], device=dev)
         b["tab_int"] = torch.zeros(max(4 * S, 1), dtype=torch.int32, device=dev)
-        b["tab_f"] = torch.zeros(max(2 * S, 1), device=dev)
+        b["tab_f"] = torch.zeros(max(2 * S * c["nG"], 1), device=dev)
         b["eps"] = torch.zeros(max(S, 1), 2, rows, model.z_dim, device=dev)
         n_dec = c["n_dec"]
         b["out"] = torch.zeros(max(n_dec, 1), rows, *c["fshape"], device=dev)[:n_dec]
@@ -456,11 +552,14 @@ class GenerateEngine:
                 b[f"{m}_{k}"] = torch.zeros(mod.n_layers, rows, mod.hidden_size, device=dev)   # updated in place by the graph
 
     def _buf(self, G, name, numel, dtype=torch.float32):
+        """Buffer `name` of numel elements.  With several output lengths (generate_lengths) a request may be a prefix of the
+        buffer: it is allocated at its first request, which is its largest, as the active row count of the steps never grows
+        (plan_lengths)."""
         t = G.bufs.get(name)
         if t is None:
             t = G.bufs[name] = torch.zeros(int(numel), dtype=dtype, device=G.cfg["dev"])
-        assert t.numel() == numel and t.dtype == dtype, name
-        return t
+        assert t.dtype == dtype and (t.numel() == numel or (G.cfg["nG"] > 1 and t.numel() > numel)), name
+        return t if t.numel() == numel else t[:numel]
 
     # ------------------------------------------------------------------ the captured sequence
     def _body(self, G):
@@ -477,10 +576,19 @@ class GenerateEngine:
         N = c["T_enc"] * B
         h_gt = self._buf(G, "gt_h", N * g)
         gt_skips = self._encode("gt", G.bufs["x"], N, h_gt)
-        Hsrc = self._buf(G, "Hsrc", (T + 1) * rows * g)     # [T + 1][rows][g]: ground truth frames, then this step's h
-        K.permute4(h_gt, Hsrc, (T, c["ns"], B * g, 1), (B * g, 0, 1, 0))
-        h_cur = Hsrc[T * rows * g:]
-        self._buf(G, "grp_zero", max(c["ns"], 1), torch.int32)   # source image n % B for every sample
+        hsrc = {}
+
+        def Hsrc(M):
+            """[T + 1][M][g] for a step on M rows: the ground truth frames, then this step's h (the module input tables
+            index rows with stride M)"""
+            t = hsrc.get(M)
+            if t is None:
+                t = hsrc[M] = self._buf(G, "Hsrc" if M == rows else f"Hsrc{M}", (T + 1) * M * g)
+                K.permute4(h_gt, t, (T, M // B, B * g, 1), (B * g, 0, 1, 0))
+            return t
+
+        Hsrc(rows)
+        self._buf(G, "grp_zero", max(rows // B, 1), torch.int32)   # source image n % B for every sample
 
         # the skip sources of all segments: one frame in place (one segment), or the nK copies behind the clip (a chain)
         f0 = c["src"][0] if nK == 1 else T
@@ -490,6 +598,8 @@ class GenerateEngine:
             # models/p2p_model.py:143-144: the last skip set while i == 1 or i < n_past comes from x_k[max(n_past - 2, 0)]
             halves0 = self._skip_halves("skip", src_skips, nK * B)
         ti, tf = G.bufs["tab_int"], G.bufs["tab_f"]
+        nG, active = c["nG"], c["active"]
+        cr = c["grows"] if nG > 1 else 0   # rows per counter group (one group: the counters apply to every row)
         zbuf = self._buf(G, "Z", 2 * rows * z)
         h_pred = self._buf(G, "h_pred", rows * g)
         eps = G.bufs["eps"]
@@ -497,29 +607,32 @@ class GenerateEngine:
         for k, (_, _, _, Sk, n_tf) in enumerate(segs):
             prev_frame = None
             for j in range(Sk):
-                tuc, dt = tf[s:s + 1], tf[S + s:S + s + 1]
+                M = active[s]   # the rows still generating: a prefix
+                Hs = Hsrc(M)
+                zb = zbuf[:2 * M * z]
+                tuc, dt = tf[s * nG:(s + 1) * nG], tf[(S + s) * nG:(S + s + 1) * nG]
                 skips_cur = None
                 if j > n_tf:   # the previous step's decoded frame: the only autoregressive encoder call
-                    skips_cur = self._encode("step", prev_frame, rows, h_cur)
+                    skips_cur = self._encode("step", prev_frame, M, Hs[T * M * g:])
                 glob = ti[3 * S + s:3 * S + s + 1]
                 # posterior || prior in one launch, then the frame predictor (models/p2p_model.py:150-179)
-                K.lstm_step([self._module("posterior", Hsrc, ti[s:s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 0], out=zbuf[:rows * z]),
-                             self._module("prior", Hsrc, ti[S + s:S + s + 1], Hsrc, glob, g, tuc, dt, eps=eps[s, 1],
-                                          out=zbuf[rows * z:])], rows, model.rnn_size)
-                K.lstm_step([self._module("frame_predictor", Hsrc, ti[S + s:S + s + 1], zbuf, ti[2 * S + s:2 * S + s + 1], z, tuc,
-                                          dt, out=h_pred)], rows, model.rnn_size)
+                K.lstm_step([self._module("posterior", Hs, ti[s:s + 1], Hs, glob, g, tuc, dt, cr, eps=eps[s, 0], out=zb[:M * z]),
+                             self._module("prior", Hs, ti[S + s:S + s + 1], Hs, glob, g, tuc, dt, cr, eps=eps[s, 1],
+                                          out=zb[M * z:])], M, model.rnn_size)
+                K.lstm_step([self._module("frame_predictor", Hs, ti[S + s:S + s + 1], zb, ti[2 * S + s:2 * S + s + 1], z, tuc,
+                                          dt, cr, out=h_pred)], M, model.rnn_size)
                 s += 1
                 if j < n_tf:
                     continue   # teacher-forced step: the predictor only advances its state (models/p2p_model.py:157-163)
                 if c["lfs"] and j > n_tf:
-                    halves = self._skip_halves("skip", skips_cur, rows)
+                    halves = self._skip_halves("skip", skips_cur, M)
                 else:
                     if halves0 is None:   # last_frame_skip: every segment's first decode, batched at the chain's first
                         halves0 = self._skip_halves("skip0", src_skips, nK * B)
                     halves = self._segment_halves(halves0, k, nK)
                 prev_frame = G.bufs["out"][d]
                 d += 1
-                self._decode(h_pred, halves, prev_frame)
+                self._decode(h_pred, halves, prev_frame, M)
 
     def _segment_halves(self, halves, k, nK):
         """Segment k's part of skip halves computed for the nK segments' sources at once (B images each)."""
@@ -634,10 +747,10 @@ class GenerateEngine:
             Hi *= 2
         return out
 
-    def _decode(self, h_pred, halves, frame_out):
-        """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied)."""
+    def _decode(self, h_pred, halves, frame_out, rows):
+        """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied), on the first rows rows."""
         K, G, model = self.K, self.G, self.model
-        adt, rows = G.cfg["adt"], G.cfg["rows"]
+        adt = G.cfg["adt"]
         dec, g = model.decoder, model.g_dim
         n = len(self.chans)
         ctop = self.chans[-1]
@@ -684,9 +797,10 @@ class GenerateEngine:
         nhwc_to_nchw(K, out32, frame_out, rows, W * W, nc)
 
     # ------------------------------------------------------------------ recurrent modules
-    def _module(self, m, seg_a, idx_a, seg_b, idx_b, gb, tuc, dt, eps=None, out=None):
+    def _module(self, m, seg_a, idx_a, seg_b, idx_b, gb, tuc, dt, counter_rows, eps=None, out=None):
         """p2pvg_lstm_step operands of module m for one step: input [seg_a[idx_a] | seg_b[idx_b] | tuc | dt], state updated in
-        place in the graph's [L][rows][R] buffers, gaussian head (with eps) or Linear + tanh head."""
+        place in the graph's [L][rows][R] buffers, gaussian head (with eps) or Linear + tanh head; counter_rows > 0: row b
+        reads the counters tuc[b / counter_rows], dt[b / counter_rows]."""
         from ._lib import LSTM_HEAD_GAUSSIAN, LSTM_HEAD_LINEAR_TANH
         G, mod = self.G, getattr(self.model, m)
         dev = G.cfg["dev"]
@@ -697,7 +811,7 @@ class GenerateEngine:
             st = [t.data_ptr() for l in range(mod.n_layers) for t in (hs[l], cs[l], hs[l], cs[l])]
             tabs = G.bufs[f"{m}_ptrs"] = torch.tensor(w + st, dtype=torch.int64, device=dev)
         L = mod.n_layers
-        d = dict(seg_a=seg_a, idx_a=idx_a, ga=self.model.g_dim, seg_b=seg_b, idx_b=idx_b, gb=gb, tuc=tuc, dt=dt,
+        d = dict(seg_a=seg_a, idx_a=idx_a, ga=self.model.g_dim, seg_b=seg_b, idx_b=idx_b, gb=gb, tuc=tuc, dt=dt, counter_rows=counter_rows,
                  w_embed=mod.embed.weight, b_embed=mod.embed.bias, layers=L, layer_w=tabs[:4 * L], state=tabs[4 * L:], out=out)
         if hasattr(mod, "mu_net"):
             d.update(head=LSTM_HEAD_GAUSSIAN, out_dim=mod.output_size, w_out=mod.mu_net.weight, b_out=mod.mu_net.bias,
@@ -744,6 +858,6 @@ class PoseGenerateEngine(GenerateEngine):
             return halves
         return [s[k * s.numel() // nK:(k + 1) * s.numel() // nK] for s in skips], nsrc // nK
 
-    def _decode(self, h_pred, halves, frame_out):
+    def _decode(self, h_pred, halves, frame_out, rows):
         skips, nsrc = halves
-        self.K.pose_mlp(self.model.decoder, True, h_pred, frame_out, self.G.cfg["rows"], skips=skips, nsrc=nsrc)
+        self.K.pose_mlp(self.model.decoder, True, h_pred, frame_out, rows, skips=skips, nsrc=nsrc)

@@ -209,10 +209,10 @@ class VggGenerateEngine(GenerateEngine):
             out.append((addS, nsrc))
         return out
 
-    def _decode(self, h_pred, halves, frame_out):
-        """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied)."""
+    def _decode(self, h_pred, halves, frame_out, rows):
+        """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied), on the first rows rows."""
         K, G, model = self.K, self.G, self.model
-        adt, rows = G.cfg["adt"], G.cfg["rows"]
+        adt = G.cfg["adt"]
         dec, g = model.decoder, model.g_dim
         if adt == torch.float32:
             hp = h_pred

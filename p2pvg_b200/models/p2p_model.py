@@ -220,6 +220,19 @@ class P2PModel(nn.Module):
         return self._graphed_engine().generate_multi_cp(x, cp_ixs, len_outputs=len_outputs, model_mode=model_mode,
                                                         skip_frame=skip_frame, nsample=nsample)
 
+    def p2p_generate_lengths(self, x, len_outputs, model_mode='full', nsample=1):
+        """One start/end pair generated at several output lengths as ONE CUDA-graph replay (an addition to the reference API;
+        see gen_engine.py).  Returns one result per entry of len_outputs, in order: what the looped calls
+
+            [p2p_generate_graphed(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) for L in len_outputs]
+
+        return, with the same NumPy draws (one per length, in order), the same eps consumption under infer.eps_stream and
+        .hidden left holding the rows of len_outputs[-1].  The rows of every length share the replay: step i runs on the
+        lengths greater than i only.  x: what p2p_generate_graphed takes.  The same models as p2p_generate_graphed;
+        ValueError before any draw or launch for an empty or malformed len_outputs, a length below 2 or a length L with
+        len(x) < min(n_past, L)."""
+        return self._graphed_engine().generate_lengths(x, len_outputs, model_mode=model_mode, nsample=nsample)
+
     def p2p_evaluate(self, x, nsample=1, len_output=None, model_mode='full', data_range=1.0, cp_ixs=None):
         """Generate and score in one call (an addition to the reference API): exactly what
         p2p_generate_graphed(x, L, L - 1, model_mode, skip_frame=False, nsample=nsample) generates (same draws, same cached
