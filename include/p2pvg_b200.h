@@ -377,6 +377,21 @@ int p2pvg_mse_plain(const float* pred, const float* x, const int* tgt, const flo
 /* the four scalars returned by P2PModel.forward (models/p2p_model.py:271): out[0..3] = mse,kld,cpc,align (/seq_len). */
 int p2pvg_finalize_losses(const float* mse_partial, int n_recon, int has_cpc, double E, const float* kl_sum, float batch_size,
                           const float* align_partial, int n_align, float seq_len, float* out, void* stream);
+/* Held-out scoring (P2PModel.p2p_losses): the four terms of P2PModel.forward's objective (models/p2p_model.py:224-257, /seq_len)
+ * split by batch row, from the buffers of an eval-mode forward with S executed steps and G = S + 1 decodes.
+ *   rec        [G][B][E] decoded frames (dtype P2PVG_F32 / P2PVG_BF16; pre-sigmoid when sigmoid != 0), decode S = the CPC decode
+ *   x          [T][B][E] fp32 targets in the same element order; decode s is scored against x[tgt[s]] (tgt[S] = T - 1)
+ *   mu, lv, mu_p, lv_p  [S][B][z] fp32 posterior / prior heads;  H [T][B][g] fp32 latents;  h_pred [G][B][g] fp32
+ *   in_idx     [>= S - 1]: step s < S - 1 adds MSE(H[in_idx[s]][0] broadcast, h_pred[s]) (the reference's h[0] quirk)
+ *   partial    [G * B][3] fp64 workspace;  counter: one uint32, zero before the first launch and left zero by every launch
+ *   per_seq    [4][B] fp64: row b's mse, kld, cpc, align -- element means over row b (kld: its KL sum / batch_size), / seq_len
+ *   out        [4] fp64: mse, cpc, align = the row means of per_seq, kld = its row sum (the values forward returns)
+ * Fixed-order fp64 sums, no float atomics: repeated launches on the same data are bit-identical.  E: 1..4 image channels
+ * at any size, or 51 for [17, 3] poses.  One launch; streams rec and the scored frames of x once. */
+int p2pvg_seq_losses(const void* rec, int dtype, int sigmoid, const float* x, const int* tgt, int S, int B, int64_t E,
+                     const float* mu, const float* lv, const float* mu_p, const float* lv_p, int z, const float* H,
+                     const int* in_idx, const float* h_pred, int g, int has_cpc, double batch_size, double seq_len,
+                     double* partial, uint32_t* counter, double* per_seq, double* out, void* stream);
 /* Early read-back of the step's scalars (models/p2p_model.py:271 returns them as host numbers: `mse.data.cpu().numpy()`): the
  * kernel stores src[0..n) and then *seq into page-locked, device-mapped host memory host_mapped[0..n] (n floats + one int);
  * the host polls host_mapped[n] for the sequence number it wrote to *seq before launching.  The values are final once the

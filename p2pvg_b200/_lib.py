@@ -440,6 +440,16 @@ class CudaKernels:
                                                 _f(batch_size), _p(align_partial), _i(n_align), _f(seq_len), _p(out),
                                                 self._stream()))
 
+    def seq_losses(self, rec, sigmoid, x, tgt, S, B, E, mu, lv, mu_p, lv_p, z, H, in_idx, h_pred, g, has_cpc, batch_size, seq_len,
+                   partial, counter, per_seq, out):
+        """p2pvg_seq_losses: per_seq fp64 [4, B] (mse, kld, cpc, align of every row) and out fp64 [4] of an eval-mode forward;
+        partial fp64 [(S + 1) * B * 3] and counter int32 [1] (zero before the first launch, left zero) are its workspace."""
+        assert partial.dtype == per_seq.dtype == out.dtype == torch.float64 and counter.dtype == torch.int32
+        self._ck(self.lib.p2pvg_seq_losses(_p(rec), _i(_dt(rec)), _i(int(sigmoid)), _p(x), _p(tgt), _i(S), _i(B), _i64(E), _p(mu), _p(lv),
+                                           _p(mu_p), _p(lv_p), _i(z), _p(H), _p(in_idx), _p(h_pred), _i(g), _i(int(has_cpc)),
+                                           _d(float(batch_size)), _d(float(seq_len)), _p(partial), _p(counter), _p(per_seq), _p(out),
+                                           self._stream()))
+
     def adam(self, p, g, m, v, n, lr, beta1, beta2, eps, step_t):
         self._ck(self.lib.p2pvg_adam_legacy(_p(p), _p(g), _p(m), _p(v), _i64(n), _d(lr), _d(beta1), _d(beta2), _d(eps),
                                             _p(step_t), self._stream()))

@@ -96,6 +96,9 @@ int p2pvg_reparam_kl_bwd_impl(const float*, const float*, const float*, const fl
 int p2pvg_build_concat_impl(float*, const float*, const int*, int, const float*, const int*, int, const float*, const float*, int, int,
                             int, cudaStream_t);
 int p2pvg_gather_add_cols_impl(float*, const float*, const int*, int, int, int, int, int, int, int, cudaStream_t);
+int p2pvg_seq_losses_impl(const void*, int, int, const float*, const int*, int, int, long long, const float*, const float*,
+                          const float*, const float*, int, const float*, const int*, const float*, int, int, double, double, double*,
+                          unsigned int*, double*, double*, cudaStream_t);
 int p2pvg_align_impl(const float*, const int*, const float*, int, int, int, float, float*, float*, float*, cudaStream_t);
 int p2pvg_colsum_impl(const void*, int, long long, int, long long, float*, int, void*, size_t, cudaStream_t);
 int p2pvg_act_fwd_impl(float*, long long, int, cudaStream_t);
@@ -322,6 +325,13 @@ int p2pvg_build_concat(float* dst, const float* A, const int* ia, int ga, const 
 int p2pvg_gather_add_cols(float* dst, const float* src, const int* idx, int S, int T, int B, int g, int W, int col0, int init,
                           void* stream) {
   return p2pvg_gather_add_cols_impl(dst, src, idx, S, T, B, g, W, col0, init, ST);
+}
+int p2pvg_seq_losses(const void* rec, int dtype, int sigmoid, const float* x, const int* tgt, int S, int B, int64_t E,
+                     const float* mu, const float* lv, const float* mu_p, const float* lv_p, int z, const float* H,
+                     const int* in_idx, const float* h_pred, int g, int has_cpc, double batch_size, double seq_len,
+                     double* partial, uint32_t* counter, double* per_seq, double* out, void* stream) {
+  return p2pvg_seq_losses_impl(rec, dtype, sigmoid, x, tgt, S, B, E, mu, lv, mu_p, lv_p, z, H, in_idx, h_pred, g, has_cpc,
+                               batch_size, seq_len, partial, counter, per_seq, out, ST);
 }
 int p2pvg_align(const float* H, const int* in_idx, const float* h_pred, int P, int B, int g, float coef, float* loss_partial,
                 float* d_hpred, float* dH, void* stream) {

@@ -213,6 +213,12 @@ class TrainEngine:
             self._pub_seq_dev = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.last_plan = None
         self.phase_events = None
+        # eval-mode forward (evaluate_losses): BatchNorm from running statistics, no statistics passes, no running-statistics
+        # update; its CUDA graphs are kept apart from the step's
+        self._eval = False
+        self._eval_graphs = {}
+        self._eval_bn = {}
+        self._eval_bufs, self._eval_buf_gen = {}, 0
 
     # ------------------------------------------------------------------ side streams ("lanes")
     # lane 0 = the caller's stream.  lane 1: the prior LSTM while the posterior runs on lane 0 (independent recurrences until
@@ -263,6 +269,18 @@ class TrainEngine:
     def buf(self, name, numel, dtype=None):
         dtype = dtype or self.adt
         t = self._bufs.get(name)
+        if self._eval:
+            # the eval-mode forward reads and writes a step buffer that is already large enough (its contents do not carry
+            # from one step to the next); anything else comes from a pool of its own, whose growth leaves the step's
+            # graphs valid
+            if t is not None and t.numel() >= numel and t.dtype == dtype:
+                return t
+            e = self._eval_bufs.get(name)
+            if e is None or e.numel() < numel or e.dtype != dtype:
+                if e is not None:
+                    self._eval_buf_gen += 1
+                e = self._eval_bufs[name] = torch.zeros(int(numel), dtype=dtype, device=self.dev)
+            return e
         if t is None or t.numel() < numel or t.dtype != dtype:
             if t is not None:
                 # a captured CUDA graph holds the raw address of every buffer it touched: once one of them is
@@ -276,6 +294,10 @@ class TrainEngine:
         """Changes whenever a buffer a captured graph may have baked in was re-allocated (engine pool or the
         kernel backend's workspaces)."""
         return (self._buf_gen, getattr(self.K, "ws_gen", 0))
+
+    def eval_graph_generation(self):
+        """The same for an eval-mode graph, which may also hold buffers of the eval pool."""
+        return self.graph_generation() + (self._eval_buf_gen,)
 
     def fbuf(self, name, numel):
         return self.buf(name, numel, torch.float32)
@@ -294,8 +316,9 @@ class TrainEngine:
             return f"upc{k + 2}.main.0", f"upc{k + 2}.main.1"
         return f"upc{self.n + 1}.0", None
 
-    def pack_weights(self, which=("encoder", "decoder")):
-        """fp32 master weights -> GEMM-layout copies in the activation dtype (layouts.pack_conv4 / pack_convt4)."""
+    def pack_weights(self, which=("encoder", "decoder"), backward=True):
+        """fp32 master weights -> GEMM-layout copies in the activation dtype (layouts.pack_conv4 / pack_convt4).  backward=False:
+        only the copies the forward phases read (the dcgan stacks have no backward-only copies)."""
         K = self.K
         if "encoder" in which:
             P = self.arena["encoder"].p
@@ -331,10 +354,10 @@ class TrainEngine:
                     tile_bias(K, P[cn + ".bias"], b16, 16)
                     self._packed["dec-1.bias16"] = b16
 
-    def pack_lstm_weights(self):
+    def pack_lstm_weights(self, backward=True):
         """Tensor-core (TF32) mode only: K-major fp32 copies of the LSTM weights for the GEMMs whose natural
         operand layout is MN-major (data gradients), and a zero-padded embed weight so that the row pitch of
-        the 258 / 140-wide inputs is TMA-compatible."""
+        the 258 / 140-wide inputs is TMA-compatible.  backward=False: the padded embed weight only (the forward GEMMs)."""
         if not self.tc_lstm:
             return
         K = self.K
@@ -349,6 +372,8 @@ class TrainEngine:
             wp = self.fbuf(f"{m}_embed_pad", R * in_p)
             K.permute4(w, wp, (R, in_p, 1, 1), (in_dim, 1, 0, 0))
             self._packed[f"{m}.embed_pad"] = wp
+            if not backward:
+                continue
             for name, shape in [("embed.weight", (R, in_dim))] + [(f"lstm.{l}.weight_{k}", (4 * R, R)) for l in range(self.lstm_layers(m)) for k in ("ih", "hh")] + \
                     ([("output.0.weight", (self.g, R))] if m == "frame_predictor" else []):
                 o, i = shape
@@ -499,6 +524,117 @@ class TrainEngine:
         st[0].replay()
         self.K.launches += st[1]
         return self._bufs["loss_out"][:4]
+
+    # ------------------------------------------------------------------ eval-mode forward (held-out scoring)
+    def evaluate_losses(self, x, probs=None, eps=None, use_graph=False):
+        """The forward half of step() with every module in eval mode: BatchNorm normalises with its running statistics, and
+        no backward pass, optimiser step, running-statistics update or collective runs.  Parameters, gradients, Adam moments
+        and BatchNorm buffers are left as they are.  x, probs, eps: as for step() (drawn in the same order when None).
+        Returns (plan, per_seq, out): per_seq fp64 [4, B] device tensor of every row's (mse, kld, cpc, align), out fp64 [4]
+        the four scalars forward returns (p2pvg_seq_losses); both are fresh tensors."""
+        T, B = int(x.shape[0]), int(x.shape[1])
+        opt = self.opt
+        if probs is None:
+            probs = np.random.uniform(0, 1, T - 1)
+        sched = skip_schedule(T, probs, opt["skip_prob"], opt["n_past"])
+        pkey = (T, tuple(i for i, _, _ in sched), bool(opt["last_frame_skip"]), int(opt["n_past"]))
+        plan = self._plans.get(pkey)
+        if plan is None:
+            if len(self._plans) > 4096:
+                self._plans.clear()
+            plan = self._plans[pkey] = StepPlan(T, probs, opt)
+        self.T, self.B, self.S = T, B, plan.S
+        if eps is None:
+            eps = torch.randn(plan.S, 2, B, self.z, device=self.dev, dtype=torch.float32)
+        ukey = (pkey, B, float(opt["weight_cpc"]), self.graph_generation())
+        if ukey != self._uploaded:
+            self.upload_plan(plan)
+            self._uploaded = ukey
+        fuse_stats, self.fuse_stats = self.fuse_stats, False   # no statistics epilogues: BatchNorm uses running statistics
+        self._eval = True
+        try:
+            if use_graph:
+                self._eval_graphed(x, eps, plan)
+            else:
+                self.eps = eps.contiguous()
+                self._run_eval(x, plan)
+        finally:
+            self._eval, self.fuse_stats = False, fuse_stats
+        return plan, self._seq_per[:4 * B].view(4, B).clone(), self._seq_out[:4].clone()
+
+    def _eval_graphed(self, x, eps, plan):
+        """evaluate_losses as a CUDA-graph replay, managed like _step_graphed (eager run, capture, replays) in a graph table of
+        its own, checked against eval_graph_generation: another skip pattern of the same signature only refreshes the index
+        tables, and nothing allocated here invalidates the step's graphs."""
+        key = plan.key + (self.B, tuple(x.shape[2:]), int(self.opt["batch_size"]))
+        xs = self.fbuf("x_eval_static", x.numel()).view(-1)[:x.numel()].view(x.shape)
+        es = self.fbuf("eps_eval_static", eps.numel()).view(-1)[:eps.numel()].view(eps.shape)
+        xs.copy_(x, non_blocking=True)
+        es.copy_(eps, non_blocking=True)
+        self.eps = es
+        st = self._eval_graphs.get(key)
+        if st is not None and st != "warm" and st[2] != self.eval_graph_generation():
+            st = None
+        if st is None:
+            gen0 = self.eval_graph_generation()
+            self._run_eval(xs, plan)
+            if self.eval_graph_generation() != gen0:
+                self._eval_graphs.clear()
+            self._eval_graphs[key] = "warm"
+            return
+        if st == "warm":
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            n0 = self.K.launches
+            gen0 = self.eval_graph_generation()
+            with torch.cuda.graph(g):
+                self._run_eval(xs, plan)
+            if self.eval_graph_generation() != gen0:
+                raise RuntimeError("a buffer was re-allocated during CUDA-graph capture (the warm-up run must size every buffer)")
+            self._eval_graphs[key] = st = (g, self.K.launches - n0, gen0)
+        st[0].replay()
+        self.K.launches += st[1]
+
+    def _run_eval(self, x, plan):
+        self.pack_weights(backward=False)   # only the copies the forward phases read
+        self.pack_lstm_weights(backward=False)
+        self.eval_bn_coeffs()
+        self.encode(x, plan)
+        self.recurrent_fwd(plan)
+        self.decode(plan)
+        self.seq_losses_fwd(plan)
+        self.join()
+
+    def eval_bn_coeffs(self):
+        """Per-channel scale / shift of every BatchNorm layer from its running statistics, once per call (p2pvg_bn_eval_coeffs),
+        looked up by bn_forward through the layer's weight."""
+        for m in ("encoder", "decoder"):
+            P, Bf = self.arena[m].p, self.buffers[m]
+            for k in Bf:
+                if not k.endswith(".running_mean"):
+                    continue
+                pre = k[:-len(".running_mean")]
+                gamma = P[pre + ".weight"]
+                C = gamma.numel()
+                sc, sh = self.fbuf(f"evbn_{m}.{pre}.scale", C), self.fbuf(f"evbn_{m}.{pre}.shift", C)
+                self.K.bn_eval_coeffs(gamma, P[pre + ".bias"], Bf[k], Bf[pre + ".running_var"], C, sc, sh)
+                self._eval_bn[gamma.data_ptr()] = (sc, sh)
+
+    def decoded(self):
+        """The decoded frames of all S+1 decoder calls ([S+1, B, E], decoder call major) and whether the output Sigmoid is
+        still to be applied."""
+        return self.dec[-1]["raw"], True
+
+    def seq_losses_fwd(self, plan):
+        B, S = self.B, self.S
+        rec, sigmoid = self.decoded()
+        partial = self.buf("seq_partial", (S + 1) * B * 3, torch.float64)
+        counter = self.buf("seq_counter", 1, torch.int32)
+        per = self._seq_per = self.buf("seq_per", 4 * B, torch.float64)
+        out = self._seq_out = self.buf("seq_out", 4, torch.float64)
+        self.K.seq_losses(rec, sigmoid, self.x_nhwc, self.ix["tgt_idx"], S, B, self.frame_elems, self.mu, self.lv, self.mu_p, self.lv_p,
+                          self.z, self.Hlat, self.ix["in_idx"], self.h_pred, self.g, plan.has_cpc, float(self.opt["batch_size"]),
+                          float(self.T), partial, counter, per, out)
 
     def _mark(self, name):
         """Phase timing for profiling (eager mode only): tools/profile_step.py --phases."""
@@ -667,10 +803,10 @@ class TrainEngine:
         else:
             self.Hlat = self.fbuf("Hlat", N * self.g)
             cast(K, y, self.Hlat, N * self.g)
-        # running statistics: one EMA update per reference call, in call order
+        # running statistics: one EMA update per reference call, in call order (training mode only)
         ncalls = len(plan.enc_order)
         Bf = self.buffers["encoder"]
-        for l in range(n + 1):
+        for l in range(0 if self._eval else n + 1):
             st = self.enc[l]["st"] if l < n else self.enc_final["st"]
             bn = self.enc_names(l)[1]
             K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], st["mean"], st["varu"], self.ix["enc_order"], ncalls,
@@ -689,8 +825,13 @@ class TrainEngine:
 
     def bn_forward(self, tag, idx, raw, y, G, R, C, gamma, beta, act, tiles=None):
         """Batch statistics per group + normalise + activation.  tiles: statistics partials already produced by the
-        epilogue of the GEMM that wrote `raw` (stat_buf) -- then only the tiny finalize kernel runs instead of a pass over raw."""
+        epilogue of the GEMM that wrote `raw` (stat_buf) -- then only the tiny finalize kernel runs instead of a pass over raw.
+        Eval mode: the running-statistics coefficients of this layer (eval_bn_coeffs), the same for every group."""
         K = self.K
+        if self._eval:
+            scale, shift = self._eval_bn[gamma.data_ptr()]
+            K.bn_act(raw, y, scale, shift, 1, G * R, C, act)
+            return dict(G=G, R=R, C=C, act=act, gamma=gamma)
         names = ("mean", "invstd", "varu", "scale", "shift", "sdz", "sdzx")
         st = {nm: self.fbuf(f"{tag}_bn{idx}_{nm}", G * C) for nm in names}
         st.update(G=G, R=R, C=C, act=act, gamma=gamma)
@@ -849,7 +990,7 @@ class TrainEngine:
                 else:
                     K.gemm(d, wD, colD, Md, 16 * cout, cd, b_mn=True)
                     K.gemm(skip, wS, colS, Ms, 16 * cout, cd, b_mn=True)
-                if k == n - 1 and cout in (1, 3) and self.fuse_last:
+                if k == n - 1 and cout in (1, 3) and self.fuse_last and not self._eval:
                     # last layer of a 1- / 3-channel stack: the tap gather, sigmoid and loss run as ONE kernel in losses_fwd
                     rec_fused = (colD, colS, Hi, P[cn + ".bias"])
                 else:
@@ -863,7 +1004,7 @@ class TrainEngine:
             self.dec.append(rec)
             Hi *= 2
         Bf = self.buffers["decoder"]
-        for k in range(-1, n - 1):
+        for k in range(-1, -1 if self._eval else n - 1):
             st = self.dec_first["st"] if k < 0 else self.dec[k]["st"]
             bn = self.dec_names(k)[1]
             K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], st["mean"], st["varu"], self.ix["dec_order"], G, st["C"], BN_MOMENTUM)

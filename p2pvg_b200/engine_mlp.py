@@ -135,7 +135,7 @@ class TrainEngineMLP(TrainEngine):
         self.d2 = ResidualLinear(self, "decoder", "fc2", "d2")
         self.d3 = Linear(self, "decoder", "fc3")
 
-    def pack_weights(self, which=("encoder", "decoder")):
+    def pack_weights(self, which=("encoder", "decoder"), backward=True):
         pass  # fp32 master weights are used directly
 
     # -- Phase E ----------------------------------------------------------------------------
@@ -173,6 +173,9 @@ class TrainEngineMLP(TrainEngine):
         d2 = self.d2.fwd(segs2, N)
         self.pred = self.fbuf("pred", N * 51)
         self.d3.fwd([(d2, h, h), (sk0, h, ld)], self.pred, N)
+
+    def decoded(self):
+        return self.pred, False   # fc3 output: the pose itself (no output nonlinearity)
 
     def losses_fwd(self, plan):
         K, B, S = self.K, self.B, self.S

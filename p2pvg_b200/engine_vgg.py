@@ -63,12 +63,13 @@ class TrainEngineVGG(TrainEngine):
             pack_conv3_t(K, w, wt, c0, cin)
             self._packed[key + ".wt"] = wt
 
-    def pack_weights(self, which=("encoder", "decoder")):
+    def pack_weights(self, which=("encoder", "decoder"), backward=True):
+        """backward=False: without the transposed copies (pack_conv3_t) that only the data gradients read."""
         K = self.K
         if "encoder" in which:
             P = self.arena["encoder"].p
             for i, j, cin, cout, pre in self.enc_layers():
-                self._pack_conv3(f"enc.{i}.{j}", P[pre + ".0.weight"], 0, cin, want_t=not (i == 0 and j == 0))
+                self._pack_conv3(f"enc.{i}.{j}", P[pre + ".0.weight"], 0, cin, want_t=backward and not (i == 0 and j == 0))
             w = P[self.top + ".0.weight"]
             wp = self.buf("wp_enc_c5", self.g * 16 * 512)
             pack_conv4(K, w, wp)
@@ -86,10 +87,10 @@ class TrainEngineVGG(TrainEngine):
                 w = P[pre + ".0.weight"]
                 if j == 0:
                     C = cin // 2
-                    self._pack_conv3(f"dec.{k}.{j}.D", w, 0, C)
-                    self._pack_conv3(f"dec.{k}.{j}.S", w, C, C)
+                    self._pack_conv3(f"dec.{k}.{j}.D", w, 0, C, want_t=backward)
+                    self._pack_conv3(f"dec.{k}.{j}.S", w, C, C, want_t=backward)
                 else:
-                    self._pack_conv3(f"dec.{k}.{j}", w, 0, cin)
+                    self._pack_conv3(f"dec.{k}.{j}", w, 0, cin, want_t=backward)
             # ConvTranspose2d(64, nc, 3, 1, 1): Wl[64, (kh,kw,co)] with the row pitch padded to ldl
             wl = self.buf("wp_dec_last", 64 * self.ldl)
             pack_conv3(K, P[self.last + ".1.weight"], wl, scratch=self.buf("wp_dec_last27", 64 * 9 * self.nc + 8))
@@ -167,7 +168,7 @@ class TrainEngineVGG(TrainEngine):
         ncalls = len(plan.enc_order)
         Bf = self.buffers["encoder"]
         bns = [(rec["pre"] + ".1", rec["st"]) for recs in self.venc for rec in recs] + [(self.top + ".1", st)]
-        for bn, s in bns:
+        for bn, s in ([] if self._eval else bns):   # running statistics: training mode only
             K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], s["mean"], s["varu"], self.ix["enc_order"], ncalls, s["C"], BN_MOMENTUM)
             Bf[bn + ".num_batches_tracked"] += ncalls
 
@@ -227,7 +228,7 @@ class TrainEngineVGG(TrainEngine):
         self.dec = [dict(raw=raw_out)]
         Bf = self.buffers["decoder"]
         bns = [("upc1.1", st)] + [(rec["pre"] + ".1", rec["st"]) for recs in self.vdec for rec in recs]
-        for bn, s in bns:
+        for bn, s in ([] if self._eval else bns):
             K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], s["mean"], s["varu"], self.ix["dec_order"], G, s["C"], BN_MOMENTUM)
             Bf[bn + ".num_batches_tracked"] += G
 

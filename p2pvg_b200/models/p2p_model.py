@@ -185,6 +185,42 @@ class P2PModel(nn.Module):
         host = eng.read_losses(out)
         return host[0], host[1], host[2], host[3]
 
+    def p2p_losses(self, x):
+        """The training objective on a held-out batch, without an update (an addition to the reference API): the four values
+        forward(x) returns with every module in eval mode -- BatchNorm normalising with its running statistics -- computed
+        before any update, with the same NumPy skip draw and the same torch.randn eps draw as forward, and nothing changed:
+        parameters, .grad, Adam moments and steps and BatchNorm buffers stay bit-identical, and captured training graphs stay
+        valid whatever the held-out batch's T, B and skip pattern (its buffers that the training step has not already
+        sized come from a pool of their own).  One CUDA-graph replay per call
+        (engine.TrainEngine.evaluate_losses, kernel p2pvg_seq_losses).
+
+        x: what forward takes.  Returns a dict: 'mse', 'kld', 'cpc', 'align' (floats, / seq_len, KL / opt.batch_size),
+        'per_sequence': per term a float64 [B] device tensor of each row's share (element means over row b for mse, cpc and
+        align, whose row mean is the scalar; row b's KL sum / opt.batch_size for kld, whose row sum is the scalar), and
+        'steps': the executed timesteps i of the skip schedule.  ValueError before any draw or launch for a model with a
+        module in training mode, a model or x not on a CUDA device, or fewer than 2 frames."""
+        for m in MODULES:
+            if any(mod.training for mod in getattr(self, m).modules()):
+                raise ValueError(f"p2p_losses needs every module in eval mode ({m} is in training mode); call model.eval() first")
+        if isinstance(x, tuple):  # h36m: (pose_2d, pose_3d, camera_view) -> pose_3d, as forward
+            x = x[1]
+        if not torch.is_tensor(x):
+            x = torch.stack(list(x))
+        if x.dim() < 3 or int(x.shape[0]) < 2:
+            raise ValueError(f"p2p_losses needs a [T, B, ...] batch with T >= 2 frames (got shape {tuple(x.shape)})")
+        dev = next(self.parameters()).device
+        if dev.type != "cuda" or not x.is_cuda:
+            raise ValueError(f"p2p_losses runs on a CUDA device: the model is on {dev} and x on {x.device}; move both with .cuda()")
+        eng = self.engine(int(x.shape[-1]))
+        eng.opt = self._opt_dict()
+        plan, per, out = eng.evaluate_losses(x.float(), use_graph=self.use_graph)
+        host = out.cpu().numpy()
+        names = ("mse", "kld", "cpc", "align")
+        res = {k: float(host[j]) for j, k in enumerate(names)}
+        res["per_sequence"] = {k: per[j] for j, k in enumerate(names)}
+        res["steps"] = list(plan.tgt_frame)
+        return res
+
     def p2p_generate(self, x, len_output, eval_cp_ix, start_ix=0, cp_ix=-1, model_mode='full', skip_frame=False,
                      init_hidden=True):
         from ..infer import p2p_generate
