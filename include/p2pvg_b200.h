@@ -480,6 +480,31 @@ int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs
  * P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, J < 1, n_pairs < 0. */
 int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream);
 
+/* One batch's scores folded into split-level totals (p2pvg_b200.evaluate.evaluate_split), in one launch.
+ *   scores     [n_pairs][n_metrics] fp64: what p2pvg_frame_metrics / p2pvg_pose_metrics wrote for the pairs of the segments
+ *   higher_mask bit m set: a higher value of metric m is better (psnr, ssim); clear: lower is better (mse, mpjpe)
+ *   segs       [n_seg][3] int32, device: per segment (one output length of the batch) its first pair off, its first column c0
+ *              and its scored frame count F; pair (frame j, row b, sample s) of the segment is off + (j * B + b) * nsample + s
+ *              and frame j is column c0 + j
+ *   col_bin    [n_cols] int32, device: the bin of every column; a bin is one (output length, scored frame) of the split
+ *   part_v     [n_cols][B][n_metrics][2] fp64 and part_c [n_cols][B][n_metrics][2] int32: workspace
+ *   counter    one uint32, zero before the first launch and left zero by every launch
+ *   sums       [n_bins][n_metrics][3] fp64, += per bin: the sum over rows of the best sample's finite value, the sum of its
+ *              squares, and the sum over rows and samples of the finite values
+ *   counts     [n_bins][n_metrics][4] uint64, += per bin: the best sample's +-inf values, its NaN values, and the +-inf and
+ *              NaN values over all samples (none of them is in sums)
+ *   rows       [n_bins] uint64, += the rows folded into each bin
+ * Best sample, per segment, row and metric: the best mean over the segment's F frames (frames summed in order, then / F),
+ * the first sample on ties, and the first NaN mean if there is one (torch's argmax / argmin).  Every sum is fp64 in a fixed
+ * order (columns of a bin in column order, rows in row order) with no float atomics, so the totals are bit-identical from
+ * run to run and do not depend on which other bins share the launch.
+ * Preconditions (not checked on the device): segs name pairs below n_pairs and columns below n_cols; a bin outside
+ * [0, n_bins) is skipped.  P2PVG_ERR_BAD_ARG: NULL or misaligned pointers, n_metrics outside 1..8, B, nsample, n_seg or
+ * n_bins < 1, n_cols < n_seg.  P2PVG_ERR_UNSUPPORTED: n_cols * B * n_metrics >= 2^31. */
+int p2pvg_metrics_fold(const double* scores, int n_metrics, int higher_mask, int B, int nsample, const int32_t* segs, int n_seg,
+                       const int32_t* col_bin, int n_cols, int n_bins, double* part_v, int32_t* part_c, uint32_t* counter,
+                       double* sums, uint64_t* counts, uint64_t* rows, void* stream);
+
 /* The pictures of the reference's misc/visualize.py vis_seq (:176-261) from generated frames, in one launch.
  *   store0 [n0][C][H][H], store1 [n1][C][H][H] fp32 frame stores (a generation graph's input and output buffers, or any
  *              stacked store); C = 1 (replicated to 3 channels) or 3; square frames, 1 <= H <= 128

@@ -503,6 +503,20 @@ class CudaKernels:
         """p2pvg_pose_metrics: out fp64 [n_pairs, 2] = mse, mpjpe of pred[pairs[p, 0]] against gt[pairs[p, 1]] ([.., J, 3])."""
         self._ck(self.lib.p2pvg_pose_metrics(_p(pred), _p(gt), _p(pairs), _i(n_pairs), _i(J), _p(out), self._stream()))
 
+    def metrics_fold(self, scores, higher_mask, B, nsample, segs, col_bin, part_v, part_c, counter, sums, counts, rows):
+        """p2pvg_metrics_fold: scores fp64 [n_pairs, n_metrics] folded into the bins sums fp64 [n_bins, n_metrics, 3], counts
+        int64 [n_bins, n_metrics, 4] and rows int64 [n_bins]; segs int32 [n_seg, 3] and col_bin int32 [n_cols] device tables
+        (checked by p2pvg_b200.evaluate); part_v fp64 / part_c int32 [n_cols * B * n_metrics * 2] and counter int32 [1]
+        (zero before the first launch, left zero) are its workspace."""
+        nm = scores.shape[1]
+        assert scores.dtype == sums.dtype == part_v.dtype == torch.float64 and counts.dtype == rows.dtype == torch.int64
+        assert segs.dtype == col_bin.dtype == part_c.dtype == counter.dtype == torch.int32
+        assert part_v.numel() >= col_bin.numel() * B * nm * 2 and part_c.numel() >= col_bin.numel() * B * nm * 2
+        assert tuple(sums.shape[1:]) == (nm, 3) and tuple(counts.shape) == (sums.shape[0], nm, 4) and rows.numel() == sums.shape[0]
+        self._ck(self.lib.p2pvg_metrics_fold(_p(scores), _i(nm), _i(higher_mask), _i(B), _i(nsample), _p(segs), _i(segs.shape[0]),
+                                             _p(col_bin), _i(col_bin.numel()), _i(sums.shape[0]), _p(part_v), _p(part_c),
+                                             _p(counter), _p(sums), _p(counts), _p(rows), self._stream()))
+
     # -- qualitative pictures ----------------------------------------------------------------
     def vis_canvas(self, store0, n0, store1, n1, C, H, tiles_host, tiles_dev, r_len, n_block, canvas, video, gif):
         """p2pvg_vis_canvas: the PNG canvas, video tensor and GIF frames of misc/visualize.py vis_seq from fp32 frame stores

@@ -118,6 +118,8 @@ int p2pvg_pose_windows_impl(const float*, const float*, int, const int64_t*, con
                             int, int, int, float*, float*, cudaStream_t);
 int p2pvg_frame_metrics_impl(const float*, const float*, const int32_t*, int, int, int, int, float, double*, cudaStream_t);
 int p2pvg_pose_metrics_impl(const float*, const float*, const int32_t*, int, int, double*, cudaStream_t);
+int p2pvg_metrics_fold_impl(const double*, int, int, int, int, const int32_t*, int, const int32_t*, int, int, double*, int32_t*,
+                            unsigned int*, double*, unsigned long long*, unsigned long long*, cudaStream_t);
 int p2pvg_vis_canvas_impl(const float*, int, const float*, int, int, int, const int32_t*, int32_t*, int, int, float*, float*, uint8_t*,
                           cudaStream_t);
 int p2pvg_vis_tiles_impl(const float*, int, const float*, int, int, int, const int32_t*, int, const int64_t*, int, void*, float*,
@@ -400,6 +402,12 @@ int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs
 }
 int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream) {
   return p2pvg_pose_metrics_impl(pred, gt, pairs, n_pairs, J, out, ST);
+}
+int p2pvg_metrics_fold(const double* scores, int n_metrics, int higher_mask, int B, int nsample, const int32_t* segs, int n_seg,
+                       const int32_t* col_bin, int n_cols, int n_bins, double* part_v, int32_t* part_c, uint32_t* counter,
+                       double* sums, uint64_t* counts, uint64_t* rows, void* stream) {
+  return p2pvg_metrics_fold_impl(scores, n_metrics, higher_mask, B, nsample, segs, n_seg, col_bin, n_cols, n_bins, part_v, part_c,
+                                 counter, sums, (unsigned long long*)counts, (unsigned long long*)rows, ST);
 }
 int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
                      int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream) {

@@ -45,7 +45,8 @@ truth h source is kept once per distinct active row count; every other buffer is
 
 ``evaluate`` (P2PModel.p2p_evaluate) runs the replay of a generate call (or chain) and, instead of assembling the output list,
 scores the decoded frames in the graph's output buffer against the ground truth in its input buffer with one metrics launch
-(metrics.plan_pairs / plan_pairs_multi_cp name the rows).
+(metrics.plan_pairs / plan_pairs_multi_cp name the rows).  ``evaluate_lengths`` (P2PModel.p2p_evaluate_lengths) does the
+same for every length of one generate_lengths replay: one metrics launch over all row groups (metrics.plan_pairs_lengths).
 
 Memory: every cached signature (at most MAX_GRAPHS, least recently used evicted) owns its buffers; the ground-truth encode
 covers all len(x) frames of the call.  ``GenerateEngine.memory_bytes()`` reports the total, ``clear()`` frees it.
@@ -211,6 +212,7 @@ class _Graph:
         self.bufs = {}
         self.graph = None
         self.ws_gen = None
+        self.eval_lengths = {}   # evaluate_lengths' pair plans, per len_outputs in caller order
 
 
 class GenerateEngine:
@@ -301,6 +303,50 @@ class GenerateEngine:
         res = res.view(len(frames), B, nsample, len(names)).permute(3, 2, 0, 1)   # [metric][sample][frame][b]
         scores = {k: res[i].contiguous() for i, k in enumerate(names)}
         return dict(frames=list(frames), **scores, best=metrics.best_of(scores, names))
+
+    @torch.no_grad()
+    def evaluate_lengths(self, x, len_outputs, nsample=1, model_mode="full", data_range=1.0):
+        """evaluate(x, nsample, L, model_mode, data_range) for every L in len_outputs, in order, from ONE generate_lengths
+        replay and ONE metrics launch (score_lengths): see P2PModel.p2p_evaluate_lengths."""
+        from . import metrics
+        (frames, offsets, B), res, names = self.score_lengths(x, len_outputs, nsample, model_mode, data_range)
+        out = []
+        for fk, o in zip(frames, offsets):
+            r = res[o:o + len(fk) * B * nsample].view(len(fk), B, nsample, len(names)).permute(3, 2, 0, 1)
+            scores = {k: r[i].contiguous() for i, k in enumerate(names)}
+            out.append(dict(frames=list(fk), **scores, best=metrics.best_of(scores, names)))
+        return out
+
+    @torch.no_grad()
+    def score_lengths(self, x, len_outputs, nsample=1, model_mode="full", data_range=1.0):
+        """The replay of generate_lengths(x, len_outputs, model_mode, nsample), then ONE metrics launch that scores every
+        length's row group in the graph's own output and input buffers (metrics.plan_pairs_lengths, planned once per graph
+        signature and len_outputs).  ValueError before any draw or launch for what check_lengths rejects, a length <= n_past
+        or a data_range that is not positive.  Returns ((frames, offsets, B), scores, names): per length its scored frames and
+        first pair and the batch size, the fp64 [n_pairs, len(names)] scores on the device, and the metric names."""
+        from . import metrics
+        if isinstance(x, tuple):
+            x = x[1]
+        self._check_model()
+        T, n_past = len(x), int(self.model.opt.n_past)
+        lens = check_lengths(len_outputs, T, n_past)
+        for L in lens:
+            if L <= n_past:
+                raise ValueError(f"p2p_evaluate_lengths: nothing is generated to score (len_output = {L} <= n_past = {n_past})")
+        metrics._check_range(data_range)
+        G, _, _, _ = self._replay_lengths(x, lens, model_mode, nsample)
+        c = G.cfg
+        plan = G.eval_lengths.get(tuple(lens))
+        if plan is None:   # the plan depends on nothing but the graph's signature and the caller's order of the lengths
+            frames, pairs, offsets = metrics.plan_pairs_lengths(lens, T, n_past, nsample, c["B"])
+            plan = G.eval_lengths[tuple(lens)] = (frames, pairs.to(c["dev"]), offsets)
+        frames, pairs, offsets = plan
+        out, xb = G.bufs["out"], G.bufs["x"]
+        if self.model.is_pose:
+            res, names = metrics.launch_pose_metrics(out, xb, pairs, c["fshape"][0]), metrics.POSE_METRICS
+        else:
+            res, names = metrics.launch_frame_metrics(out, xb, pairs, c["fshape"], data_range), metrics.FRAME_METRICS
+        return (frames, offsets, c["B"]), res, names
 
     @torch.no_grad()
     def vis_canvas(self, x, len_output, model_mode, nsample, plan):

@@ -9,7 +9,8 @@ mse over the J * 3 values and mpjpe, the mean over joints of the Euclidean joint
 ``frame_metrics`` / ``pose_metrics`` score any set of (pred index, gt index) pairs of two stores in one launch, so the
 generated frames of several samples can be scored against one copy of the ground truth.  ``plan_pairs`` (one call) and
 ``plan_pairs_multi_cp`` (a chain through control points) are the pair lists ``P2PModel.p2p_evaluate`` scores inside the
-generation engine's buffers.
+generation engine's buffers; ``plan_pairs_lengths`` is the list ``P2PModel.p2p_evaluate_lengths`` scores (every output length
+of one generate_lengths replay).
 """
 from __future__ import annotations
 
@@ -55,6 +56,31 @@ def plan_pairs_multi_cp(cp_ixs, n_past, nsample, B):
         dec += [len(dec) + j for j in range(b - a + 1 - n_past)]
         frames += [a + i for i in range(n_past, b - a + 1)]
     return frames, _pairs(dec, frames, nsample, B)
+
+
+def plan_pairs_lengths(lens, len_x, n_past, nsample, B):
+    """plan_pairs of every output length of ONE generate_lengths replay (P2PModel.p2p_evaluate_lengths).  The lengths
+    engine gives length lens[k] the row group g = gen_engine.lengths_order(lens).index(k) of nsample * B rows, and decodes
+    its frame i (n_past <= i < lens[k]) of sample s, batch row b into row (i - n_past) * rows + g * nsample * B + s * B + b of
+    its output store (rows = len(lens) * nsample * B).  Each length's frames and gt rows are plan_pairs'.
+
+    Returns (frames, pairs, offsets): per length its scored frame indices; int32 [n, 2] pairs, the lengths in caller order,
+    each length's pairs ordered (frame, b, sample) as plan_pairs orders them; per length the index of its first pair."""
+    from .gen_engine import lengths_order
+    order = lengths_order(lens)
+    grows = nsample * B
+    rows = len(lens) * grows
+    frames, parts, offsets, n = [], [], [], 0
+    for k, L in enumerate(lens):
+        fk, pk = plan_pairs(L, len_x, n_past, nsample, B)
+        pred = pk[:, 0].to(torch.int64)
+        # plan_pairs' row f * grows + r of a one-length store is row f * rows + g * grows + r here
+        pk = torch.stack([(pred // grows) * rows + order.index(k) * grows + pred % grows, pk[:, 1].to(torch.int64)], 1)
+        frames.append(fk)
+        parts.append(pk.to(torch.int32))
+        offsets.append(n)
+        n += len(pk)
+    return frames, torch.cat(parts), offsets
 
 
 def _pairs(dec, gts, nsample, B):

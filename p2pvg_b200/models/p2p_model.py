@@ -289,6 +289,19 @@ class P2PModel(nn.Module):
         return self._graphed_engine().evaluate(x, nsample=nsample, len_output=len_output, model_mode=model_mode,
                                                data_range=data_range, cp_ixs=cp_ixs)
 
+    def p2p_evaluate_lengths(self, x, len_outputs, nsample=1, model_mode='full', data_range=1.0):
+        """Generate at several output lengths and score them in one call (an addition to the reference API): ONE
+        p2p_generate_lengths replay (the same draws, row groups and .hidden afterwards) and ONE metrics launch over every
+        length's rows.  Returns one dict per entry of len_outputs, in order, each what the looped call
+
+            p2p_evaluate(x, nsample, len_output=L, model_mode=model_mode, data_range=data_range)
+
+        returns: L == len(x) scores every generated frame, any other L only the control point.  The same models as
+        p2p_generate_graphed.  ValueError before any draw or launch for what p2p_generate_lengths rejects, a length <= n_past
+        or a data_range that is not positive."""
+        return self._graphed_engine().evaluate_lengths(x, len_outputs, nsample=nsample, model_mode=model_mode,
+                                                       data_range=data_range)
+
     def _graphed_engine(self):
         from ..gen_engine import GenerateEngine, PoseGenerateEngine
         from ..gen_engine_vgg import VggGenerateEngine
