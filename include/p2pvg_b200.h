@@ -565,6 +565,36 @@ size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_ed
 int p2pvg_histograms(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* workspace, size_t ws_bytes,
                      int64_t* counts, double* stats, void* stream);
 
+/* PNG files (8-bit RGB, colour type 2) of n images in one call, every stage on the device: quantisation, per-row filter
+ * choice, deflate in segments of P2PVG_PNG_SEGMENT filtered bytes (one IDAT chunk each), zlib framing, chunk CRCs and the
+ * packing of every file into one buffer.
+ *   images     [n][5] int64, HOST memory: per image the device address of a contiguous [C][H][W] array, its dtype
+ *              (P2PVG_F32, 4-byte aligned, or P2PVG_PNG_U8), C (1: the channel is replicated to RGB, or 3), H and W
+ *              (1 .. 2^24 - 1 each)
+ *   rule       P2PVG_PNG_SAVE_IMAGE: u8 = trunc(clamp((x * 255) + 0.5, 0, 255)), each operation one fp32 rounding
+ *              (torchvision.utils.save_image); P2PVG_PNG_TENSORBOARD: u8 = trunc(clamp(x * 255, 0, 255))
+ *              (torch.utils.tensorboard.summary.image for float input).  uint8 images are taken as they are.  NaN is
+ *              outside the contract.
+ *   workspace  p2pvg_png_workspace_bytes(images, n) bytes, 256-byte aligned (tables, filtered streams, LZ77 scratch)
+ *   out        at least p2pvg_png_out_bytes(images, n) bytes: the files, back to back in image order
+ *   files      [n][2] int64 (8-byte aligned): offset in out and size of each file
+ * Each segment is deflated by one CTA (matches reach up to 32 KB back, into earlier segments of the same image but never
+ * before its first byte); every segment but an image's last ends with an empty stored block.  The Adler-32 of an image's
+ * stream is combined from its segments' (sum of bytes, sum of (bytes to the segment's end) * byte) parts:
+ * a = 1 + sum S_k, b = N + sum (W_k + (bytes after segment k) * S_k), mod 65521.  The bytes of a file depend on its image
+ * and the rule alone, not on the other images of the call.
+ * n == 0 returns P2PVG_OK without a launch.  P2PVG_ERR_BAD_ARG: a malformed table row, rule or pointer;
+ * P2PVG_ERR_UNSUPPORTED: an image of 2^24 rows or columns or more; P2PVG_ERR_WORKSPACE: workspace or out too small.
+ * The size queries return 0 for a table the encoder rejects. */
+#define P2PVG_PNG_U8 3
+#define P2PVG_PNG_SAVE_IMAGE 0
+#define P2PVG_PNG_TENSORBOARD 1
+#define P2PVG_PNG_SEGMENT 65536
+size_t p2pvg_png_workspace_bytes(const int64_t* images, int n);
+size_t p2pvg_png_out_bytes(const int64_t* images, int n);
+int p2pvg_png_encode(const int64_t* images, int n, int rule, void* workspace, size_t ws_bytes, uint8_t* out, size_t out_bytes,
+                     int64_t* files, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,8 @@ def load_library():
         _lib.p2pvg_bn_workspace_bytes.restype = ctypes.c_size_t
         _lib.p2pvg_bn_wgrad_c1_partial_bytes.restype = ctypes.c_size_t
         _lib.p2pvg_histograms_workspace_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_png_workspace_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_png_out_bytes.restype = ctypes.c_size_t
     return _lib
 
 
@@ -546,3 +548,16 @@ class CudaKernels:
         self._ck(self.lib.p2pvg_histograms(_vp(segs_host.ctypes.data), _i(len(segs_host)), _vp(edges_host.ctypes.data),
                                            _i(len(edges_host)), _p(workspace), _sz(workspace.numel() * workspace.element_size()),
                                            _p(counts), _p(stats), self._stream()))
+
+    # -- PNG files -----------------------------------------------------------------------------
+    def png_bytes(self, images_host):
+        """(workspace bytes, output bytes) p2pvg_png_encode needs for the int64 host image table images_host [n, 5]
+        (address, dtype, C, H, W); (0, 0) for a table it rejects."""
+        ptr, n = _vp(images_host.ctypes.data), _i(len(images_host))
+        return int(self.lib.p2pvg_png_workspace_bytes(ptr, n)), int(self.lib.p2pvg_png_out_bytes(ptr, n))
+
+    def png_encode(self, images_host, rule, workspace, out, files):
+        """p2pvg_png_encode: the PNG files of the images of images_host (checked by the library before any launch) packed into
+        the uint8 device buffer out, with their (offset, size) in the int64 device tensor files [n, 2]."""
+        self._ck(self.lib.p2pvg_png_encode(_vp(images_host.ctypes.data), _i(len(images_host)), _i(rule), _p(workspace),
+                                           _sz(workspace.numel()), _p(out), _sz(out.numel()), _p(files), self._stream()))

@@ -126,6 +126,9 @@ int p2pvg_vis_tiles_impl(const float*, int, const float*, int, int, int, const i
                          long long, uint8_t*, long long, cudaStream_t);
 size_t p2pvg_histograms_workspace_bytes_impl(const int64_t*, int, int);
 int p2pvg_histograms_impl(const int64_t*, int, const double*, int, void*, size_t, int64_t*, double*, cudaStream_t);
+size_t p2pvg_png_workspace_bytes_impl(const int64_t*, int);
+size_t p2pvg_png_out_bytes_impl(const int64_t*, int);
+int p2pvg_png_encode_impl(const int64_t*, int, int, void*, size_t, uint8_t*, size_t, int64_t*, cudaStream_t);
 
 static int g_gemm_impl = 0;  // 0 auto, 1 simt, 2 wgmma
 int p2pvg_gemm_impl_forced() { return g_gemm_impl; }
@@ -425,6 +428,12 @@ size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_ed
 int p2pvg_histograms(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* workspace, size_t ws_bytes,
                      int64_t* counts, double* stats, void* stream) {
   return p2pvg_histograms_impl(segs, n_seg, edges, n_edges, workspace, ws_bytes, counts, stats, ST);
+}
+size_t p2pvg_png_workspace_bytes(const int64_t* images, int n) { return p2pvg_png_workspace_bytes_impl(images, n); }
+size_t p2pvg_png_out_bytes(const int64_t* images, int n) { return p2pvg_png_out_bytes_impl(images, n); }
+int p2pvg_png_encode(const int64_t* images, int n, int rule, void* workspace, size_t ws_bytes, uint8_t* out, size_t out_bytes,
+                     int64_t* files, void* stream) {
+  return p2pvg_png_encode_impl(images, n, rule, workspace, ws_bytes, out, out_bytes, files, ST);
 }
 
 }  // extern "C"

@@ -12,6 +12,8 @@ event records.
 - ``add_param_histograms(writer, model, step)``: ``train.py``'s logging block in one launch.
 - ``HistogramWriterMixin``: a writer whose ``add_histogram`` takes the GPU path for fp32 / fp64 values and TensorBoard's
   default (or an explicit) edge table; ``dropin/tensorboardX`` puts it under ``train.py``'s ``SummaryWriter``.
+- ``add_image_gpu(writer, ...)``: ``add_image`` of a 3-channel float32 / uint8 image with the PNG encoded on the GPU
+  (``p2pvg_b200.png``); ``dropin/tensorboardX``'s ``SummaryWriter.add_image`` takes it first.
 
 The one visible difference from the host computation: sum and sum_squares are fp64 sums in another order (fixed-size
 chunks of each tensor), so they agree with ``values.sum()`` / ``values.dot(values)`` to rounding, not bit for bit.
@@ -208,3 +210,56 @@ class HistogramWriterMixin:
         (counts, stats), = histograms([t.view(-1)], edges)
         self.add_histogram_raw(tag, **histogram_fields(counts, stats, edges, max_bins), global_step=global_step,
                                walltime=walltime)
+
+
+def _gpu_image(img, dataformats):
+    """img as a contiguous CUDA [3, H, W] float32 / uint8 tensor when the GPU image path takes it, else None."""
+    if dataformats not in ("CHW", "HWC") or not torch.cuda.is_available():
+        return None
+    if isinstance(img, np.ndarray):
+        if img.dtype not in (np.float32, np.uint8):
+            return None
+        t = torch.from_numpy(np.ascontiguousarray(img))
+    elif torch.is_tensor(img):
+        t = img.detach()
+    else:
+        return None
+    if t.dtype not in (torch.float32, torch.uint8) or t.dim() != 3 or t.shape[dataformats.index("C")] != 3 or t.numel() == 0:
+        return None
+    if t.device.type != "cuda":
+        if t.device.type != "cpu":
+            return None
+        t = t.to("cuda")
+    if dataformats == "HWC":
+        t = t.permute(2, 0, 1)
+    t = t.contiguous()
+    if t.dtype == torch.float32 and bool(torch.isnan(t).any()):
+        return None
+    return t
+
+
+def add_image_gpu(writer, tag, img_tensor, global_step=None, walltime=None, dataformats='CHW'):
+    """``writer.add_image`` of a 3-channel float32 or uint8 image (CHW or HWC, a NumPy array or a tensor) with the PNG
+    encoded on the GPU, when a CUDA device exists: the base writer's quantisation (float32: x * 255 clipped to [0, 255]
+    and truncated; uint8 as it is) and the same ``Summary.Image`` record (tag, step, height, width, colorspace), written
+    through ``writer._get_file_writer()``.  The pixels equal the base writer's; the compressed bytes differ.  Returns
+    False, having written nothing, for any other call and for float input with NaN."""
+    t = _gpu_image(img_tensor, dataformats)
+    if t is None:
+        return False
+    from . import png
+    data, = png.encode_png([t], "tensorboard")
+    Summary = _summary_class(writer)
+    image = Summary.Image(height=int(t.shape[1]), width=int(t.shape[2]), colorspace=3, encoded_image_string=data)
+    writer._get_file_writer().add_summary(Summary(value=[Summary.Value(tag=tag, image=image)]), global_step, walltime)
+    return True
+
+
+def _summary_class(writer):
+    """The Summary protobuf class of the writer's base package (the ``summary`` module beside the module of the first base
+    class that defines add_image: torch.utils.tensorboard or tensorboardX)."""
+    import importlib
+    for cls in type(writer).__mro__[1:]:
+        if "add_image" in vars(cls):
+            return importlib.import_module(cls.__module__.rsplit(".", 1)[0] + ".summary").Summary
+    raise TypeError("add_image_gpu needs a SummaryWriter")

@@ -201,10 +201,11 @@ def _render(vis, poses, camera_view, nb):
 
 
 def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, skip_frame=True, h36m_visualizer=None, writer=None,
-            opt=None):
+            opt=None, save_png=None):
     """misc/visualize.py vis_seq (same arguments, files and TensorBoard entries) on the graphed generator and one
-    p2pvg_vis_canvas launch; see the module docstring.  ValueError before any draw or launch when check_vis_seq rejects the
-    arguments.  Returns (canvas, video, gif) on the device."""
+    p2pvg_vis_canvas launch; see the module docstring.  ``save_png(canvas, file_name)`` writes the PNG file
+    (torchvision.utils.save_image when None; p2pvg_b200.png.save_image encodes it on the GPU).  ValueError before any draw
+    or launch when check_vis_seq rejects the arguments.  Returns (canvas, video, gif) on the device."""
     opt = model.opt if opt is None else opt
     check_vis_seq(model, x, output_len, model_mode, skip_frame, opt)
     import imageio
@@ -255,7 +256,7 @@ def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, ski
             tiles = plan_tiles(seq_len, L, nb, nsample, lambda t: (0, t * nb), sample_ref)
             canvas, video, gif = compose(store0, samples, tiles, int(frames.shape[2]), int(frames.shape[3]))
     png_name, gif_name = file_names(opt, epoch, output_len, model_mode, recon_mode)
-    vutils.save_image(canvas, png_name)
+    (vutils.save_image if save_png is None else save_png)(canvas, png_name)
     imageio.mimsave(gif_name, list(gif.cpu().numpy()))
     img_tag, vid_tag = tags(output_len, model_mode, recon_mode)
     writer.add_image(img_tag, canvas.cpu().numpy(), epoch)
