@@ -180,13 +180,13 @@ def conv_locate(kind, H, s):
             row, ph = (n * H + y // 2) * H + x // 2, (y & 1) * 2 + (x & 1)
         else:
             row, ph = (n * H + y) * H + x, 0
-        return s.where(0, row // 128, c // s.BN, ph)
+        return s.where(0, row // s.BM, c // s.BN, ph)
     return loc
 
 
 def image_slices(N, HW, unit, s, sms):
     """Three tile-aligned image ranges (first, middle, last round) whose launch has at most `sms` tiles."""
-    tiles_per_img = lambda n: cdiv(n * HW, 128) * s.tiles_n * s.phases
+    tiles_per_img = lambda n: cdiv(n * HW, s.BM) * s.tiles_n * s.phases
     ni = unit
     while ni + unit <= N and tiles_per_img(ni + unit) <= sms:
         ni += unit
@@ -209,11 +209,11 @@ CONV_CASES = [
 ]
 
 
-def conv_fit(kind, H, Ck, Cn_cands, N0, step, sms):
+def conv_fit(kind, H, Ck, Cn_cands, N0, step, sms, **kw):
     # Cn <= 128 is a single column tile (BN = 64 or 128), n0 = 0 on every tile: no n0 change to ask for.  Kind 2 decodes nt from
-    # t >> 2 and the phase from t & 3; on 132 SMs the phase of a CTA never changes (132 % 4 == 0).
+    # t >> 2 and the phase from t & 3; on 132 SMs the phase of a CTA never changes (132 % 4 == 0).  kw: stat / eval_epi.
     cands = ((N0 + step * j, Cn) for Cn in Cn_cands for j in range(200))
-    return fit(cands, lambda N, Cn: conv_tiles(kind, N, H, H, Ck, Cn, 0, sms), need_n_change=Cn_cands[0] > 128)
+    return fit(cands, lambda N, Cn: conv_tiles(kind, N, H, H, Ck, Cn, 0, sms, **kw), need_n_change=Cn_cands[0] > 128)
 
 
 @pytest.mark.parametrize("case", CONV_CASES, ids=[c[0] for c in CONV_CASES])
@@ -221,6 +221,7 @@ def test_conv_gemm_multi_round(K, sms, case):
     name, kind, H, Ck, Cn_cands, N0, step, B = case
     (N, Cn), s = conv_fit(kind, H, Ck, Cn_cands, N0, step, sms)
     assert s.bres == name.endswith("bres")
+    assert s.BM == (256 if kind == 2 and Cn == 64 else 128)
     torch.manual_seed(14)
     a, b = conv_operands(kind, N, H, Ck, Cn)
     bias = randn(Cn) if kind != 5 else None
@@ -236,7 +237,7 @@ def test_conv_gemm_multi_round(K, sms, case):
         combos = [(torch.float32, torch.float32), (torch.bfloat16, torch.float32), (torch.float32, torch.bfloat16),
                   (torch.bfloat16, torch.bfloat16)]
     HW = H * H
-    unit = math.lcm(step, max(1, 128 // HW))
+    unit = math.lcm(step, max(1, s.BM // HW))
     for cdt, adt in combos:
         out = torch.full(out_shape(kind, N, H, Cn), NAN, device="cuda", dtype=cdt)
         kw = dict(bias=bias)
@@ -330,7 +331,8 @@ def rows_by_tile(out, kind, N, H, Cn, tiles_m):
 @pytest.mark.parametrize("case", STAT_CASES, ids=[c[0] for c in STAT_CASES])
 def test_fused_statistics_every_row_multi_round(K, sms, case, cdt):
     name, kind, H, Ck, Cn_cands, N0, B = case
-    (N, Cn), s = conv_fit(kind, H, Ck, Cn_cands, N0, B, sms)
+    (N, Cn), s = conv_fit(kind, H, Ck, Cn_cands, N0, B, sms, stat=True)
+    assert s.BM == 128
     torch.manual_seed(16)
     a, b = conv_operands(kind, N, H, Ck, Cn)
     bias = randn(Cn)
@@ -389,7 +391,8 @@ EVAL_CASES = [
 def test_eval_epilogue_multi_round(K, sms, case, act):
     """act(scale * (conv + bias + addend) + shift) stored by the epilogue, against float64."""
     name, kind, H, Ck, Cn_cands, N0, step, B = case
-    (N, Cn), s = conv_fit(kind, H, Ck, Cn_cands, N0, step, sms)
+    (N, Cn), s = conv_fit(kind, H, Ck, Cn_cands, N0, step, sms, eval_epi=True)
+    assert s.BM == 128
     torch.manual_seed(17)
     a, b = conv_operands(kind, N, H, Ck, Cn)
     bias = randn(Cn)
