@@ -694,14 +694,15 @@ inline int check_bn_shape(int C, int vec, const char* what) {
 
 }  // namespace
 
-size_t p2pvg_bn_workspace_bytes_impl(int G, int C) { return (size_t)G * BN_MAXCHUNK * C * sizeof(double2); }
+extern "C" size_t p2pvg_bn_workspace_bytes(int G, int C) { return (size_t)G * BN_MAXCHUNK * C * sizeof(double2); }
 
-int p2pvg_bn_fwd_stats_impl(const void* x, int dtype, int G, long long R, int C, const float* gamma, const float* beta, float eps,
-                            void* ws, size_t ws_bytes, float* mean, float* invstd, float* var_unbiased, float* scale,
-                            float* shift, cudaStream_t st) {
+extern "C" int p2pvg_bn_fwd_stats(const void* x, int dtype, int G, int64_t R, int C, const float* gamma, const float* beta, float eps,
+                                  void* ws, size_t ws_bytes, float* mean, float* invstd, float* var_unbiased, float* scale, float* shift,
+                                  void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   const int vec = dtype == P2PVG_BF16 ? 8 : 4;
   if (int e = check_bn_shape(C, vec, "bn_fwd_stats")) return e;
-  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes_impl(G, C), P2PVG_ERR_WORKSPACE, "bn_fwd_stats: workspace too small");
+  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes(G, C), P2PVG_ERR_WORKSPACE, "bn_fwd_stats: workspace too small");
   if (G == 0) return P2PVG_OK;
   Chunking ch = choose_chunks(R, C, vec);
   dim3 grid(ch.nchunk, G);
@@ -712,8 +713,9 @@ int p2pvg_bn_fwd_stats_impl(const void* x, int dtype, int G, long long R, int C,
   return p2pvg_check_launch("bn_fwd_stats");
 }
 
-int p2pvg_bn_act_impl(const void* x, void* y, int dtype, const float* scale, const float* shift, int G, long long R, int C, int act,
-                      cudaStream_t st) {
+extern "C" int p2pvg_bn_act(const void* x, void* y, int dtype, const float* scale, const float* shift, int G, int64_t R, int C, int act,
+                            void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   const int vec = dtype == P2PVG_BF16 ? 8 : 4;
   if (int e = check_bn_shape(C, vec, "bn_act")) return e;
   if (G == 0 || R == 0) return P2PVG_OK;
@@ -723,14 +725,15 @@ int p2pvg_bn_act_impl(const void* x, void* y, int dtype, const float* scale, con
   return p2pvg_check_launch("bn_act");
 }
 
-int p2pvg_bn_bwd_impl(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
-                      const float* gamma, int G, long long R, int C, int act, void* ws, size_t ws_bytes, void* dx, float* sum_dz,
-                      float* sum_dzx, const float* scale, const float* shift, cudaStream_t st) {
+extern "C" int p2pvg_bn_bwd(const void* dy, const void* x, const void* y, int dtype, const float* mean, const float* invstd,
+                            const float* gamma, int G, int64_t R, int C, int act, void* ws, size_t ws_bytes, void* dx, float* sum_dz,
+                            float* sum_dzx, const float* scale, const float* shift, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(y != nullptr || (act == P2PVG_ACT_LRELU && scale && shift), P2PVG_ERR_BAD_ARG,
                 "bn_bwd: y may only be omitted for LeakyReLU with scale/shift supplied");
   const int vec = dtype == P2PVG_BF16 ? 8 : 4;
   if (int e = check_bn_shape(C, vec, "bn_bwd")) return e;
-  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes_impl(G, C), P2PVG_ERR_WORKSPACE, "bn_bwd: workspace too small");
+  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes(G, C), P2PVG_ERR_WORKSPACE, "bn_bwd: workspace too small");
   if (G == 0) return P2PVG_OK;
   Chunking ch = choose_chunks(R, C, vec);
   dim3 grid(ch.nchunk, G);
@@ -742,7 +745,7 @@ int p2pvg_bn_bwd_impl(const void* dy, const void* x, const void* y, int dtype, c
   return p2pvg_check_launch("bn_bwd");
 }
 
-size_t p2pvg_bn_wgrad_c1_partial_bytes_impl(int G) { return (size_t)G * BN_MAXCHUNK * 64 * 16 * sizeof(float); }
+extern "C" size_t p2pvg_bn_wgrad_c1_partial_bytes(int G) { return (size_t)G * BN_MAXCHUNK * 64 * 16 * sizeof(float); }
 
 // log2(Ho) for the weight-gradient passes: Ho a power of two, R a whole number of Ho x Ho maps below 2^31 rows
 static int wgrad_c1_geometry(const char* what, long long R, int Ho, int G, size_t wpart_bytes, int* lg) {
@@ -750,7 +753,7 @@ static int wgrad_c1_geometry(const char* what, long long R, int Ho, int G, size_
   while (*lg < 15 && (1 << *lg) < Ho) (*lg)++;
   P2PVG_REQUIRE(Ho >= 1 && (1 << *lg) == Ho && R % ((long long)Ho * Ho) == 0 && R < (1LL << 31), P2PVG_ERR_BAD_ARG,
                 "%s: R = %lld is not a whole number of %dx%d maps (Ho a power of two, R < 2^31)", what, R, Ho, Ho);
-  P2PVG_REQUIRE(wpart_bytes >= p2pvg_bn_wgrad_c1_partial_bytes_impl(G), P2PVG_ERR_WORKSPACE, "%s: partial buffer too small", what);
+  P2PVG_REQUIRE(wpart_bytes >= p2pvg_bn_wgrad_c1_partial_bytes(G), P2PVG_ERR_WORKSPACE, "%s: partial buffer too small", what);
   return P2PVG_OK;
 }
 
@@ -761,7 +764,7 @@ static int bn_bwd_sums_lrelu(const char* what, const void* dy, const void* x, co
                              const void* dout, int Ho, float* wpart, size_t wpart_bytes, float* dw, cudaStream_t st) {
   P2PVG_REQUIRE(dy && x && mean && invstd && sum_dz && sum_dzx && scale && shift, P2PVG_ERR_BAD_ARG, "%s: null pointer", what);
   if (int e = check_bn_shape(C, 8, what)) return e;
-  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes_impl(G, C), P2PVG_ERR_WORKSPACE, "%s: workspace too small", what);
+  P2PVG_REQUIRE(ws_bytes >= p2pvg_bn_workspace_bytes(G, C), P2PVG_ERR_WORKSPACE, "%s: workspace too small", what);
   Chunking ch = choose_chunks(R, C, 8);
   if (dout) {
     P2PVG_REQUIRE(C == 64 && wpart && dw, P2PVG_ERR_BAD_ARG, "%s: the weight-gradient reduce needs C = 64, wpart and dw", what);
@@ -778,10 +781,11 @@ static int bn_bwd_sums_lrelu(const char* what, const void* dy, const void* x, co
   return P2PVG_OK;
 }
 
-int p2pvg_bn_bwd_group_sum_impl(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G, long long R,
-                                int C, void* ws, size_t ws_bytes, void* dx, float* sum_dz, float* sum_dzx, const float* scale,
-                                const float* shift, const int* grp_src, int F, void* dx_sum, const void* dout, int Ho, float* wpart,
-                                size_t wpart_bytes, float* dw, cudaStream_t st) {
+extern "C" int p2pvg_bn_bwd_group_sum(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                                      int64_t R, int C, void* ws, size_t ws_bytes, void* dx, float* sum_dz, float* sum_dzx,
+                                      const float* scale, const float* shift, const int* grp_src, int F, void* dx_sum, const void* dout,
+                                      int Ho, float* wpart, size_t wpart_bytes, float* dw, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(gamma && dx && grp_src && dx_sum && F >= 1, P2PVG_ERR_BAD_ARG, "bn_bwd_group_sum: bad arguments");
   if (G == 0 || R == 0) return P2PVG_OK;
   if (int e = bn_bwd_sums_lrelu("bn_bwd_group_sum", dy, x, mean, invstd, G, R, C, ws, ws_bytes, sum_dz, sum_dzx, scale, shift, dout, Ho,
@@ -794,9 +798,11 @@ int p2pvg_bn_bwd_group_sum_impl(const void* dy, const void* x, const float* mean
   return p2pvg_check_launch("bn_bwd_group_sum");
 }
 
-int p2pvg_bn_bwd_wgrad_c1_impl(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G, long long R,
-                               void* ws, size_t ws_bytes, float* sum_dz, float* sum_dzx, const float* scale, const float* shift,
-                               const void* cin, int Ho, float* wpart, size_t wpart_bytes, float* dw, cudaStream_t st) {
+extern "C" int p2pvg_bn_bwd_wgrad_c1(const void* dy, const void* x, const float* mean, const float* invstd, const float* gamma, int G,
+                                     int64_t R, void* ws, size_t ws_bytes, float* sum_dz, float* sum_dzx, const float* scale,
+                                     const float* shift, const void* cin, int Ho, float* wpart, size_t wpart_bytes, float* dw,
+                                     void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   const int C = 64;
   P2PVG_REQUIRE(gamma && cin && wpart && dw, P2PVG_ERR_BAD_ARG, "bn_bwd_wgrad_c1: null pointer");
   int lg;
@@ -814,27 +820,31 @@ int p2pvg_bn_bwd_wgrad_c1_impl(const void* dy, const void* x, const float* mean,
   return p2pvg_check_launch("bn_bwd_wgrad_c1");
 }
 
-int p2pvg_bn_param_grad_impl(const float* sum_dz, const float* sum_dzx, int G, int C, float* dgamma, float* dbeta, cudaStream_t st) {
+extern "C" int p2pvg_bn_param_grad(const float* sum_dz, const float* sum_dzx, int G, int C, float* dgamma, float* dbeta, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   bn_param_grad_kernel<<<cdiv(C, 128), 128, 0, st>>>(sum_dz, sum_dzx, G, C, dgamma, dbeta);
   return p2pvg_check_launch("bn_param_grad");
 }
 
-int p2pvg_bn_ema_impl(float* rmean, float* rvar, const float* mean, const float* var_unbiased, const int* order, int ncalls, int C,
-                      float momentum, cudaStream_t st) {
+extern "C" int p2pvg_bn_ema(float* rmean, float* rvar, const float* mean, const float* var_unbiased, const int* order, int ncalls, int C,
+                            float momentum, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   bn_ema_kernel<<<cdiv(C, 128), 128, 0, st>>>(rmean, rvar, mean, var_unbiased, order, ncalls, C, momentum);
   return p2pvg_check_launch("bn_ema");
 }
 
-int p2pvg_bn_eval_coeffs_impl(const float* gamma, const float* beta, const float* rmean, const float* rvar, float eps, int C, float* scale,
-                              float* shift, cudaStream_t st) {
+extern "C" int p2pvg_bn_eval_coeffs(const float* gamma, const float* beta, const float* rmean, const float* rvar, float eps, int C,
+                                    float* scale, float* shift, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   bn_eval_coeffs_kernel<<<cdiv(C, 128), 128, 0, st>>>(gamma, beta, rmean, rvar, eps, C, scale, shift);
   return p2pvg_check_launch("bn_eval_coeffs");
 }
 
 // Forward statistics from GEMM-epilogue partials (see bn_finalize_tiles_kernel).  R = elements per (group, channel).
-int p2pvg_bn_fwd_finalize_tiles_impl(const void* partial, int parts_per_group, int ldp, int fold, int G, long long R, int C,
-                                     const float* gamma, const float* beta, float eps, float* mean, float* invstd, float* var_unbiased,
-                                     float* scale, float* shift, cudaStream_t st) {
+extern "C" int p2pvg_bn_fwd_finalize_tiles(const void* partial, int parts_per_group, int ldp, int fold, int G, int64_t R, int C,
+                                           const float* gamma, const float* beta, float eps, float* mean, float* invstd,
+                                           float* var_unbiased, float* scale, float* shift, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(partial && parts_per_group > 0 && fold > 0 && ldp >= fold * C, P2PVG_ERR_BAD_ARG, "bn_fwd_finalize_tiles: bad partial layout");
   if (G == 0) return P2PVG_OK;
   dim3 grid(cdiv(C, 32), G);

@@ -5,21 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
-#define P2PVG_OK 0
-#define P2PVG_ERR_BAD_ARG -1
-#define P2PVG_ERR_UNSUPPORTED -2
-#define P2PVG_ERR_CUDA -3
-#define P2PVG_ERR_WORKSPACE -4
-
-#define P2PVG_F32 0
-#define P2PVG_BF16 1
-#define P2PVG_F64 2   // only the histogram segments take fp64
-
-#define P2PVG_ACT_NONE 0
-#define P2PVG_ACT_LRELU 1
-#define P2PVG_ACT_TANH 2
-#define P2PVG_ACT_SIGMOID 3
-#define P2PVG_ACT_RELU 4
+// error codes, dtypes, activations and the extern "C" entry points every .cu file defines against
+#include "../../include/p2pvg_b200.h"
 
 // thread-local error string (C ABI: p2pvg_last_error)
 void p2pvg_set_error(const char* fmt, ...);
@@ -122,6 +109,34 @@ static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b)
 // c_dtype.  Deterministic: each element is summed by one thread in ascending z.
 int p2pvg_splitk_reduce(const float* partial, int splits, void* C, int c_dtype, long long ldc, int M, int N, int accumulate,
                         const float* bias, const void* addend, long long ldd, int transposed, cudaStream_t st);
+
+// The kernels behind p2pvg_gemm (api.cu).  gemm_simt.cu: CUDA cores, every dtype pair, exact fp32 accumulation.
+int p2pvg_gemm_simt(const void* A, int in_dtype, int a_mn, long long lda, const void* B, int b_mn, long long ldb, void* C,
+                    int c_dtype, long long ldc, int M, int N, int K, int accumulate, const float* bias, const void* addend,
+                    long long ldd, void* workspace, size_t ws_bytes, cudaStream_t st);
+// gemm_tc.cu: bf16 operands on wgmma; operands that are not TMA-compatible run on p2pvg_gemm_simt unless
+// p2pvg_gemm_impl_forced() == 2 (P2PVG_ERR_UNSUPPORTED then).
+int p2pvg_gemm_tc(const void* A, int a_mn, long long lda, const void* B, int b_mn, long long ldb, void* C, int c_dtype, long long ldc,
+                  int M, int N, int K, int accumulate, const float* bias, const void* addend, long long ldd, void* workspace,
+                  size_t ws_bytes, cudaStream_t st);
+// gemm_tc.cu: K-major fp32 operands on wgmma .tf32; P2PVG_ERR_UNSUPPORTED when they are not TMA-compatible.
+int p2pvg_gemm_tf32(const void* A, long long lda, const void* B, long long ldb, void* C, int c_dtype, long long ldc, int M, int N,
+                    int K, int accumulate, const float* bias, const void* addend, long long ldd, cudaStream_t st);
+int p2pvg_gemm_tc_available();
+// p2pvg_set_gemm_impl's choice: 0 auto, 1 simt, 2 wgmma
+int p2pvg_gemm_impl_forced();
+
+// The thread-block-cluster LSTM scans behind p2pvg_lstm_scan_fwd / _bwd (lstm_scan.cu): clusters of 8 CTAs for the hidden
+// sizes p2pvg_lstm_cluster_supported accepts (lstm_cluster.cu), clusters of 16 for R = 512 (lstm_cluster512.cu).
+bool p2pvg_lstm_cluster_supported(int R);
+int p2pvg_lstm_cluster_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                           int R, cudaStream_t st);
+int p2pvg_lstm_cluster_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
+                           cudaStream_t st);
+int p2pvg_lstm_cluster512_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                              cudaStream_t st);
+int p2pvg_lstm_cluster512_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B,
+                              cudaStream_t st);
 
 #define DISPATCH_DTYPE(dt, T, ...)                                   \
   do {                                                               \

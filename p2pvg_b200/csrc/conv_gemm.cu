@@ -498,11 +498,19 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, void* C, int c_dtype, l
 
 // a, b: see the kind table at the top.  H, W: SMALL-map size.  Returns P2PVG_ERR_UNSUPPORTED when the shape does not
 // fit the pixel-box tiling (the caller then uses the explicit im2col / col2im path).
-int p2pvg_conv_gemm_impl(int kind, const void* a, const void* b, long long ldb, void* c, int c_dtype, long long ldc, int N, int H, int W,
-                         int Ck, int Cn, int Cm, const float* bias, const float* addend, const int* grp_src, int imgs_per_group,
-                         int accumulate, void* ws, size_t ws_bytes, void* stat_partial_v, int addend_dtype, const float* eval_scale,
-                         const float* eval_shift, int act, cudaStream_t st) {
-  float2* stat_partial = reinterpret_cast<float2*>(stat_partial_v);
+extern "C" int p2pvg_conv_gemm(int kind, const void* a, const void* b, int64_t ldb, void* c, int c_dtype, int64_t ldc, int N, int H, int W,
+                               int Ck, int Cn, int Cm, const float* bias, const void* addend_v, const int* grp_src, int imgs_per_group,
+                               int accumulate, void* ws, size_t ws_bytes, const p2pvg_conv_fusion_t* fusion, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  P2PVG_REQUIRE(a && b && c, P2PVG_ERR_BAD_ARG, "conv_gemm: null operand");
+  float2* stat_partial = fusion ? reinterpret_cast<float2*>(fusion->fwd_stat_partial) : nullptr;
+  P2PVG_REQUIRE(!(stat_partial && accumulate), P2PVG_ERR_BAD_ARG, "conv_gemm: statistics of an accumulating GEMM are not defined");
+  const int addend_dtype = fusion ? fusion->addend_dtype : P2PVG_F32;
+  P2PVG_REQUIRE(addend_dtype == P2PVG_F32 || addend_dtype == P2PVG_BF16, P2PVG_ERR_BAD_ARG, "conv_gemm: bad addend dtype %d", addend_dtype);
+  const float* addend = reinterpret_cast<const float*>(addend_v);
+  const float* eval_scale = fusion ? fusion->eval_scale : nullptr;
+  const float* eval_shift = fusion ? fusion->eval_shift : nullptr;
+  const int act = fusion ? fusion->act : 0;
   EvalEpi ev;
   ev.scale = eval_scale; ev.shift = eval_shift; ev.act = act;
   P2PVG_REQUIRE(driver().encode != nullptr, P2PVG_ERR_UNSUPPORTED, "conv_gemm: cuTensorMapEncodeTiled unavailable");

@@ -330,7 +330,8 @@ inline int grid_for(long long total, int block) {
 
 }  // namespace
 
-int p2pvg_im2col_k4s2p1_impl(const void* x, void* col, int dtype, int N, int H, int W, int C, cudaStream_t st) {
+extern "C" int p2pvg_im2col_k4s2p1(const void* x, void* col, int dtype, int N, int H, int W, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE((H % 2 == 0) && (W % 2 == 0), P2PVG_ERR_BAD_ARG, "im2col: odd spatial size %dx%d", H, W);
   if (N == 0) return P2PVG_OK;
   const int vec = (dtype == P2PVG_BF16) ? 8 : 4;
@@ -353,8 +354,9 @@ int p2pvg_im2col_k4s2p1_impl(const void* x, void* col, int dtype, int N, int H, 
   return p2pvg_check_launch("im2col_k4s2p1");
 }
 
-int p2pvg_col2im_k4s2p1_impl(const void* col, const void* col2, const int* grp_src, int imgs_per_group, void* y, int dtype,
-                             int N, int Hi, int Wi, int C, const float* bias, int accumulate, cudaStream_t st) {
+extern "C" int p2pvg_col2im_k4s2p1(const void* col, const void* col2, const int* grp_src, int imgs_per_group, void* y, int dtype, int N,
+                                   int Hi, int Wi, int C, const float* bias, int accumulate, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return P2PVG_OK;
   P2PVG_REQUIRE(col2 == nullptr || (grp_src != nullptr && imgs_per_group > 0), P2PVG_ERR_BAD_ARG, "col2im: col2 needs grp_src");
   const int vec = (dtype == P2PVG_BF16) ? 8 : 4;
@@ -375,8 +377,9 @@ int p2pvg_col2im_k4s2p1_impl(const void* col, const void* col2, const int* grp_s
   return p2pvg_check_launch("col2im_k4s2p1");
 }
 
-int p2pvg_permute4_impl(const void* src, int src_dtype, void* dst, int dst_dtype, const int* dims, const long long* src_strides,
-                        int accumulate, cudaStream_t st) {
+extern "C" int p2pvg_permute4(const void* src, int src_dtype, void* dst, int dst_dtype, const int* dims, const int64_t* src_strides,
+                              int accumulate, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   Perm4 p;
   long long total = 1;
   for (int i = 0; i < 4; i++) {
@@ -425,7 +428,8 @@ int p2pvg_permute4_impl(const void* src, int src_dtype, void* dst, int dst_dtype
   return p2pvg_check_launch("permute4");
 }
 
-int p2pvg_nchw_to_nhwc_dual_impl(const float* src, float* dst32, void* dsta, int act_dtype, long long N, int hw, int C, cudaStream_t st) {
+extern "C" int p2pvg_nchw_to_nhwc_dual(const float* src, float* dst32, void* dsta, int act_dtype, int64_t N, int hw, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return P2PVG_OK;
   if (hw % 4 != 0 || (C != 2 && C != 3 && C != 4) || (!dst32 && !dsta)) {
     p2pvg_set_error("nchw_to_nhwc_dual: needs H*W % 4 == 0, C in {2,3,4} and at least one destination");
@@ -446,13 +450,15 @@ int p2pvg_nchw_to_nhwc_dual_impl(const float* src, float* dst32, void* dsta, int
   return p2pvg_check_launch("nchw_to_nhwc_dual");
 }
 
-int p2pvg_add_indexed_impl(void* dst, const void* src, int dtype, const int* dst_idx, int F, long long n, cudaStream_t st) {
+extern "C" int p2pvg_add_indexed(void* dst, const void* src, int dtype, const int* dst_idx, int F, int64_t n, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (F == 0 || n == 0) return P2PVG_OK;
   DISPATCH_DTYPE(dtype, T, (add_indexed_kernel<T><<<grid_for((long long)F * n, 256), 256, 0, st>>>((T*)dst, (const T*)src, dst_idx, F, n)));
   return p2pvg_check_launch("add_indexed");
 }
 
-int p2pvg_transpose_batched_impl(const void* src, int src_dtype, void* dst, int dst_dtype, int A, int P, int Q, cudaStream_t st) {
+extern "C" int p2pvg_transpose_batched(const void* src, int src_dtype, void* dst, int dst_dtype, int A, int P, int Q, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(A > 0 && P > 0 && Q > 0 && A <= 65535, P2PVG_ERR_BAD_ARG, "transpose_batched: bad shape %d x %d x %d", A, P, Q);
   dim3 grid(cdiv(Q, 32), cdiv(P, 32), A);
   if (src_dtype == P2PVG_F32 && dst_dtype == P2PVG_F32) transpose_batched_kernel<float, float><<<grid, 256, 0, st>>>((const float*)src, (float*)dst, P, Q);
@@ -465,7 +471,8 @@ int p2pvg_transpose_batched_impl(const void* src, int src_dtype, void* dst, int 
   return p2pvg_check_launch("transpose_batched");
 }
 
-int p2pvg_blockdiag_impl(const void* src, int src_dtype, void* dst, int dst_dtype, int R, int C, int g, cudaStream_t st) {
+extern "C" int p2pvg_blockdiag(const void* src, int src_dtype, void* dst, int dst_dtype, int R, int C, int g, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(R > 0 && C > 0 && g > 0, P2PVG_ERR_BAD_ARG, "blockdiag: bad shape");
   const long long total = (long long)g * R * g * C;
   const int grid = grid_for(total, 256);
@@ -479,7 +486,8 @@ int p2pvg_blockdiag_impl(const void* src, int src_dtype, void* dst, int dst_dtyp
   return p2pvg_check_launch("blockdiag");
 }
 
-int p2pvg_group_sum_impl(const void* in, void* out, int dtype, const int* grp_src, int G, int F, long long n, cudaStream_t st) {
+extern "C" int p2pvg_group_sum(const void* in, void* out, int dtype, const int* grp_src, int G, int F, int64_t n, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(n % 4 == 0, P2PVG_ERR_BAD_ARG, "group_sum: n must be a multiple of 4");
   if (F == 0 || n == 0) return P2PVG_OK;
   DISPATCH_DTYPE(dtype, T, (group_sum_kernel<T><<<grid_for((long long)F * (n / 4), 256), 256, 0, st>>>((const T*)in, (T*)out, grp_src, G, F, n / 4)));

@@ -177,9 +177,6 @@ int p2pvg_splitk_reduce(const float* partial, int splits, void* C, int c_dtype, 
   return p2pvg_check_launch("splitk_reduce");
 }
 
-int p2pvg_gemm_simt(const void*, int, int, long long, const void*, int, long long, void*, int, long long, int, int, int, int,
-                    const float*, const void*, long long, void*, size_t, cudaStream_t);
-
 static bool tc_operand_ok(const void* p, long long ld, int elem = 2) {
   return ((reinterpret_cast<uintptr_t>(p) & 15) == 0) && ((ld * elem) % 16 == 0);
 }
@@ -205,7 +202,6 @@ int p2pvg_gemm_tc(const void* A, int a_mn, long long lda, const void* B, int b_m
                   int M, int N, int K, int accumulate, const float* bias, const void* addend, long long ldd, void* workspace,
                   size_t ws_bytes, cudaStream_t st) {
   if (M <= 0 || N <= 0) return P2PVG_OK;
-  extern int p2pvg_gemm_impl_forced();
   if (!p2pvg_gemm_tc_available() || !tc_operand_ok(A, lda) || !tc_operand_ok(B, ldb) || K <= 0) {
     if (p2pvg_gemm_impl_forced() == 2) {
       p2pvg_set_error("gemm_tc: operands not TMA-compatible (A=%p lda=%lld B=%p ldb=%lld K=%d, driver=%d)", A, lda, B, ldb, K,

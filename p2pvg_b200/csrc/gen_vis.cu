@@ -38,9 +38,10 @@ __global__ void __launch_bounds__(GV_THREADS) gen_vis_kernel(const float* __rest
 
 }  // namespace
 
-int p2pvg_vis_tiles_impl(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
-                         int n_tiles, const int64_t* images_host, int n_images, void* tables_dev, float* out_f, long long n_f,
-                         uint8_t* out_u8, long long n_u8, cudaStream_t st) {
+extern "C" int p2pvg_vis_tiles(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                               int n_tiles, const int64_t* images_host, int n_images, void* tables_dev, float* out_f, long long n_f,
+                               uint8_t* out_u8, long long n_u8, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(tiles_host && images_host && tables_dev, P2PVG_ERR_BAD_ARG, "vis_tiles: null table");
   P2PVG_REQUIRE(((uintptr_t)tables_dev & 7) == 0, P2PVG_ERR_BAD_ARG, "vis_tiles: tables_dev not 8-byte aligned");
   P2PVG_REQUIRE(C == 1 || C == 3, P2PVG_ERR_BAD_ARG, "vis_tiles: C = %d (needs 1 or 3)", C);

@@ -222,13 +222,14 @@ int check_args(const int64_t* segs, int n_seg, const double* edges, int n_edges)
 
 }  // namespace
 
-size_t p2pvg_histograms_workspace_bytes_impl(const int64_t* segs, int n_seg, int n_edges) {
+extern "C" size_t p2pvg_histograms_workspace_bytes(const int64_t* segs, int n_seg, int n_edges) {
   if (n_seg <= 0 || !segs || n_edges < 2 || n_edges > HIST_MAX_EDGES) return 0;
   return layout(segs, n_seg, n_edges).total;
 }
 
-int p2pvg_histograms_impl(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* ws, size_t ws_bytes,
-                          int64_t* counts, double* stats, cudaStream_t st) {
+extern "C" int p2pvg_histograms(const int64_t* segs, int n_seg, const double* edges, int n_edges, void* ws, size_t ws_bytes,
+                                int64_t* counts, double* stats, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   const int rc = check_args(segs, n_seg, edges, n_edges);
   if (rc != P2PVG_OK) return rc;
   if (n_seg == 0) return P2PVG_OK;

@@ -163,18 +163,22 @@ __global__ void scale_kernel(float* __restrict__ x, long long n, float a) {
 
 }  // namespace
 
-int p2pvg_mse_chunks_impl() { return MSE_CHUNKS; }
+extern "C" int p2pvg_mse_chunks(void) { return MSE_CHUNKS; }
 
-int p2pvg_sigmoid_mse_impl(const void* raw, int dtype, const float* x, const int* tgt, const float* coef, int G, long long E,
-                           void* pred, void* d_raw, float* partial, cudaStream_t st) {
+extern "C" int p2pvg_sigmoid_mse(const void* raw, int dtype, const float* x, const int* tgt, const float* coef, int G, int64_t E,
+                                 void* pred, void* d_raw, float* partial, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (G == 0 || E == 0) return P2PVG_OK;
   dim3 grid(MSE_CHUNKS, G);
   DISPATCH_DTYPE(dtype, T, (sigmoid_mse_kernel<T><<<grid, 256, 0, st>>>((const T*)raw, x, tgt, coef, E, (T*)pred, (T*)d_raw, partial)));
   return p2pvg_check_launch("sigmoid_mse");
 }
 
-int p2pvg_convt_c1_loss_impl(const void* col, const void* col2, int dtype, const int* grp_src, const float* bias, const float* x, const int* tgt,
-                             const float* coef, int G, int B, int Hi, int Wi, int C, void* d_raw, float* partial, cudaStream_t st) {
+extern "C" int p2pvg_convt_c1_loss(const void* col, const void* col2, int dtype, const int* grp_src, const float* bias, const float* x,
+                                   const int* tgt, const float* coef, int G, int B, int Hi, int Wi, int C, void* d_raw, float* partial,
+                                   void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  P2PVG_REQUIRE(col && col2 && grp_src && x && tgt && coef && d_raw && partial, P2PVG_ERR_BAD_ARG, "convt_c1_loss: null argument");
   if (G == 0 || B == 0) return P2PVG_OK;
   P2PVG_REQUIRE(C == 1 || C == 3, P2PVG_ERR_UNSUPPORTED, "convt_c1_loss: 1 or 3 output channels (got %d)", C);
   P2PVG_REQUIRE((long long)B * Hi * Wi * 16 * C < (1LL << 31), P2PVG_ERR_UNSUPPORTED, "convt_c1_loss: group too large for 32-bit indexing");
@@ -189,14 +193,16 @@ int p2pvg_convt_c1_loss_impl(const void* col, const void* col2, int dtype, const
   return p2pvg_check_launch("convt_c1_loss");
 }
 
-int p2pvg_finalize_losses_impl(const float* mse_partial, int n_recon, int has_cpc, double E, const float* kl_sum, float batch_size,
-                               const float* align_partial, int n_align, float seq_len, float* out, cudaStream_t st) {
+extern "C" int p2pvg_finalize_losses(const float* mse_partial, int n_recon, int has_cpc, double E, const float* kl_sum, float batch_size,
+                                     const float* align_partial, int n_align, float seq_len, float* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   finalize_losses_kernel<<<1, 32, 0, st>>>(mse_partial, n_recon, has_cpc, MSE_CHUNKS, E, kl_sum, batch_size, align_partial, n_align,
                                            seq_len, out);
   return p2pvg_check_launch("finalize_losses");
 }
 
-int p2pvg_publish_scalars_impl(const float* src, int n, float* host_mapped, const int* seq, cudaStream_t st) {
+extern "C" int p2pvg_publish_scalars(const float* src, int n, float* host_mapped, const int* seq, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0 || n > 64 || !src || !host_mapped || !seq) {
     p2pvg_set_error("publish_scalars: bad arguments");
     return P2PVG_ERR_BAD_ARG;
@@ -205,8 +211,9 @@ int p2pvg_publish_scalars_impl(const float* src, int n, float* host_mapped, cons
   return p2pvg_check_launch("publish_scalars");
 }
 
-int p2pvg_adam_legacy_impl(float* p, const float* g, float* m, float* v, long long n, double lr, double beta1, double beta2, double eps,
-                           const int* step_ptr, cudaStream_t st) {
+extern "C" int p2pvg_adam_legacy(float* p, const float* g, float* m, float* v, int64_t n, double lr, double beta1, double beta2, double eps,
+                                 const int* step_ptr, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return P2PVG_OK;
   P2PVG_REQUIRE(step_ptr != nullptr, P2PVG_ERR_BAD_ARG, "adam: step counter pointer is null");
   long long blocks = (n + 255) / 256;
@@ -215,7 +222,8 @@ int p2pvg_adam_legacy_impl(float* p, const float* g, float* m, float* v, long lo
   return p2pvg_check_launch("adam_legacy");
 }
 
-int p2pvg_scale_impl(float* x, long long n, float a, cudaStream_t st) {
+extern "C" int p2pvg_scale(float* x, int64_t n, float a, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return P2PVG_OK;
   long long blocks = (n + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;

@@ -256,52 +256,60 @@ inline int grid_for(long long total, int block) {
 
 }  // namespace
 
-int p2pvg_lstm_pointwise_fwd_impl(float* gates, const float* c_prev, float* c_out, float* h_out, int B, int R, cudaStream_t st) {
+extern "C" int p2pvg_lstm_pointwise_fwd(float* gates, const float* c_prev, float* c_out, float* h_out, int B, int R, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (B * R == 0) return P2PVG_OK;
   lstm_pointwise_fwd_kernel<<<cdiv((long long)B * R, 256), 256, 0, st>>>(gates, c_prev, c_out, h_out, B, R);
   return p2pvg_check_launch("lstm_pointwise_fwd");
 }
-int p2pvg_lstm_pointwise_bwd_impl(const float* dh, const float* dc_next, const float* gates, const float* c_prev, const float* c,
-                                  float* dgates, float* dc_prev, int B, int R, cudaStream_t st) {
+extern "C" int p2pvg_lstm_pointwise_bwd(const float* dh, const float* dc_next, const float* gates, const float* c_prev, const float* c,
+                                        float* dgates, float* dc_prev, int B, int R, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (B * R == 0) return P2PVG_OK;
   lstm_pointwise_bwd_kernel<<<cdiv((long long)B * R, 256), 256, 0, st>>>(dh, dc_next, gates, c_prev, c, dgates, dc_prev, B, R);
   return p2pvg_check_launch("lstm_pointwise_bwd");
 }
-int p2pvg_reparam_kl_fwd_impl(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
-                              const float* eps_p, float* z, float* z_p, int n, float* kl_sum, cudaStream_t st) {
+extern "C" int p2pvg_reparam_kl_fwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
+                                    const float* eps_p, float* z, float* z_p, int n, float* kl_sum, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   reparam_kl_fwd_kernel<<<RKL_CTAS, 1024, 0, st>>>(mu, lv, mu_p, lv_p, eps, eps_p, z, z_p, n, kl_sum);
   return p2pvg_check_launch("reparam_kl_fwd");
 }
-int p2pvg_reparam_kl_bwd_impl(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
-                              const float* eps_p, const float* dz, const float* dz_p, float kl_coef, float* dmu, float* dlv,
-                              float* dmu_p, float* dlv_p, int n, cudaStream_t st) {
+extern "C" int p2pvg_reparam_kl_bwd(const float* mu, const float* lv, const float* mu_p, const float* lv_p, const float* eps,
+                                    const float* eps_p, const float* dz, const float* dz_p, float kl_coef, float* dmu, float* dlv,
+                                    float* dmu_p, float* dlv_p, int n, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return P2PVG_OK;
   reparam_kl_bwd_kernel<<<cdiv(n, 256), 256, 0, st>>>(mu, lv, mu_p, lv_p, eps, eps_p, dz, dz_p, kl_coef, dmu, dlv, dmu_p, dlv_p, n);
   return p2pvg_check_launch("reparam_kl_bwd");
 }
-int p2pvg_build_concat_impl(float* dst, const float* A, const int* ia, int ga, const float* Bm, const int* ib, int gb,
-                            const float* tuc, const float* dt, int S, int B, int ld, cudaStream_t st) {
+extern "C" int p2pvg_build_concat(float* dst, const float* A, const int* ia, int ga, const float* Bm, const int* ib, int gb,
+                                  const float* tuc, const float* dt, int S, int B, int ld, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(ld >= ga + gb + 2, P2PVG_ERR_BAD_ARG, "build_concat: row pitch %d < %d", ld, ga + gb + 2);
   long long total = (long long)S * B * ld;
   if (total == 0) return P2PVG_OK;
   build_concat_kernel<<<grid_for(total, 256), 256, 0, st>>>(dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld);
   return p2pvg_check_launch("build_concat");
 }
-int p2pvg_gather_add_cols_impl(float* dst, const float* src, const int* idx, int S, int T, int B, int g, int W, int col0, int init,
-                               cudaStream_t st) {
+extern "C" int p2pvg_gather_add_cols(float* dst, const float* src, const int* idx, int S, int T, int B, int g, int W, int col0, int init,
+                                     void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   long long total = (long long)T * B * g;
   if (total == 0) return P2PVG_OK;
   gather_add_cols_kernel<<<grid_for(total, 256), 256, 0, st>>>(dst, src, idx, S, T, B, g, W, col0, init);
   return p2pvg_check_launch("gather_add_cols");
 }
-int p2pvg_align_impl(const float* H, const int* in_idx, const float* h_pred, int P, int B, int g, float coef, float* loss_partial,
-                     float* d_hpred, float* dH, cudaStream_t st) {
+extern "C" int p2pvg_align(const float* H, const int* in_idx, const float* h_pred, int P, int B, int g, float coef, float* loss_partial,
+                           float* d_hpred, float* dH, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (P <= 0) return P2PVG_OK;
   align_kernel<<<P, 1024, 0, st>>>(H, in_idx, h_pred, P, B, g, coef, loss_partial, d_hpred, dH);
   return p2pvg_check_launch("align");
 }
-int p2pvg_colsum_impl(const void* x, int dtype, long long rows, int cols, long long ld, float* out, int accumulate, void* ws,
-                      size_t ws_bytes, cudaStream_t st) {
+extern "C" int p2pvg_colsum(const void* x, int dtype, int64_t rows, int cols, int64_t ld, float* out, int accumulate, void* ws,
+                            size_t ws_bytes, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (cols == 0) return P2PVG_OK;
   // very thin contiguous matrices (bias gradient of a 1/3-channel layer): fold 256 rows into one so that a warp reads 32
   // consecutive elements, then sum the 256*cols folded columns per original column
@@ -309,9 +317,9 @@ int p2pvg_colsum_impl(const void* x, int dtype, long long rows, int cols, long l
   if (cols <= 4 && ld == cols && rows >= 64 * FOLD && rows % FOLD == 0 && ws != nullptr &&
       ws_bytes >= (size_t)(1025 * FOLD * cols) * sizeof(float)) {
     float* tmp = reinterpret_cast<float*>(ws) + (size_t)1024 * FOLD * cols;
-    int rc = p2pvg_colsum_impl(x, dtype, rows / FOLD, FOLD * cols, (long long)FOLD * cols, tmp, 0, ws, (size_t)1024 * FOLD * cols * sizeof(float), st);
+    int rc = p2pvg_colsum(x, dtype, rows / FOLD, FOLD * cols, (long long)FOLD * cols, tmp, 0, ws, (size_t)1024 * FOLD * cols * sizeof(float), st);
     if (rc) return rc;
-    return p2pvg_colsum_impl(tmp, P2PVG_F32, FOLD, cols, cols, out, accumulate, ws, (size_t)1024 * FOLD * cols * sizeof(float), st);
+    return p2pvg_colsum(tmp, P2PVG_F32, FOLD, cols, cols, out, accumulate, ws, (size_t)1024 * FOLD * cols * sizeof(float), st);
   }
   // enough chunks to fill the machine (132 SMs x a few blocks), at least 64 rows per chunk
   long long want = (132LL * 8) / cdiv(cols, 32) + 1;
@@ -328,12 +336,14 @@ int p2pvg_colsum_impl(const void* x, int dtype, long long rows, int cols, long l
   colsum_finish_kernel<<<cdiv(cols, 128), 128, 0, st>>>((const float*)ws, (int)nchunk, cols, out, accumulate);
   return p2pvg_check_launch("colsum");
 }
-int p2pvg_act_fwd_impl(float* x, long long n, int act, cudaStream_t st) {
+extern "C" int p2pvg_act_fwd(float* x, int64_t n, int act, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return P2PVG_OK;
   act_fwd_kernel<<<grid_for(n, 256), 256, 0, st>>>(x, n, act);
   return p2pvg_check_launch("act_fwd");
 }
-int p2pvg_act_bwd_impl(const float* dy, const float* y, float* dx, long long n, int act, cudaStream_t st) {
+extern "C" int p2pvg_act_bwd(const float* dy, const float* y, float* dx, int64_t n, int act, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return P2PVG_OK;
   act_bwd_kernel<<<grid_for(n, 256), 256, 0, st>>>(dy, y, dx, n, act);
   return p2pvg_check_launch("act_bwd");

@@ -367,7 +367,7 @@ int launch_bwd(const float* dhtop, const float* whh, const float* gates, const f
 bool p2pvg_lstm_cluster_supported(int R) { return R == 64 || R == 128 || R == 256; }
 
 // diagnostics: cudaOccupancyMaxActiveClusters of the R = 256 scans (clusters of 8): which = 0 fwd MT=1, 1 fwd MT=2, 2 bwd MT=1, 3 bwd MT=2
-int p2pvg_lstm_cluster_max_clusters_impl(int which) {
+extern "C" int p2pvg_lstm_cluster_max_clusters(int which) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CS * 64);
   cfg.blockDim = dim3(NT);
@@ -397,8 +397,8 @@ int p2pvg_lstm_cluster_max_clusters_impl(int which) {
 // slabs of 32 rows (MT = 2) above this batch size: fewer clusters of 8 CTAs, so that large batches need fewer waves
 constexpr int kMt2Above = 128;
 
-int p2pvg_lstm_cluster_fwd_impl(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
-                                int R, cudaStream_t st) {
+int p2pvg_lstm_cluster_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                           int R, cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   const bool two = B > kMt2Above;
   switch (R) {
@@ -410,8 +410,8 @@ int p2pvg_lstm_cluster_fwd_impl(const float* pre, const float* whh, const float*
   return P2PVG_ERR_UNSUPPORTED;
 }
 
-int p2pvg_lstm_cluster_bwd_impl(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
-                                cudaStream_t st) {
+int p2pvg_lstm_cluster_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
+                           cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   const bool two = B > kMt2Above;
   switch (R) {

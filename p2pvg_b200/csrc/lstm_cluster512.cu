@@ -433,7 +433,7 @@ int launch_cluster16(Kern kern, const char* what, int grid, size_t smem, cudaStr
 }  // namespace
 
 // cudaOccupancyMaxActiveClusters of the cluster-16 scans (which = 0: forward 16-row slabs, 1: 32 rows, 3: 48 rows, 2: backward 16 rows)
-int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
+extern "C" int p2pvg_lstm_cluster512_max_clusters(int which) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CS * 64);
   cfg.blockDim = dim3(NT);
@@ -478,7 +478,7 @@ int p2pvg_lstm_cluster512_max_clusters_impl(int which) {
 static int fwd_slab_tiles(int B) {
   static int maxc = 0;
   if (maxc == 0) {
-    maxc = p2pvg_lstm_cluster512_max_clusters_impl(1);
+    maxc = p2pvg_lstm_cluster512_max_clusters(1);
     if (maxc <= 0) maxc = 7;
   }
   int best = 1;
@@ -491,8 +491,8 @@ static int fwd_slab_tiles(int B) {
   return best;
 }
 
-int p2pvg_lstm_cluster512_fwd_impl(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
-                                   cudaStream_t st) {
+int p2pvg_lstm_cluster512_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                              cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   static bool a1 = false, a2 = false, a3 = false;
   const int mt = fwd_slab_tiles(B);
@@ -501,8 +501,8 @@ int p2pvg_lstm_cluster512_fwd_impl(const float* pre, const float* whh, const flo
   return launch_cluster16(lstm_cl16_fwd_kernel<1>, "lstm_cl16_fwd", CS * cdiv(B, 16), fwd_smem(1), st, a1, pre, whh, bhh, gates, hs, cs, S, B);
 }
 
-int p2pvg_lstm_cluster512_bwd_impl(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B,
-                                   cudaStream_t st) {
+int p2pvg_lstm_cluster512_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B,
+                              cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   // 16-row slabs: the receive slots of larger slabs leave no shared memory for the weight half that does not fit the registers
   static bool a = false;

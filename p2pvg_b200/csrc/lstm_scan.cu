@@ -276,8 +276,8 @@ size_t g_fwd_attr = 0, g_bwd_attr = 0;  // largest dynamic shared memory size en
 
 }  // namespace
 
-int p2pvg_lstm_scan_fwd_impl(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
-                             int R, int tf32, unsigned* counter, cudaStream_t st) {
+static int cooperative_scan_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                                int R, int tf32, unsigned* counter, cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   P2PVG_REQUIRE(R % 8 == 0 && R % 4 == 0, P2PVG_ERR_UNSUPPORTED, "lstm_scan: hidden size %d must be a multiple of 8", R);
   const size_t smem = (size_t)(32 * (R + PAD) + RB * (R + PAD) + RB * 33) * sizeof(float);
@@ -300,8 +300,8 @@ int p2pvg_lstm_scan_fwd_impl(const float* pre, const float* whh, const float* bh
   return P2PVG_OK;
 }
 
-int p2pvg_lstm_scan_bwd_impl(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
-                             int tf32, unsigned* counter, cudaStream_t st) {
+static int cooperative_scan_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
+                                int tf32, unsigned* counter, cudaStream_t st) {
   if (S <= 0 || B <= 0) return P2PVG_OK;
   P2PVG_REQUIRE(R % 64 == 0, P2PVG_ERR_UNSUPPORTED, "lstm_scan_bwd: hidden size %d must be a multiple of 64", R);
   const size_t smem = (size_t)(UB * (4 * R + PAD) + RB * (256 + PAD) + 2 * RB * 9) * sizeof(float);
@@ -322,4 +322,22 @@ int p2pvg_lstm_scan_bwd_impl(const float* dhtop, const float* whh, const float* 
     return P2PVG_ERR_CUDA;
   }
   return P2PVG_OK;
+}
+
+// tensor-core mode: thread-block-cluster scans, clusters of 16 CTAs for R = 512 (BASELINE config 5, lstm_cluster512.cu) and of 8
+// CTAs for R in {64,128,256} (lstm_cluster.cu); the exact-fp32 mode runs the cooperative-grid scans
+extern "C" int p2pvg_lstm_scan_fwd(const float* pre, const float* whh, const float* bhh, float* gates, float* hs, float* cs, int S, int B,
+                                   int R, int tf32, unsigned* counter, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tf32 && R == 512) return p2pvg_lstm_cluster512_fwd(pre, whh, bhh, gates, hs, cs, S, B, st);
+  if (tf32 && p2pvg_lstm_cluster_supported(R)) return p2pvg_lstm_cluster_fwd(pre, whh, bhh, gates, hs, cs, S, B, R, st);
+  return cooperative_scan_fwd(pre, whh, bhh, gates, hs, cs, S, B, R, tf32, counter, st);
+}
+
+extern "C" int p2pvg_lstm_scan_bwd(const float* dhtop, const float* whh, const float* gates, const float* cs, float* dG, int S, int B, int R,
+                                   int tf32, unsigned* counter, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tf32 && R == 512) return p2pvg_lstm_cluster512_bwd(dhtop, whh, gates, cs, dG, S, B, st);
+  if (tf32 && p2pvg_lstm_cluster_supported(R)) return p2pvg_lstm_cluster_bwd(dhtop, whh, gates, cs, dG, S, B, R, st);
+  return cooperative_scan_bwd(dhtop, whh, gates, cs, dG, S, B, R, tf32, counter, st);
 }

@@ -10,7 +10,6 @@
 
 #include "cluster_rows.cuh"
 #include "common.cuh"
-#include "../../include/p2pvg_b200.h"
 
 namespace cg = cooperative_groups;
 
@@ -125,7 +124,8 @@ lstm_step_kernel(p2pvg_lstm_step_module m0, p2pvg_lstm_step_module m1, int rows,
 
 }  // namespace
 
-int p2pvg_lstm_step_impl(const p2pvg_lstm_step_module* mods, int n_mods, int rows, int R, cudaStream_t st) {
+extern "C" int p2pvg_lstm_step(const p2pvg_lstm_step_module* mods, int n_mods, int rows, int R, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(mods != nullptr && (n_mods == 1 || n_mods == 2), P2PVG_ERR_BAD_ARG, "lstm_step: 1 or 2 modules");
   P2PVG_REQUIRE(R % CS == 0 && R >= 64 && R <= 512, P2PVG_ERR_UNSUPPORTED, "lstm_step: hidden size %d (64..512, multiple of 8)", R);
   int in_max = 0;

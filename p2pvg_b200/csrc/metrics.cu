@@ -197,8 +197,9 @@ __global__ void __launch_bounds__(PM_THREADS) pose_metrics_kernel(const float* _
 
 }  // namespace
 
-int p2pvg_frame_metrics_impl(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int C, int H, int W,
-                             float data_range, double* out, cudaStream_t st) {
+extern "C" int p2pvg_frame_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int C, int H, int W,
+                                   float data_range, double* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(pred && gt && ((pairs && out) || n_pairs == 0), P2PVG_ERR_BAD_ARG, "frame_metrics: null pointer");
   P2PVG_REQUIRE(((uintptr_t)pred & 15) == 0 && ((uintptr_t)gt & 15) == 0 && ((uintptr_t)pairs & 3) == 0 &&
                     ((uintptr_t)out & 7) == 0,
@@ -216,8 +217,8 @@ int p2pvg_frame_metrics_impl(const float* pred, const float* gt, const int32_t* 
   return p2pvg_check_launch("frame_metrics");
 }
 
-int p2pvg_pose_metrics_impl(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out,
-                            cudaStream_t st) {
+extern "C" int p2pvg_pose_metrics(const float* pred, const float* gt, const int32_t* pairs, int n_pairs, int J, double* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(pred && gt && ((pairs && out) || n_pairs == 0), P2PVG_ERR_BAD_ARG, "pose_metrics: null pointer");
   P2PVG_REQUIRE(((uintptr_t)pred & 3) == 0 && ((uintptr_t)gt & 3) == 0 && ((uintptr_t)pairs & 3) == 0 && ((uintptr_t)out & 7) == 0,
                 P2PVG_ERR_BAD_ARG, "pose_metrics: misaligned pointer");

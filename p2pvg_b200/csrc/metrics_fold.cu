@@ -112,9 +112,10 @@ __global__ void __launch_bounds__(MF_THREADS) metrics_fold_kernel(const double* 
 
 }  // namespace
 
-int p2pvg_metrics_fold_impl(const double* scores, int n_metrics, int higher_mask, int B, int nsample, const int32_t* segs, int n_seg,
-                            const int32_t* col_bin, int n_cols, int n_bins, double* part_v, int32_t* part_c, unsigned int* counter,
-                            double* sums, unsigned long long* counts, unsigned long long* rows, cudaStream_t st) {
+extern "C" int p2pvg_metrics_fold(const double* scores, int n_metrics, int higher_mask, int B, int nsample, const int32_t* segs, int n_seg,
+                                  const int32_t* col_bin, int n_cols, int n_bins, double* part_v, int32_t* part_c, uint32_t* counter,
+                                  double* sums, uint64_t* counts, uint64_t* rows, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(scores && segs && col_bin && part_v && part_c && counter && sums && counts && rows, P2PVG_ERR_BAD_ARG,
                 "metrics_fold: null pointer");
   P2PVG_REQUIRE(((uintptr_t)scores & 7) == 0 && ((uintptr_t)part_v & 7) == 0 && ((uintptr_t)sums & 7) == 0 &&
@@ -129,6 +130,7 @@ int p2pvg_metrics_fold_impl(const double* scores, int n_metrics, int higher_mask
                 "metrics_fold: too many (column, row, metric) values");
   const unsigned grid = (unsigned)((tasks + MF_THREADS - 1) / MF_THREADS);
   metrics_fold_kernel<<<grid, MF_THREADS, 0, st>>>(scores, n_metrics, higher_mask, B, nsample, segs, n_seg, col_bin, n_cols, n_bins,
-                                                   part_v, part_c, counter, sums, counts, rows);
+                                                   part_v, part_c, counter, sums, (unsigned long long*)counts,
+                                                   (unsigned long long*)rows);
   return p2pvg_check_launch("metrics_fold");
 }

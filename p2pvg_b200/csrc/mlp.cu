@@ -127,15 +127,17 @@ __global__ void __launch_bounds__(256) mse_plain_kernel(const float* __restrict_
 
 }  // namespace
 
-int p2pvg_layernorm_fwd_impl(const float* x, const float* gamma, const float* beta, float* y, float* mean, float* rstd, long long rows,
-                             int C, float eps, cudaStream_t st) {
+extern "C" int p2pvg_layernorm_fwd(const float* x, const float* gamma, const float* beta, float* y, float* mean, float* rstd, int64_t rows,
+                                   int C, float eps, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (rows == 0) return P2PVG_OK;
   layernorm_fwd_kernel<<<cdiv(rows, 8), 256, 0, st>>>(x, gamma, beta, y, mean, rstd, rows, C, eps);
   return p2pvg_check_launch("layernorm_fwd");
 }
 
-int p2pvg_layernorm_bwd_impl(const float* dy, const float* x, const float* mean, const float* rstd, const float* gamma, float* dx,
-                             float* dgamma, float* dbeta, long long rows, int C, void* ws, size_t ws_bytes, cudaStream_t st) {
+extern "C" int p2pvg_layernorm_bwd(const float* dy, const float* x, const float* mean, const float* rstd, const float* gamma, float* dx,
+                                   float* dgamma, float* dbeta, int64_t rows, int C, void* ws, size_t ws_bytes, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (rows == 0) return P2PVG_OK;
   if (dgamma) {  // parameter gradients first: dx may alias dy
     long long nchunk = (rows + 255) / 256;
@@ -152,10 +154,11 @@ int p2pvg_layernorm_bwd_impl(const float* dy, const float* x, const float* mean,
   return p2pvg_check_launch("layernorm_bwd");
 }
 
-int p2pvg_mse_plain_impl(const float* pred, const float* x, const int* tgt, const float* coef, int G, long long E, float* d_pred,
-                         float* partial, int chunks, cudaStream_t st) {
+extern "C" int p2pvg_mse_plain(const float* pred, const float* x, const int* tgt, const float* coef, int G, int64_t E, float* d_pred,
+                               float* partial, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (G == 0 || E == 0) return P2PVG_OK;
-  dim3 grid(chunks, G);
+  dim3 grid(p2pvg_mse_chunks(), G);
   mse_plain_kernel<<<grid, 256, 0, st>>>(pred, x, tgt, coef, E, d_pred, partial);
   return p2pvg_check_launch("mse_plain");
 }

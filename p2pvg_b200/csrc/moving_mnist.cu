@@ -108,8 +108,9 @@ __global__ void __launch_bounds__(MM_THREADS) moving_mnist_kernel(const uint8_t*
 
 }  // namespace
 
-int p2pvg_moving_mnist_impl(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B,
-                            int S, int num_digits, int deterministic, cudaStream_t st) {
+extern "C" int p2pvg_moving_mnist(const uint8_t* digits, int n_digits, const int32_t* draws, int draw_stride, float* out, int T, int B,
+                                  int S, int num_digits, int deterministic, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(digits && draws && out, P2PVG_ERR_BAD_ARG, "moving_mnist: null pointer");
   P2PVG_REQUIRE(n_digits >= 1, P2PVG_ERR_BAD_ARG, "moving_mnist: n_digits = %d", n_digits);
   P2PVG_REQUIRE(S >= MM_DIGIT + 1 && S % 4 == 0, P2PVG_ERR_BAD_ARG, "moving_mnist: S = %d (needs S >= 33, S %% 4 == 0)", S);

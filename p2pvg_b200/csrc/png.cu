@@ -745,18 +745,19 @@ size_t out_bound(const int64_t* images, int n) {
 
 }  // namespace
 
-size_t p2pvg_png_workspace_bytes_impl(const int64_t* images, int n) {
+extern "C" size_t p2pvg_png_workspace_bytes(const int64_t* images, int n) {
   if (check_images(images, n, 0) != P2PVG_OK) return 0;
   return layout(images, n).total;
 }
 
-size_t p2pvg_png_out_bytes_impl(const int64_t* images, int n) {
+extern "C" size_t p2pvg_png_out_bytes(const int64_t* images, int n) {
   if (check_images(images, n, 0) != P2PVG_OK) return 0;
   return out_bound(images, n);
 }
 
-int p2pvg_png_encode_impl(const int64_t* images, int n, int rule, void* ws, size_t ws_bytes, uint8_t* out, size_t out_bytes,
-                          int64_t* files, cudaStream_t st) {
+extern "C" int p2pvg_png_encode(const int64_t* images, int n, int rule, void* ws, size_t ws_bytes, uint8_t* out, size_t out_bytes,
+                                int64_t* files, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   const int rc = check_images(images, n, rule);
   if (rc != P2PVG_OK) return rc;
   if (n == 0) return P2PVG_OK;
@@ -792,7 +793,7 @@ int p2pvg_png_encode_impl(const int64_t* images, int n, int rule, void* ws, size
   const Seg* d_seg = reinterpret_cast<const Seg*>(w + L.off_segs);
   long long* meta = reinterpret_cast<long long*>(w + L.off_meta);
   long long* piece = reinterpret_cast<long long*>(w + L.off_piece);
-  uint8_t* stream = w + L.off_stream;
+  uint8_t* filtered = w + L.off_stream;
   uint8_t* slots = w + L.off_slots;
 
   int dev = 0;
@@ -806,9 +807,9 @@ int p2pvg_png_encode_impl(const int64_t* images, int n, int rule, void* ws, size
     }
     if (dev < 64) attr_set |= 1ULL << dev;
   }
-  filter_kernel<<<(unsigned)L.rows, PNG_THREADS, 0, st>>>(d_img, n, rule, stream);
+  filter_kernel<<<(unsigned)L.rows, PNG_THREADS, 0, st>>>(d_img, n, rule, filtered);
   deflate_kernel<<<(unsigned)L.n_seg, PNG_THREADS, sizeof(DeflateSmem), st>>>(
-      d_img, d_seg, stream, reinterpret_cast<uint16_t*>(w + L.off_cand), reinterpret_cast<unsigned*>(w + L.off_tok), slots,
+      d_img, d_seg, filtered, reinterpret_cast<uint16_t*>(w + L.off_cand), reinterpret_cast<unsigned*>(w + L.off_tok), slots,
       meta);
   scan_kernel<<<1, 1024, 0, st>>>(d_img, n, d_seg, L.n_seg, meta, piece, reinterpret_cast<long long*>(files));
   container_kernel<<<(unsigned)L.n_seg, PNG_THREADS, 0, st>>>(d_img, d_seg, meta, slots, piece, out);

@@ -32,9 +32,10 @@ __global__ void __launch_bounds__(PW_THREADS) pose_windows_kernel(const float* _
 
 }  // namespace
 
-int p2pvg_pose_windows_impl(const float* pose2d, const float* pose3d, int J, const int64_t* seq_first, const int32_t* seq_len,
-                            int n_seq, const int32_t* entries, const int32_t* draws, int B, int speed_lo, int speed_hi, int L, int T,
-                            float* out2d, float* out3d, cudaStream_t st) {
+extern "C" int p2pvg_pose_windows(const float* pose2d, const float* pose3d, int J, const int64_t* seq_first, const int32_t* seq_len,
+                                  int n_seq, const int32_t* entries, const int32_t* draws, int B, int speed_lo, int speed_hi, int L, int T,
+                                  float* out2d, float* out3d, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(pose2d && pose3d && seq_first && seq_len && entries && draws && out2d && out3d, P2PVG_ERR_BAD_ARG,
                 "pose_windows: null pointer");
   P2PVG_REQUIRE((((uintptr_t)pose2d | (uintptr_t)pose3d | (uintptr_t)seq_len | (uintptr_t)entries | (uintptr_t)draws |

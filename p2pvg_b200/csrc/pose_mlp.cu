@@ -11,7 +11,6 @@
 
 #include "cluster_rows.cuh"
 #include "common.cuh"
-#include "../../include/p2pvg_b200.h"
 
 namespace cg = cooperative_groups;
 
@@ -176,7 +175,8 @@ bool residual_complete(const p2pvg_pose_residual& p) {
 
 }  // namespace
 
-int p2pvg_pose_mlp_impl(const p2pvg_pose_mlp_args* args, int rows, cudaStream_t st) {
+extern "C" int p2pvg_pose_mlp(const p2pvg_pose_mlp_args* args, int rows, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(args != nullptr && rows >= 0, P2PVG_ERR_BAD_ARG, "pose_mlp: bad arguments");
   const p2pvg_pose_mlp_args& a = *args;
   P2PVG_REQUIRE(a.g >= 8, P2PVG_ERR_BAD_ARG, "pose_mlp: g = %d (>= 8)", a.g);

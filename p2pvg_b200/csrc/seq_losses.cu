@@ -115,14 +115,15 @@ __global__ void __launch_bounds__(SL_THREADS) seq_losses_kernel(const T* __restr
 
 }  // namespace
 
-int p2pvg_seq_losses_impl(const void* rec, int dtype, int sigmoid, const float* x, const int* tgt, int S, int B, long long E,
-                          const float* mu, const float* lv, const float* mu_p, const float* lv_p, int z, const float* H,
-                          const int* in_idx, const float* h_pred, int g, int has_cpc, double batch_size, double seq_len,
-                          double* partial, unsigned int* counter, double* per_seq, double* out, cudaStream_t st) {
+extern "C" int p2pvg_seq_losses(const void* rec, int dtype, int sigmoid, const float* x, const int* tgt, int S, int B, int64_t E,
+                                const float* mu, const float* lv, const float* mu_p, const float* lv_p, int z, const float* H,
+                                const int* in_idx, const float* h_pred, int g, int has_cpc, double batch_size, double seq_len,
+                                double* partial, uint32_t* counter, double* per_seq, double* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(rec && x && tgt && mu && lv && mu_p && lv_p && H && in_idx && h_pred && partial && counter && per_seq && out,
                 P2PVG_ERR_BAD_ARG, "seq_losses: null pointer");
   P2PVG_REQUIRE(S >= 1 && B >= 1 && E >= 1 && z >= 1 && g >= 1 && batch_size > 0.0 && seq_len > 0.0, P2PVG_ERR_BAD_ARG,
-                "seq_losses: bad shape (S %d, B %d, E %lld, z %d, g %d)", S, B, E, z, g);
+                "seq_losses: bad shape (S %d, B %d, E %lld, z %d, g %d)", S, B, (long long)E, z, g);
   // 4-wide loads when every row starts on a vector boundary (16 B for fp32, 8 B for bf16)
   const int vec = (E & 3) == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)rec & (dtype == P2PVG_BF16 ? 7 : 15)) == 0;
   const long long grid = (long long)(S + 1) * B;

@@ -259,7 +259,8 @@ inline bool vec_ok(int dtype, int C, long long total, const void* a, const void*
 
 }  // namespace
 
-int p2pvg_im2col3_impl(const void* x, void* col, int dtype, int N, int H, int W, int C, int ld, int sgn, cudaStream_t st) {
+extern "C" int p2pvg_im2col3(const void* x, void* col, int dtype, int N, int H, int W, int C, int ld, int sgn, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(ld >= 9 * C, P2PVG_ERR_BAD_ARG, "im2col3: ld %d < 9*C", ld);
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * H * W * ld;
@@ -274,7 +275,8 @@ int p2pvg_im2col3_impl(const void* x, void* col, int dtype, int N, int H, int W,
   return p2pvg_check_launch("im2col3");
 }
 
-int p2pvg_col2im3_impl(const void* col, void* y, int dtype, int N, int H, int W, int C, int ld, const float* bias, cudaStream_t st) {
+extern "C" int p2pvg_col2im3(const void* col, void* y, int dtype, int N, int H, int W, int C, int ld, const float* bias, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(ld >= 9 * C, P2PVG_ERR_BAD_ARG, "col2im3: ld %d < 9*C", ld);
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * H * W * C;
@@ -282,7 +284,8 @@ int p2pvg_col2im3_impl(const void* col, void* y, int dtype, int N, int H, int W,
   return p2pvg_check_launch("col2im3");
 }
 
-int p2pvg_maxpool2_fwd_impl(const void* x, void* y, int dtype, int N, int H, int W, int C, cudaStream_t st) {
+extern "C" int p2pvg_maxpool2_fwd(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(H % 2 == 0 && W % 2 == 0, P2PVG_ERR_BAD_ARG, "maxpool2: odd map %dx%d", H, W);
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * (H / 2) * (W / 2) * C;
@@ -296,7 +299,8 @@ int p2pvg_maxpool2_fwd_impl(const void* x, void* y, int dtype, int N, int H, int
   return p2pvg_check_launch("maxpool2_fwd");
 }
 
-int p2pvg_maxpool2_bwd_impl(const void* x, const void* dy, void* dx, int dtype, int N, int H, int W, int C, cudaStream_t st) {
+extern "C" int p2pvg_maxpool2_bwd(const void* x, const void* dy, void* dx, int dtype, int N, int H, int W, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(H % 2 == 0 && W % 2 == 0, P2PVG_ERR_BAD_ARG, "maxpool2: odd map %dx%d", H, W);
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * (H / 2) * (W / 2) * C;
@@ -310,7 +314,8 @@ int p2pvg_maxpool2_bwd_impl(const void* x, const void* dy, void* dx, int dtype, 
   return p2pvg_check_launch("maxpool2_bwd");
 }
 
-int p2pvg_upsample2_fwd_impl(const void* x, void* y, int dtype, int N, int H, int W, int C, cudaStream_t st) {
+extern "C" int p2pvg_upsample2_fwd(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * 4 * H * W * C;
   if (vec_ok(dtype, C, total / 4, x, y, nullptr)) {
@@ -323,7 +328,8 @@ int p2pvg_upsample2_fwd_impl(const void* x, void* y, int dtype, int N, int H, in
   return p2pvg_check_launch("upsample2_fwd");
 }
 
-int p2pvg_upsample2_bwd_impl(const void* dy, void* dx, int dtype, int N, int H, int W, int C, cudaStream_t st) {
+extern "C" int p2pvg_upsample2_bwd(const void* dy, void* dx, int dtype, int N, int H, int W, int C, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return P2PVG_OK;
   const long long total = (long long)N * H * W * C;
   if (vec_ok(dtype, C, total, dy, dx, nullptr)) {
@@ -336,7 +342,8 @@ int p2pvg_upsample2_bwd_impl(const void* dy, void* dx, int dtype, int N, int H, 
   return p2pvg_check_launch("upsample2_bwd");
 }
 
-int p2pvg_gather_add_impl(void* dst, int dtype, const float* src, const int* grp_src, int G, long long n, cudaStream_t st) {
+extern "C" int p2pvg_gather_add(void* dst, int dtype, const float* src, const int* grp_src, int G, int64_t n, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   if (G == 0 || n == 0) return P2PVG_OK;
   DISPATCH_DTYPE(dtype, T, (gather_add_kernel<T><<<grid_for((long long)G * n, 256), 256, 0, st>>>((T*)dst, src, grp_src, G, n)));
   return p2pvg_check_launch("gather_add");

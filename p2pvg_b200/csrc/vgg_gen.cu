@@ -149,8 +149,9 @@ int last_nc(int nc, const void* d, const float* w, const float* bias, float* out
 
 }  // namespace
 
-int p2pvg_vgg_first_eval_impl(const float* x, int nc, const float* w, const float* bias, const float* scale, const float* shift, void* y,
-                              int y_dtype, int N, int H, int W, cudaStream_t st) {
+extern "C" int p2pvg_vgg_first_eval(const float* x, int nc, const float* w, const float* bias, const float* scale, const float* shift,
+                                    void* y, int y_dtype, int N, int H, int W, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(x && w && bias && scale && shift && y, P2PVG_ERR_BAD_ARG, "vgg_first_eval: null argument");
   P2PVG_REQUIRE(N >= 0 && H >= 1 && W >= 1, P2PVG_ERR_BAD_ARG, "vgg_first_eval: bad size N=%d H=%d W=%d", N, H, W);
   P2PVG_REQUIRE((reinterpret_cast<uintptr_t>(y) & 15) == 0, P2PVG_ERR_BAD_ARG, "vgg_first_eval: y must be 16-byte aligned");
@@ -161,8 +162,9 @@ int p2pvg_vgg_first_eval_impl(const float* x, int nc, const float* w, const floa
   return P2PVG_OK;
 }
 
-int p2pvg_vgg_last_eval_impl(const void* d, int d_dtype, const float* w, const float* bias, float* out, int nc, int N, int H, int W,
-                             cudaStream_t st) {
+extern "C" int p2pvg_vgg_last_eval(const void* d, int d_dtype, const float* w, const float* bias, float* out, int nc, int N, int H, int W,
+                                   void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(d && w && bias && out, P2PVG_ERR_BAD_ARG, "vgg_last_eval: null argument");
   P2PVG_REQUIRE(N >= 0 && H >= 1 && W >= 1, P2PVG_ERR_BAD_ARG, "vgg_last_eval: bad size N=%d H=%d W=%d", N, H, W);
   P2PVG_REQUIRE((reinterpret_cast<uintptr_t>(d) & 15) == 0, P2PVG_ERR_BAD_ARG, "vgg_last_eval: d must be 16-byte aligned");

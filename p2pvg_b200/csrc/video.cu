@@ -58,9 +58,10 @@ __global__ void __launch_bounds__(VW_THREADS) video_windows_kernel(const uint8_t
 
 }  // namespace
 
-int p2pvg_video_windows_impl(const uint8_t* frames, const int64_t* clip_first, const int32_t* clip_len, int n_clips,
-                             const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H,
-                             int W, float* out, cudaStream_t st) {
+extern "C" int p2pvg_video_windows(const uint8_t* frames, const int64_t* clip_first, const int32_t* clip_len, int n_clips,
+                                   const int32_t* entries, const int32_t* draws, int paired_flips, int B, int L, int T, int C, int H, int W,
+                                   float* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(frames && clip_first && clip_len && entries && out, P2PVG_ERR_BAD_ARG, "video_windows: null pointer");
   P2PVG_REQUIRE(((uintptr_t)frames & 3) == 0 && ((uintptr_t)out & 15) == 0, P2PVG_ERR_BAD_ARG,
                 "video_windows: frames must be 4-byte and out 16-byte aligned");

@@ -41,9 +41,9 @@ __global__ void __launch_bounds__(VIS_THREADS) vis_canvas_kernel(const float* __
 
 }  // namespace
 
-int p2pvg_vis_canvas_impl(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
-                          int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif,
-                          cudaStream_t st) {
+extern "C" int p2pvg_vis_canvas(const float* store0, int n0, const float* store1, int n1, int C, int H, const int32_t* tiles_host,
+                                int32_t* tiles_dev, int r_len, int n_block, float* canvas, float* video, uint8_t* gif, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
   P2PVG_REQUIRE(tiles_host && tiles_dev && canvas && video && gif, P2PVG_ERR_BAD_ARG, "vis_canvas: null pointer");
   P2PVG_REQUIRE(C == 1 || C == 3, P2PVG_ERR_BAD_ARG, "vis_canvas: C = %d (needs 1 or 3)", C);
   P2PVG_REQUIRE(H >= 1 && H <= VIS_MAX_W, P2PVG_ERR_BAD_ARG, "vis_canvas: H = W = %d (needs 1..%d)", H, VIS_MAX_W);

@@ -26,3 +26,8 @@ def test_library_exports_every_declared_symbol():
     missing = [n for n in sorted(names) if not hasattr(lib, n)]
     assert not missing, missing
     assert lib.p2pvg_version() >= 100
+    # and the other way round: every entry point the ctypes binding calls is declared in the header
+    called = set(re.findall(r"lib\.(p2pvg_[a-z0-9_]+)", open(os.path.join(ROOT, "p2pvg_b200", "_lib.py")).read()))
+    assert len(called) > 30
+    undeclared = sorted(called - names)
+    assert not undeclared, undeclared
