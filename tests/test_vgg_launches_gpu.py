@@ -155,10 +155,18 @@ def _dedup(launches):
     return out
 
 
+def encoder_first(backward):
+    """A backward list with the encoder's launches first, in layer order (the engine runs them last, in reverse): each shape
+    is then represented by its longest launch (all T B frames) under the encoder layer's name."""
+    enc = [L for L in backward if L["name"].startswith("enc")]
+    return enc[::-1] + [L for L in backward if not L["name"].startswith("enc")]
+
+
 def _c3_conv_launches():
     p = c3_plan()
     T, B = C3["T"], C3["B"]
-    return _dedup([L for L in forward_launches(T, B, p.S, p.nskip) + backward_launches(T, B, p.S, p.nskip) if L["kind"] != 4])
+    return _dedup([L for L in forward_launches(T, B, p.S, p.nskip) + encoder_first(backward_launches(T, B, p.S, p.nskip, has_cpc=p.has_cpc))
+                   if L["kind"] != 4])
 
 
 C3_CONV = _c3_conv_launches()
@@ -166,16 +174,25 @@ C3_CONV = _c3_conv_launches()
 
 def test_c3_launch_list_matches_the_engine():
     """The derived list has the rows the C3 table has: bres at 64x64, fused statistics exactly from 16x16 down, a bf16 addend
-    on every decoder stage entry, and a data gradient per layer."""
+    on every decoder stage entry, and a data gradient per layer: the decoder's at S B = 3712 images (reconstruction calls)
+    and B = 128 (the CPC decode and the skip halves), the encoder's at T B = 3840 but none for the first layer."""
     p = c3_plan()
     fwd = forward_launches(C3["T"], C3["B"], p.S, p.nskip)
-    assert p.S == 29 and p.nskip == 1
+    bwd = backward_launches(C3["T"], C3["B"], p.S, p.nskip, has_cpc=p.has_cpc)
+    assert p.S == 29 and p.nskip == 1 and p.has_cpc
     assert [(L["H"], L["stat"] is not None) for L in fwd if L["name"].startswith("enc")] == \
         [(64, False), (32, False), (32, False), (16, True), (16, True), (16, True), (8, True), (8, True), (8, True)]
     entries = [L for L in fwd if L["name"].endswith(".D")]
     assert [(L["H"], L["stat"] is not None, L["ipg"]) for L in entries] == [(8, True, 128), (16, True, 128), (32, False, 128), (64, False, 128)]
     assert all(L["N"] == 3840 for L in fwd if not L["name"].endswith(".S"))
     assert all(L["N"] == 128 for L in fwd if L["name"].endswith(".S"))
+    dec = [L for L in bwd if "dec" in L["name"]]
+    assert {(L["kind"], L["N"]) for L in dec if L["name"].startswith("dec") and ".S " not in L["name"]} == {(5, 3712), (4, 3712)}
+    assert {(L["kind"], L["N"]) for L in dec if ".S " in L["name"]} == {(5, 128), (4, 128)}
+    assert {(L["kind"], L["N"]) for L in dec if L["name"].startswith("cpc ")} == {(5, 128)}
+    assert sum(L["kind"] == 5 for L in dec) == 2 * 9 + 4
+    assert {L["N"] for L in bwd if L["name"].startswith("enc")} == {3840}
+    assert not any(L["name"].startswith("enc0.0") for L in bwd)
 
 
 @pytest.mark.parametrize("L", C3_CONV, ids=[L["name"].replace(" ", "_") for L in C3_CONV])
@@ -184,11 +201,11 @@ def test_c3_conv_launch(K, sms, L):
     run_conv(K, sms, L, torch.bfloat16, seed=21)
 
 
-def _wgrad_classes():
-    p = c3_plan()
+def wgrad_classes(launches):
+    """The first kind-4 launch of each (map size, swapped roles) class of a backward list, encoder launches first."""
     sms_ = sm_count() if torch.cuda.is_available() else 132
     seen, out = set(), []
-    for L in backward_launches(C3["T"], C3["B"], p.S, p.nskip):
+    for L in encoder_first(launches):
         if L["kind"] != 4:
             continue
         s = conv_tiles(4, L["N"], L["H"], L["H"], 0, L["Cn"], L["Cm"], sms_)
@@ -198,16 +215,22 @@ def _wgrad_classes():
     return out
 
 
-C3_WGRAD = _wgrad_classes()
+_p = c3_plan()
+C3_WGRAD = wgrad_classes(backward_launches(C3["T"], C3["B"], _p.S, _p.nskip, has_cpc=_p.has_cpc))
 
 
 @pytest.mark.parametrize("L", C3_WGRAD, ids=[f"{L['H']}x{L['H']}_{L['Cm']}x{L['Cn']}" for L in C3_WGRAD])
 def test_c3_weight_gradient(K, sms, L):
     """One kind-4 launch per (map size, swapped roles) class at C3 size, against a full float64 reduction over all
-    N * H * W pixels (K = 15.7M at 64x64).  Zero-mean operands would cancel: over such a K the worst-case accumulation bound
-    is larger than the result itself.  So (1) 0 / 1 operands, whose fp32 sums are exact integers: the result must equal
-    float64 bit for bit, and one lost 64-pixel block or split changes it; (2) real operands that do not cancel (one positive,
-    one of mean 1/2), so that the bound is a small fraction of the value."""
+    N * H * W pixels (K = 15.7M at 64x64)."""
+    run_wgrad(K, sms, L)
+
+
+def run_wgrad(K, sms, L):
+    """A kind-4 launch as L describes.  Zero-mean operands would cancel: over K = N H W the worst-case accumulation bound is
+    larger than the result itself.  So (1) 0 / 1 operands, whose fp32 sums are exact integers: the result must equal float64
+    bit for bit, and one lost 64-pixel block or split changes it; (2) real operands that do not cancel (one positive, one of
+    mean 1/2), so that the bound is a small fraction of the value."""
     N, H, Cm, Cn = L["N"], L["H"], L["Cm"], L["Cn"]
     s = conv_tiles(4, N, H, H, 0, Cn, Cm, sms)
     name = f"wgrad {L['name']} {H}x{H} {Cm}x{Cn} swap={s.swap} splits={s.splits}"
@@ -228,9 +251,14 @@ def test_c3_weight_gradient(K, sms, L):
 
 
 def test_c3_end_gemms(K):
-    """The explicit GEMMs of the 3-channel ends at C3 size: the first encoder layer ([M, 32] x [64, 32] after im2col3) and the
-    last decoder layer ([M, 64] x [64, 32], MN-major weight), and the weight gradient of the first layer (K = M)."""
-    M = C3["T"] * C3["B"] * 64 * 64
+    """The explicit GEMMs of the 3-channel ends at C3 size."""
+    run_end_gemms(K, C3["T"] * C3["B"] * 64 * 64)
+
+
+def run_end_gemms(K, M):
+    """The explicit GEMMs of the 3-channel ends over M pixels: the first encoder layer ([M, 32] x [64, 32] after im2col3) and
+    the last decoder layer ([M, 64] x [64, 32], MN-major weight), and the [64, 32] weight gradient with K = M that both the
+    first layer (dy^T col) and the last layer (x^T dcol, row pitch up8(27) = 32) launch."""
     torch.manual_seed(23)
     col = randn(M, 32)
     col[:, 27:] = 0
@@ -342,9 +370,13 @@ def misaligned_like(n, dtype):
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=["bf16", "f32"])
 def test_maxpool_c3(K, dtype):
-    """maxpool2_fwd / maxpool2_bwd on the 64x64x64 encoder map of C3 (N = 3840: 10^9 input elements), with planted ties:
-    equal pairs, four equal values, and -0 / +0.  The gradient goes to the first maximum in row-major order."""
-    N, H, C = C3_N, 64, 64
+    """maxpool2_fwd / maxpool2_bwd on the 64x64x64 encoder map of C3 (N = 3840: 10^9 input elements)."""
+    run_maxpool(K, C3_N, 64, 64, dtype, "C3")
+
+
+def run_maxpool(K, N, H, C, dtype, label):
+    """maxpool2_fwd / maxpool2_bwd on an N x H x H x C map with planted ties: equal pairs, four equal values, and -0 / +0.
+    The gradient goes to the first maximum in row-major order; the scalar paths equal the vector ones."""
     torch.manual_seed(26)
     x = randn(N, H, H, C, dtype=dtype)
     w = windows(x, N, H, H, C)
@@ -367,7 +399,7 @@ def test_maxpool_c3(K, dtype):
     K.maxpool2_bwd(x, dy, dx, N, H, H, C)
     dxs = misaligned_like(x.numel(), dtype).view_as(x)
     K.maxpool2_bwd(x, dy, dxs, N, H, H, C)
-    check_maxpool(x, y, dy, dx, N, H, H, C, f"C3 {dtype}")
+    check_maxpool(x, y, dy, dx, N, H, H, C, f"{label} {dtype}")
     for n0 in range(0, N, 256):
         sl = slice(n0, n0 + 256)
         assert torch.equal(ys[sl], y[sl]) and torch.equal(dxs[sl], dx[sl]), f"scalar and vector paths differ, images [{n0}, ..)"
@@ -379,15 +411,20 @@ def test_maxpool_c3(K, dtype):
 @pytest.mark.parametrize("dtype", DTYPES, ids=["bf16", "f32"])
 def test_upsample_c3(K, dtype):
     """upsample2_fwd / upsample2_bwd at the 64x64 decoder stage entry of C3 (32x32x64 -> 64x64x64 at N = 3840: 10^9 upsampled
-    elements): forward exact; backward bit for bit against torch's fp32 (a + b) + (c + d) and within one rounding of float64."""
-    N, H, C = C3_N, 32, 64
+    elements)."""
+    run_upsample(K, C3_N, 32, 64, dtype, "C3")
+
+
+def run_upsample(K, N, H, C, dtype, label):
+    """upsample2_fwd / upsample2_bwd from an N x H x H x C map: forward exact; backward bit for bit against torch's fp32
+    (a + b) + (c + d) and within one rounding of float64; the scalar paths equal the vector ones."""
     torch.manual_seed(27)
     x = randn(N, H, H, C, dtype=dtype)
     u = torch.empty(N, 2 * H, 2 * H, C, device="cuda", dtype=dtype)
     K.upsample2_fwd(x, u, N, H, H, C)
     us = misaligned_like(u.numel(), dtype).view_as(u)
     K.upsample2_fwd(x, us, N, H, H, C)
-    check_upsample_fwd(x, u, N, H, H, C, f"C3 {dtype}")
+    check_upsample_fwd(x, u, N, H, H, C, f"{label} {dtype}")
     for n0 in range(0, N, 256):
         assert torch.equal(us[n0:n0 + 256], u[n0:n0 + 256]), f"upsample2_fwd scalar and vector paths differ, images [{n0}, ..)"
     del us
@@ -396,7 +433,7 @@ def test_upsample_c3(K, dtype):
     K.upsample2_bwd(dy, dx, N, H, H, C)
     dxs = misaligned_like(dx.numel(), dtype).view_as(dx)
     K.upsample2_bwd(dy, dxs, N, H, H, C)
-    worst = check_upsample_bwd(dy, dx, N, H, H, C, f"C3 {dtype}")
+    worst = check_upsample_bwd(dy, dx, N, H, H, C, f"{label} {dtype}")
     for n0 in range(0, N, 256):
         assert torch.equal(dxs[n0:n0 + 256], dx[n0:n0 + 256]), f"upsample2_bwd scalar and vector paths differ, images [{n0}, ..)"
     print(f"[bound] upsample2 {dtype} N={N} {H}x{H}x{C}: fwd exact, bwd bit-exact, worst error/bound vs float64 {worst:.3g}")
@@ -406,9 +443,14 @@ def test_upsample_c3(K, dtype):
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=["bf16", "f32"])
 def test_im2col3_col2im3_c3(K, dtype):
-    """The 3-channel ends at C3 size (N = 3840 frames of 64x64x3): im2col3's row32 path (ld = 32) against the generic one
-    (ld = 40) and an exact statement for both tap signs, pad columns zero; col2im3 within 9 fp32 adds and one rounding."""
-    N, H, C = C3_N, 64, 3
+    """The 3-channel ends at C3 size (N = 3840 frames of 64x64x3)."""
+    run_im2col3_col2im3(K, C3_N, 64, dtype, "C3")
+
+
+def run_im2col3_col2im3(K, N, H, dtype, label):
+    """The 3-channel ends on N frames of H x H x 3: im2col3's row32 path (ld = 32) against the generic one (ld = 40) and an
+    exact statement for both tap signs, pad columns zero; col2im3 within 9 fp32 adds and one rounding."""
+    C = 3
     torch.manual_seed(28)
     x = randn(N, H, H, C, dtype=dtype)
     for sgn in (1, -1):
@@ -416,15 +458,15 @@ def test_im2col3_col2im3_c3(K, dtype):
         c40 = torch.full((N * H * H, 40), 7.0, device="cuda", dtype=dtype)
         K.im2col3(x, c32, N, H, H, C, 32, sgn)
         K.im2col3(x, c40, N, H, H, C, 40, sgn)
-        check_im2col3(x, c40, N, H, H, C, 40, sgn, f"C3 generic {dtype}")
-        check_im2col3(x, c32, N, H, H, C, 32, sgn, f"C3 row32 {dtype}")
+        check_im2col3(x, c40, N, H, H, C, 40, sgn, f"{label} generic {dtype}")
+        check_im2col3(x, c32, N, H, H, C, 32, sgn, f"{label} row32 {dtype}")
         del c32, c40
     ld = 32
     col = randn(N * H * H, ld, dtype=dtype)
     bias = randn(C, dtype=torch.float32)
     y = torch.full((N, H, H, C), NAN, device="cuda", dtype=dtype)
     K.col2im3(col, y, N, H, H, C, ld, bias=bias)
-    worst = check_col2im3(col, y, N, H, H, C, ld, bias, f"C3 {dtype}")
+    worst = check_col2im3(col, y, N, H, H, C, ld, bias, f"{label} {dtype}")
     print(f"[bound] im2col3 exact (row32 == generic), col2im3 {dtype}: worst error/bound {worst:.3g}")
     del x, col, y
     _release()
@@ -434,23 +476,29 @@ def test_im2col3_col2im3_c3(K, dtype):
 def test_skip_index_kernels_c3(K, dtype):
     """gather_add, group_sum and add_indexed at the engine's C3 sizes at 64x64x64 (groups of B = 128 images, G = 30 calls):
     n = 33.5M elements per group, 10^9 in all; three distinct skip sources."""
-    G, B, H, C, nsrc = C3["T"], C3["B"], 64, 64, 3
+    run_skip_index(K, C3["T"], C3["B"], 64, 64, dtype, gather=True)
+
+
+def run_skip_index(K, G, B, H, C, dtype, gather):
+    """(gather: gather_add,) group_sum and add_indexed over G groups of B images of H x H x C, three distinct skip sources."""
+    nsrc = 3
     n = B * H * H * C
     src = torch.tensor([(g + 1) % nsrc for g in range(G)], dtype=torch.int32, device="cuda")
     srcl = src.tolist()
     torch.manual_seed(29)
     big = randn(G * n, dtype=dtype)
-    small = randn(nsrc * n, dtype=torch.float32)
-    dst0 = big.clone()
-    # gather_add: dst[g] += src[grp_src[g]] (fp32 addend); a bf16 destination rounds twice (fp32, then bf16): one bf16 ulp
-    K.gather_add(big, small, src, G, n)
-    worst = 0.0
-    for g in range(G):
-        ref = dst0[g * n:(g + 1) * n].double() + small[srcl[g] * n:(srcl[g] + 1) * n].double()
-        rel = 2.0 ** -7 if dtype == torch.bfloat16 else 2.0 ** -23
-        worst = max(worst, bound_check(big[g * n:(g + 1) * n], ref, rel * ref.abs(), f"gather_add group {g}"))
-    print(f"[bound] gather_add {dtype} G={G} n={n}: worst error/bound {worst:.3g}")
-    del dst0, small
+    if gather:
+        small = randn(nsrc * n, dtype=torch.float32)
+        dst0 = big.clone()
+        # gather_add: dst[g] += src[grp_src[g]] (fp32 addend); a bf16 destination rounds twice (fp32, then bf16): one bf16 ulp
+        K.gather_add(big, small, src, G, n)
+        worst = 0.0
+        for g in range(G):
+            ref = dst0[g * n:(g + 1) * n].double() + small[srcl[g] * n:(srcl[g] + 1) * n].double()
+            rel = 2.0 ** -7 if dtype == torch.bfloat16 else 2.0 ** -23
+            worst = max(worst, bound_check(big[g * n:(g + 1) * n], ref, rel * ref.abs(), f"gather_add group {g}"))
+        print(f"[bound] gather_add {dtype} G={G} n={n}: worst error/bound {worst:.3g}")
+        del dst0, small
     # group_sum: out[f] = sum over the groups reading source f (fp32 in group order, one output rounding)
     out = torch.full((nsrc * n,), NAN, device="cuda", dtype=dtype)
     K.group_sum(big, out, src, G, nsrc, n)
@@ -682,22 +730,43 @@ def _make_audit_class():
     return AuditKernels
 
 
-def _step(kernels, optkw, T, B, np_seed):
+def vgg_step(kernels, optkw, T, B, np_seed, W0=64, use_graph=False):
+    """One bf16 vgg step (vgg_64 or vgg_128 by W0) from the seeded initial state: (plan, losses, gradients, engine).
+    use_graph: the step replayed from a captured CUDA graph, the engine restored in place to its initial state before the
+    replay."""
     from p2pvg_b200.engine_vgg import TrainEngineVGG
-    cfg = dict(g_dim=128, z_dim=10, rnn_size=256, channels=3, image_width=64, backbone="vgg", predictor_rnn_layers=2,
+    cfg = dict(g_dim=128, z_dim=10, rnn_size=256, channels=3, image_width=W0, backbone="vgg", predictor_rnn_layers=2,
                posterior_rnn_layers=1, prior_rnn_layers=1)
     state = O.build_state(cfg, seed=1)
     opt = O.default_opt(**optkw)
     opt["batch_size"] = B
     eng = TrainEngineVGG(state, cfg, opt, kernels, act_dtype=torch.bfloat16)
-    x = torch.rand(T, B, 3, 64, 64, generator=torch.Generator().manual_seed(5))
+    x = torch.rand(T, B, 3, W0, W0, generator=torch.Generator().manual_seed(5)).cuda()
     probs = np.random.RandomState(np_seed).uniform(0, 1, T - 1)
     plan = StepPlan(T, probs, opt)
-    eps = O.draw_eps(plan.S, B, 10, seed=11)
-    losses = eng.step(x.cuda(), probs=probs, eps=eps.cuda())
+    eps = O.draw_eps(plan.S, B, 10, seed=11).cuda()
+    if use_graph:
+        from tests.test_measured_gpu import restore, snapshot
+        snap = snapshot(eng)
+        for _ in range(2):   # eager warm-up, then capture
+            eng.step(x, probs=probs, eps=eps, use_graph=True)
+        restore(eng, snap)
+        del snap
+        losses = eng.step(x, probs=probs, eps=eps, use_graph=True)
+        assert any(v != "warm" for v in eng._graphs.values()), "the step was not graph-replayed"
+    else:
+        losses = eng.step(x, probs=probs, eps=eps)
     torch.cuda.synchronize()
     grads = {m: {k: v.detach().clone() for k, v in eng.arena[m].g.items()} for m in eng.arena}
     return plan, np.asarray(losses), grads, eng
+
+
+def assert_equal_steps(a, b, what):
+    """(losses, gradients) of two steps are equal bit for bit."""
+    assert np.array_equal(a[0], b[0]), f"{what}: losses {a[0]} vs {b[0]}"
+    for m in a[1]:
+        for k in a[1][m]:
+            assert torch.equal(a[1][m][k], b[1][m][k]), f"{what}: grad {m}.{k} differs"
 
 
 def _skip_seed(T):
@@ -715,25 +784,30 @@ AUDIT_CASES = [("bench_options", BENCH_OPT, None), ("skip_lfs", dict(skip_prob=0
 
 @pytest.mark.parametrize("case", AUDIT_CASES, ids=[c[0] for c in AUDIT_CASES])
 def test_audit_vgg_step(K, case):
-    """One eager bf16 vgg_64 step at T = 30, B = 32 with every launch checked as it runs; every path of the launch list must
-    occur, and the audited step must equal (torch.equal) the same step on plain CudaKernels."""
-    from p2pvg_b200._lib import CudaKernels
+    """One eager bf16 vgg_64 step at T = 30, B = 32 with every launch checked as it runs."""
     name, optkw, seed = case
-    T, B = 30, 32
+    audit_step(name, optkw, 30, 32, seed, W0=64)
+
+
+def audit_step(name, optkw, T, B, seed, W0):
+    """One eager bf16 vgg step with every launch checked as it runs; every path of the launch list must occur, every skip
+    addend must be read through the plan's skip sources, and the audited step must equal (torch.equal) the same step on plain
+    CudaKernels.  seed "search": _skip_seed.  Returns the plain step's (losses, gradients)."""
+    from p2pvg_b200._lib import CudaKernels
     seed = _skip_seed(T) if seed == "search" else 0
-    plan, losses, grads, eng = _step(CudaKernels("cuda"), optkw, T, B, seed)
+    plan, losses, grads, eng = vgg_step(CudaKernels("cuda"), optkw, T, B, seed, W0)
     del eng
     _release()
     if name == "skip_lfs":
         assert len(set(plan.skip_src)) >= 3
     audit = _make_audit_class()("cuda")
-    plan_a, losses_a, grads_a, eng = _step(audit, optkw, T, B, seed)
+    plan_a, losses_a, grads_a, eng = vgg_step(audit, optkw, T, B, seed, W0)
     log, seen, skip_reads = eng.K.log, eng.K.seen, eng.K.skip_reads
     del eng
     _release()
     # coverage: every variant of the derived launch list (and every wrapped data-movement kernel) occurred
     want = set()
-    for L in forward_launches(T, B, plan.S, plan.nskip) + backward_launches(T, B, plan.S, plan.nskip):
+    for L in forward_launches(T, B, plan.S, plan.nskip, W0) + backward_launches(T, B, plan.S, plan.nskip, W0, plan.has_cpc):
         if L["kind"] == 4:
             want.add(variant(4, 0, L["Cn"], False, None, torch.float32, swap=conv_tiles(4, L["N"], L["H"], L["H"], 0, L["Cn"], L["Cm"], sm_count()).swap))
         else:
@@ -747,12 +821,10 @@ def test_audit_vgg_step(K, case):
     assert not missing, f"launch variants that did not occur in the step: {sorted(missing)}"
     assert any(v[0] == "gemm" for v in seen)
     # every decoder stage entry reads, for decoder call s, the skip frame the reference's schedule names (models/p2p_model.py)
-    assert len(skip_reads) == sum(1 for L in forward_launches(T, B, plan.S, plan.nskip) if L["addend"])
+    assert len(skip_reads) == sum(1 for L in forward_launches(T, B, plan.S, plan.nskip, W0) if L["addend"])
     for r in skip_reads:
         assert r == plan.skip_src, f"skip addend read through {r}, the schedule says {plan.skip_src}"
-    print(f"[audit] {name}: {len(log)} launches checked, worst error/bound {max(w for _, _, w in log):.3g}")
+    print(f"[audit] {name} {W0}x{W0}: {len(log)} launches checked, worst error/bound {max(w for _, _, w in log):.3g}")
     # the audit does not perturb the step
-    assert np.array_equal(losses, losses_a), (losses, losses_a)
-    for m in grads:
-        for k in grads[m]:
-            assert torch.equal(grads[m][k], grads_a[m][k]), f"grad {m}.{k} differs under the audit"
+    assert_equal_steps((losses, grads), (losses_a, grads_a), f"{name}: the audited step")
+    return losses, grads

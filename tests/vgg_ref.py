@@ -1,8 +1,9 @@
-"""The vgg_64 training step's kernel launches, derived from the engine's layer tables, and the float64 statements the launch
-tests check them against (tests/test_vgg_launches_gpu.py).
+"""The vgg_64 and vgg_128 training steps' kernel launches, derived from the engine's layer tables, and the float64 statements
+the launch tests check them against (tests/test_vgg_launches_gpu.py, tests/test_vgg128_launches_gpu.py).
 
-`forward_launches` / `backward_launches` walk VGG_ENC / VGG_DEC the way TrainEngineVGG.encode / decode / *_backward do and
-ask the engine's own rules (implicit_shape, TrainEngine.stat_buf with BN_FUSE_MIN) which launches take the implicit GEMM,
+`forward_launches` / `backward_launches` walk the backbone's layer tables (VGG_ENC / VGG_DEC for 64x64 frames, VGG_ENC_128 /
+VGG_DEC_128 for 128x128) the way TrainEngineVGG.encode / decode / decoder_backward / encoder_backward do and ask the engine's
+own rules (implicit_shape, TrainEngine.stat_buf with BN_FUSE_MIN) which launches take the implicit GEMM,
 which get fused BatchNorm statistics and which carry the skip addend, so the list follows the engine when it changes.
 
 The checkers work in image chunks so that float64 references of C3-sized tensors (up to 10^9 elements) stay a few GiB:
@@ -17,7 +18,7 @@ import torch
 import torch.nn.functional as F
 
 from p2pvg_b200.engine import TrainEngine
-from p2pvg_b200.engine_vgg import VGG_DEC, VGG_ENC
+from p2pvg_b200.engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128
 from p2pvg_b200.layouts import implicit_shape
 from tests.tc_schedule import BETA, alpha_for, assert_within, cdiv
 from tests.test_tc_schedule_gpu import rows_by_tile
@@ -33,11 +34,19 @@ def _stat_rule(M, C, rows_per_group, kred):
     return TrainEngine.stat_buf(stub, "", M, 1, C, rows_per_group, kred=kred)
 
 
+def vgg_tables(W0):
+    """(encoder, decoder) layer tables of the vgg backbone for W0 x W0 frames, as TrainEngineVGG.__init__ picks them."""
+    if W0 not in (64, 128):
+        raise ValueError(f"no vgg backbone for {W0}x{W0} frames")
+    return (VGG_ENC_128, VGG_DEC_128) if W0 == 128 else (VGG_ENC, VGG_DEC)
+
+
 def forward_launches(T, B, S, nskip, W0=64):
-    """Every implicit-GEMM forward convolution of one bf16 vgg_64 step (encode, then decode), in engine order."""
+    """Every implicit-GEMM forward convolution of one bf16 vgg step (encode, then decode), in engine order."""
+    ENC, DEC = vgg_tables(W0)
     out = []
     N, H, C = T * B, W0, None
-    for i, stage in enumerate(VGG_ENC):
+    for i, stage in enumerate(ENC):
         for j, (cin, cout) in enumerate(stage):
             if j == 0 and i > 0:
                 H //= 2
@@ -45,7 +54,7 @@ def forward_launches(T, B, S, nskip, W0=64):
                 st = _stat_rule(N * H * H, cout, B * H * H, 9 * cin)
                 out.append(dict(name=f"enc{i}.{j}", kind=3, N=N, H=H, Ck=cin, Cn=cout, bias=True, addend=False, ipg=0, stat=st, B=B))
     N, H = (S + 1) * B, 4
-    for k, stage in enumerate(VGG_DEC):
+    for k, stage in enumerate(DEC):
         for j, (cin, cout) in enumerate(stage):
             if j == 0:
                 H *= 2
@@ -62,14 +71,71 @@ def forward_launches(T, B, S, nskip, W0=64):
     return out
 
 
-def backward_launches(T, B, S, nskip, W0=64):
-    """The data-gradient (kind 5) and weight-gradient (kind 4) launches that mirror each implicit forward launch."""
+def _dgrad(name, N, H, cout, cin, B):
+    return dict(name=name + " dgrad", kind=5, N=N, H=H, Ck=cout, Cn=cin, bias=False, addend=False, ipg=0, stat=None, B=B)
+
+
+def _wgrad(name, N, H, cout, cin):
+    return dict(name=name + " wgrad", kind=4, N=N, H=H, Cm=cout, Cn=cin)
+
+
+def _decoder_backward(out, DEC, N, B, nskip, want_wgrad, want_skip, tag):
+    """TrainEngineVGG.decoder_backward over N = (g1 - g0) B images: stages last to first, layers in reverse; a stage entry's
+    upsampled half at N, its skip half (want_skip) over the nskip B skip images the group_sum of its output gradient feeds."""
+    for k in range(len(DEC) - 1, -1, -1):
+        H = 8 << k
+        for j in range(len(DEC[k]) - 1, -1, -1):
+            cin, cout = DEC[k][j]
+            if j == 0:
+                C = cin // 2
+                if implicit_shape(cout, C):
+                    out.append(_dgrad(f"{tag}dec{k}.0.D", N, H, cout, C, B))
+                if want_wgrad and implicit_shape(C, cout):
+                    out.append(_wgrad(f"{tag}dec{k}.0.D", N, H, cout, C))
+                if want_skip:
+                    if implicit_shape(cout, C):
+                        out.append(_dgrad(f"{tag}dec{k}.0.S", nskip * B, H, cout, C, B))
+                    if want_wgrad and implicit_shape(C, cout):
+                        out.append(_wgrad(f"{tag}dec{k}.0.S", nskip * B, H, cout, C))
+            else:
+                if implicit_shape(cout, cin):
+                    out.append(_dgrad(f"{tag}dec{k}.{j}", N, H, cout, cin, B))
+                if want_wgrad and implicit_shape(cin, cout):
+                    out.append(_wgrad(f"{tag}dec{k}.{j}", N, H, cout, cin))
+
+
+def backward_launches(T, B, S, nskip, W0=64, has_cpc=True):
+    """The data-gradient (kind 5) and weight-gradient (kind 4) launches of one bf16 vgg step, in the order the step enqueues
+    them (engine.py TrainEngine.phases, mode A): backward_decoder's decoder_backward(0, S) with weight and skip gradients over
+    the S B reconstruction images (engine.py:1236), the CPC decode's decoder_backward(S, S + 1) with data gradients only over
+    B images (backward_prior, :1355), then encoder_backward over all T B frames, where the first layer (3 input channels) has
+    an explicit weight gradient and no data gradient."""
+    ENC, DEC = vgg_tables(W0)
     out = []
-    for f in forward_launches(T, B, S, nskip, W0):
-        N, H, ci, co = f["N"], f["H"], f["Ck"], f["Cn"]
-        out.append(dict(name=f["name"] + " dgrad", kind=5, N=N, H=H, Ck=co, Cn=ci, bias=False, addend=False, ipg=0, stat=None, B=B))
-        out.append(dict(name=f["name"] + " wgrad", kind=4, N=N, H=H, Cm=co, Cn=ci))
+    _decoder_backward(out, DEC, S * B, B, nskip, True, True, "")
+    if has_cpc:
+        _decoder_backward(out, DEC, B, B, nskip, False, False, "cpc ")
+    N = T * B
+    for i in range(len(ENC) - 1, -1, -1):
+        H = W0 >> i
+        for j in range(len(ENC[i]) - 1, -1, -1):
+            cin, cout = ENC[i][j]
+            if cin is None:
+                continue
+            if implicit_shape(cin, cout):
+                out.append(_wgrad(f"enc{i}.{j}", N, H, cout, cin))
+            if implicit_shape(cout, cin):
+                out.append(_dgrad(f"enc{i}.{j}", N, H, cout, cin, B))
     return out
+
+
+def launch_key(L):
+    """What a conv_gemm launch is, as the launch-list test compares it: kind, N, H, Ck, Cn, Cm, bias, addend dtype (the bf16
+    skip half), images per group, fused statistics."""
+    if L["kind"] == 4:
+        return (4, L["N"], L["H"], 0, L["Cn"], L["Cm"], False, None, 0, False)
+    return (L["kind"], L["N"], L["H"], L["Ck"], L["Cn"], 0, L["bias"], torch.bfloat16 if L["addend"] else None, L["ipg"],
+            L["stat"] is not None)
 
 
 def row_cooperative(c_dtype, stat, accumulate, addend_dtype):
