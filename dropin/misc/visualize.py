@@ -1,6 +1,6 @@
 """Drop-in for the reference's ``misc/visualize.py``: ``vis_seq`` runs ``p2pvg_b200.visualize.vis_seq`` (only the displayed
 rows generated, all samples in one CUDA-graph replay, the pictures composed in one launch, the PNG file encoded on the GPU by
-``p2pvg_b200.png.save_image``) whenever
+``p2pvg_b200.png.save_image`` and the GIF file by ``p2pvg_b200.gif.save_gif``) whenever
 ``p2pvg_b200.visualize.check_vis_seq`` accepts the call, and the reference's own ``vis_seq`` otherwise.  Every other name
 (``add_gt_cp_border``, ``add_samples_cp_border``, ``save_utils``, ...) is the reference's, from its module loaded from the
 reference's ``misc/`` directory."""
@@ -8,6 +8,7 @@ import importlib.util
 import os
 
 import misc as _pkg
+from p2pvg_b200 import gif as _gif
 from p2pvg_b200 import png as _png
 from p2pvg_b200 import visualize as _fast
 
@@ -45,4 +46,5 @@ def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, ski
         return _reference().vis_seq(model, x, epoch, output_len, model_mode=model_mode, recon_mode=recon_mode,
                                     skip_frame=skip_frame, h36m_visualizer=h36m_visualizer, writer=writer, opt=opt)
     _fast.vis_seq(model, x, epoch, output_len, model_mode=model_mode, recon_mode=recon_mode, skip_frame=skip_frame,
-                  h36m_visualizer=h36m_visualizer, writer=writer, opt=opt, save_png=_png.save_image)
+                  h36m_visualizer=h36m_visualizer, writer=writer, opt=opt, save_png=_png.save_image,
+                  save_gif=_gif.save_gif)

@@ -595,6 +595,38 @@ size_t p2pvg_png_out_bytes(const int64_t* images, int n);
 int p2pvg_png_encode(const int64_t* images, int n, int rule, void* workspace, size_t ws_bytes, uint8_t* out, size_t out_bytes,
                      int64_t* files, void* stream);
 
+/* GIF89a animations of n frame sequences in one call, every per-pixel stage on the device: quantisation, each frame's
+ * colour set and palette, the index map, LZW in independent segments of P2PVG_GIF_SEGMENT pixels, the bit packing, the
+ * data sub-blocks and the packing of every file into one buffer.
+ *   anims      [n][7] int64, HOST memory: per animation the device address of contiguous frames -- P2PVG_PNG_U8
+ *              [T][H][W][3] or P2PVG_F32 [T][3][H][W] (4-byte aligned) --, T, H and W (1..65535 each), the delay of every
+ *              frame in centiseconds and the NETSCAPE2.0 loop count (0: forever; 0..65535 each)
+ *   rule       the quantisation of fp32 frames, as p2pvg_png_encode's (P2PVG_PNG_SAVE_IMAGE or P2PVG_PNG_TENSORBOARD)
+ *   workspace  p2pvg_gif_workspace_bytes(anims, n) bytes, 256-byte aligned
+ *   out        at least p2pvg_gif_out_bytes(anims, n) bytes: the files, back to back in animation order
+ *   files      [n][2] int64 (8-byte aligned): offset in out and size of each file
+ * A file: the header and a logical screen descriptor without a global colour table, a NETSCAPE2.0 loop block, per frame a
+ * graphic control extension (the delay, no transparency), an image descriptor of the whole frame with a local table of 256
+ * entries, LZW minimum code size 8 and the data sub-blocks; then the trailer.  The palette: a frame of at most 256 distinct
+ * colours lists exactly those, sorted by 24-bit key (0xRRGGBB), and is lossless; otherwise median cut (split the box of
+ * largest count-weighted squared error along its widest channel at the count-weighted median) to 256 boxes, their rounded
+ * means, then 3 Lloyd iterations over the distinct colours.  Each pixel takes its nearest entry (squared RGB distance,
+ * lowest index on ties).  LZW: each segment starts from the post-clear state and ends with a CLEAR at its final code width
+ * (the frame's last with an EOI); the stream opens with a CLEAR; a table of 4096 codes emits a CLEAR at 12 bits.  The bytes
+ * of a file depend on its frames, rule, delay and loop alone, not on the other animations of the call.
+ * n == 0 returns P2PVG_OK without a launch.  P2PVG_ERR_BAD_ARG: a malformed table row, rule or pointer;
+ * P2PVG_ERR_UNSUPPORTED: 2^40 pixels or 2^24 frames in all or more; P2PVG_ERR_WORKSPACE: workspace or out too small.
+ * The size queries return 0 for a table the encoder rejects. */
+#define P2PVG_GIF_SEGMENT 65536
+size_t p2pvg_gif_workspace_bytes(const int64_t* anims, int n);
+size_t p2pvg_gif_out_bytes(const int64_t* anims, int n);
+int p2pvg_gif_encode(const int64_t* anims, int n, int rule, void* workspace, size_t ws_bytes, uint8_t* out, size_t out_bytes,
+                     int64_t* files, void* stream);
+
+/* CRC-32C (Castagnoli) of n host bytes, continuing from crc (0 to start): crc32c(a + b) = p2pvg_crc32c(b, crc32c(a)).
+ * Host code (no device, no stream); data may be NULL when n == 0. */
+uint32_t p2pvg_crc32c(const void* data, size_t n, uint32_t crc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -37,6 +37,10 @@ def load_library():
         _lib.p2pvg_histograms_workspace_bytes.restype = ctypes.c_size_t
         _lib.p2pvg_png_workspace_bytes.restype = ctypes.c_size_t
         _lib.p2pvg_png_out_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_gif_workspace_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_gif_out_bytes.restype = ctypes.c_size_t
+        _lib.p2pvg_crc32c.restype = ctypes.c_uint32
+        _lib.p2pvg_crc32c.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_uint32]
     return _lib
 
 
@@ -561,3 +565,22 @@ class CudaKernels:
         the uint8 device buffer out, with their (offset, size) in the int64 device tensor files [n, 2]."""
         self._ck(self.lib.p2pvg_png_encode(_vp(images_host.ctypes.data), _i(len(images_host)), _i(rule), _p(workspace),
                                            _sz(workspace.numel()), _p(out), _sz(out.numel()), _p(files), self._stream()))
+
+    # -- GIF files -----------------------------------------------------------------------------
+    def gif_bytes(self, anims_host):
+        """(workspace bytes, output bytes) p2pvg_gif_encode needs for the int64 host animation table anims_host [n, 7]
+        (address, dtype, T, H, W, delay, loop); (0, 0) for a table it rejects."""
+        ptr, n = _vp(anims_host.ctypes.data), _i(len(anims_host))
+        return int(self.lib.p2pvg_gif_workspace_bytes(ptr, n)), int(self.lib.p2pvg_gif_out_bytes(ptr, n))
+
+    def gif_encode(self, anims_host, rule, workspace, out, files):
+        """p2pvg_gif_encode: the GIF files of the animations of anims_host (checked by the library before any launch) packed
+        into the uint8 device buffer out, with their (offset, size) in the int64 device tensor files [n, 2]."""
+        self._ck(self.lib.p2pvg_gif_encode(_vp(anims_host.ctypes.data), _i(len(anims_host)), _i(rule), _p(workspace),
+                                           _sz(workspace.numel()), _p(out), _sz(out.numel()), _p(files), self._stream()))
+
+
+def crc32c(data, crc=0):
+    """p2pvg_crc32c: the CRC-32C of the bytes ``data``, continuing from ``crc``.  Host code: needs the library, no device."""
+    data = bytes(data)
+    return int(load_library().p2pvg_crc32c(data, len(data), crc))

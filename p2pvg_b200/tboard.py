@@ -14,6 +14,10 @@ event records.
   default (or an explicit) edge table; ``dropin/tensorboardX`` puts it under ``train.py``'s ``SummaryWriter``.
 - ``add_image_gpu(writer, ...)``: ``add_image`` of a 3-channel float32 / uint8 image with the PNG encoded on the GPU
   (``p2pvg_b200.png``); ``dropin/tensorboardX``'s ``SummaryWriter.add_image`` takes it first.
+- ``add_video_gpu(writer, ...)``: ``add_video`` of one 3-channel float32 / uint8 video with the GIF encoded on the GPU
+  (``p2pvg_b200.gif``); ``dropin/tensorboardX``'s ``SummaryWriter.add_video`` takes it first.
+- ``native_record_crc(file_writer)``: the file writer's event records framed with the library's CRC-32C instead of
+  TensorBoard's pure-Python one; the same bytes.
 
 The one visible difference from the host computation: sum and sum_squares are fp64 sums in another order (fixed-size
 chunks of each tensor), so they agree with ``values.sum()`` / ``values.dot(values)`` to rounding, not bit for bit.
@@ -21,10 +25,12 @@ Buckets, limits, num, min and max are exact.
 """
 from __future__ import annotations
 
+import struct
+
 import numpy as np
 import torch
 
-from ._lib import F32, kernels_for
+from ._lib import F32, crc32c, kernels_for
 
 F64 = 2           # P2PVG_F64
 MAX_EDGES = 4096  # the largest edge table p2pvg_histograms takes
@@ -253,6 +259,91 @@ def add_image_gpu(writer, tag, img_tensor, global_step=None, walltime=None, data
     image = Summary.Image(height=int(t.shape[1]), width=int(t.shape[2]), colorspace=3, encoded_image_string=data)
     writer._get_file_writer().add_summary(Summary(value=[Summary.Value(tag=tag, image=image)]), global_step, walltime)
     return True
+
+
+def _gpu_video(vid):
+    """vid as a CUDA [T, 3, H, W] float32 / uint8 tensor when the GPU video path takes it (one video of 3 channels, sides
+    in 1..65535, no NaN), else None."""
+    from .gif import MAX_SIDE
+    if not torch.cuda.is_available():
+        return None
+    if isinstance(vid, np.ndarray):
+        if vid.dtype not in (np.float32, np.uint8):
+            return None
+        t = torch.from_numpy(np.ascontiguousarray(vid))
+    elif torch.is_tensor(vid):
+        t = vid.detach()
+    else:
+        return None
+    if t.dtype not in (torch.float32, torch.uint8) or t.dim() != 5 or t.shape[0] != 1 or t.shape[2] != 3:
+        return None
+    if not all(1 <= int(v) <= MAX_SIDE for v in (t.shape[1], t.shape[3], t.shape[4])):
+        return None
+    if t.device.type != "cuda":
+        if t.device.type != "cpu":
+            return None
+        t = t.to("cuda")
+    t = t[0]
+    if t.dtype == torch.float32 and bool(torch.isnan(t).any()):
+        return None
+    return t
+
+
+def add_video_gpu(writer, tag, vid_tensor, global_step=None, fps=4, walltime=None):
+    """``writer.add_video`` of one video (N = 1) of 3 channels, float32 or uint8, a NumPy array or a tensor [1, T, 3, H, W],
+    with the GIF encoded on the GPU, when a CUDA device exists: the base writer's quantisation (float32: x * 255 clipped to
+    [0, 255] and truncated; uint8 as it is), every frame shown round(100 / fps) centiseconds, looping forever (moviepy's
+    ``write_gif`` defaults), and the base writer's ``Summary.Image`` record (tag, step, height, width, colorspace 3),
+    written through ``writer._get_file_writer()``.  A frame of at most 256 colours decodes to the quantised pixels; others
+    carry a 256-colour palette (``p2pvg_b200.gif``).  Returns False, having written nothing, for any other call, for float
+    input with NaN and for an fps whose delay does not fit the GIF field."""
+    from . import gif
+    try:
+        delay = round(100 / fps)
+    except (TypeError, ZeroDivisionError):
+        return False
+    if not 0 <= delay <= gif.MAX_SIDE:
+        return False
+    t = _gpu_video(vid_tensor)
+    if t is None:
+        return False
+    frames = t.contiguous() if t.dtype == torch.float32 else t.permute(0, 2, 3, 1).contiguous()
+    data, = gif.encode_gif([frames], "tensorboard", delay_cs=int(delay), loop=0)
+    Summary = _summary_class(writer)
+    image = Summary.Image(height=int(t.shape[2]), width=int(t.shape[3]), colorspace=3, encoded_image_string=data)
+    writer._get_file_writer().add_summary(Summary(value=[Summary.Value(tag=tag, image=image)]), global_step, walltime)
+    return True
+
+
+def masked_crc32c(data):
+    """TensorBoard's masked CRC-32C of the bytes ``data``, with the library's CRC-32C."""
+    x = crc32c(data)
+    return (((x >> 15) | (x << 17)) + 0xa282ead8) & 0xffffffff
+
+
+def _record_writer(file_writer):
+    """The RecordWriter under a torch.utils.tensorboard / tensorboard file writer (event_writer._async_writer._writer), or
+    None for any other layout."""
+    rw = getattr(getattr(getattr(file_writer, "event_writer", None), "_async_writer", None), "_writer", None)
+    if rw is None or type(rw).__name__ != "RecordWriter" or not hasattr(rw, "_writer"):
+        return None
+    return rw
+
+
+def native_record_crc(file_writer):
+    """Frame the file writer's event records with ``masked_crc32c`` above: its RecordWriter instance's ``write`` becomes one
+    that writes the same bytes (length, masked CRC of the length, the record, masked CRC of the record).  The module-level
+    ``masked_crc32c`` of tensorboard and every other writer stay as they are; a writer of another layout is left alone."""
+    rw = _record_writer(file_writer)
+    if rw is None or "write" in vars(rw):
+        return
+    out = rw._writer
+
+    def write(data):
+        header = struct.pack("<Q", len(data))
+        out.write(header + struct.pack("<I", masked_crc32c(header)) + data + struct.pack("<I", masked_crc32c(data)))
+
+    rw.write = write
 
 
 def _summary_class(writer):

@@ -201,14 +201,15 @@ def _render(vis, poses, camera_view, nb):
 
 
 def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, skip_frame=True, h36m_visualizer=None, writer=None,
-            opt=None, save_png=None):
+            opt=None, save_png=None, save_gif=None):
     """misc/visualize.py vis_seq (same arguments, files and TensorBoard entries) on the graphed generator and one
     p2pvg_vis_canvas launch; see the module docstring.  ``save_png(canvas, file_name)`` writes the PNG file
-    (torchvision.utils.save_image when None; p2pvg_b200.png.save_image encodes it on the GPU).  ValueError before any draw
+    (torchvision.utils.save_image when None; p2pvg_b200.png.save_image encodes it on the GPU).  ``save_gif(file_name,
+    gif)`` writes the GIF file from the device's uint8 frames (imageio.mimsave of their host copy when None;
+    p2pvg_b200.gif.save_gif encodes it on the GPU).  ValueError before any draw
     or launch when check_vis_seq rejects the arguments.  Returns (canvas, video, gif) on the device."""
     opt = model.opt if opt is None else opt
     check_vis_seq(model, x, output_len, model_mode, skip_frame, opt)
-    import imageio
     import torchvision.utils as vutils
     nsample, nb, L = int(opt.nsample), n_block_of(opt), int(output_len)
     pose = opt.dataset == "h36m"
@@ -257,7 +258,11 @@ def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, ski
             canvas, video, gif = compose(store0, samples, tiles, int(frames.shape[2]), int(frames.shape[3]))
     png_name, gif_name = file_names(opt, epoch, output_len, model_mode, recon_mode)
     (vutils.save_image if save_png is None else save_png)(canvas, png_name)
-    imageio.mimsave(gif_name, list(gif.cpu().numpy()))
+    if save_gif is None:
+        import imageio
+        imageio.mimsave(gif_name, list(gif.cpu().numpy()))
+    else:
+        save_gif(gif_name, gif)
     img_tag, vid_tag = tags(output_len, model_mode, recon_mode)
     writer.add_image(img_tag, canvas.cpu().numpy(), epoch)
     writer.add_video(vid_tag, video.unsqueeze(0).cpu().numpy(), epoch, fps=2)
