@@ -13,7 +13,7 @@ when it changes.  Each entry is a dict with `op`:
     weight gradient).
 `key(L)` is what a recording of the step is compared on.
 
-The float64 checkers work in image chunks (vgg_ref.CHUNK elements) so that references of C2-sized tensors stay a few GiB.
+The float64 checkers work in image chunks (ref64.CHUNK elements) so that references of C2-sized tensors stay a few GiB.
 """
 import types
 
@@ -22,9 +22,9 @@ import torch.nn.functional as F
 
 from p2pvg_b200.engine import BN_FUSE_MIN, TrainEngine
 from p2pvg_b200.layouts import implicit_shape
-from tests.tc_schedule import BETA, alpha_for, box_for, cdiv, conv_ref64
-from tests.test_tc_schedule_gpu import rows_by_tile
-from tests.vgg_ref import A_STAT, CHUNK, assert_within, row_cooperative
+from tests.ref64 import A_STAT, CHUNK
+from tests.tc_schedule import BETA, alpha_for, assert_within, box_for, cdiv, conv_ref64, rows_by_tile
+from tests.vgg_ref import row_cooperative
 
 ACT_LRELU, ACT_TANH = 1, 2
 G_DIM = 128
@@ -372,33 +372,6 @@ def wgrad4_ref64(a, b, N, H, Cm, Cn):
 
 
 # ------------------------------------------------------------------ BatchNorm, group by group
-
-EPS = 1e-5
-
-
-def bn_group_ref64(x, dy, gamma, beta, act, side=None, y=None):
-    """Float64 training-mode BatchNorm of one group x [R, C] followed by `act`: statistics, dz = dy * act'(pre), and
-    dx = gamma invstd (dz - mean dz - xhat mean(dz xhat)) with its magnitude.  LeakyReLU: `side` is the slope side the kernel
-    uses (sign of its fp32 fmaf); tanh: 1 - y^2 of the stored y."""
-    x = x.double()
-    R = x.shape[0]
-    m = x.mean(0)
-    v = ((x - m) ** 2).mean(0)
-    inv = 1.0 / torch.sqrt(v + EPS)
-    xh = (x - m) * inv
-    if dy is None:
-        return dict(mean=m, var=v, invstd=inv, xhat=xh)
-    if act == ACT_LRELU:
-        dz = dy.double() * torch.where(side, 1.0, 0.2)
-    else:
-        dz = dy.double() * (1 - y.double() ** 2)
-    sdz, sdzx = dz.sum(0), (dz * xh).sum(0)
-    k0 = gamma.double() * inv
-    dx = k0 * (dz - sdz / R - xh * sdzx / R)
-    mag = k0.abs() * (dz.abs() + (dz.abs().sum(0) + xh.abs() * (dz * xh).abs().sum(0)) / R)
-    return dict(mean=m, var=v, invstd=inv, dz=dz, sdz=sdz, sdzx=sdzx, dx=dx, dx_mag=mag, sdz_mag=dz.abs().sum(0),
-                sdzx_mag=(dz * xh).abs().sum(0))
-
 
 BN_MAXCHUNK = 64
 

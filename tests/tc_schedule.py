@@ -1,5 +1,5 @@
 """Host-side launch decisions of the persistent tensor-core kernels, mirrored in Python, plus the float64 references and the
-error bound the multi-round tests share (tests/test_tc_schedule_gpu.py).
+error bound the multi-round tests (tests/test_tc_schedule_gpu.py) and the launch tests share.
 
 The persistent kernels (gemm_tc.cu, conv_gemm.cu) launch grid = min(tiles, SMs) CTAs and every CTA walks the tiles
 t = blockIdx.x, blockIdx.x + gridDim.x, ...  `gemm_tc_tiles` and `conv_tiles` transcribe the launchers' choices (tile width,
@@ -87,6 +87,18 @@ def assert_multi_round(s, need_n_change=True, min_tiles=None):
         assert s.tiles_n > 1 and s.n0_changes(), f"tiles_n={s.tiles_n} on {s.sms} SMs: every CTA keeps one n0"
 
 
+def fit(cands, sched, need_n_change=True, min_tiles=None):
+    """The first candidate shape whose schedule meets the multi-round invariants (fails loudly if none does)."""
+    for shape in cands:
+        s = sched(*shape)
+        try:
+            assert_multi_round(s, need_n_change, min_tiles)
+        except AssertionError:
+            continue
+        return shape, s
+    raise AssertionError("no candidate shape reaches the rounds this case is meant to test on this device")
+
+
 def gemm_tc_tiles(M, N, K, sms, tf32=False, ws_bytes=GEMM_WS_BYTES):
     """p2pvg_gemm_tc (gemm_tc.cu:214-241) and p2pvg_gemm_tf32 (gemm_tc.cu:190-198); grid: launch() (gemm_tc.cu:157) and
     launch_persistent() (tc_common.cuh:429-430)."""
@@ -170,6 +182,31 @@ def conv_tiles(kind, N, H, W, Ck, Cn, Cm, sms, ws_bytes=GEMM_WS_BYTES, bres_enab
     tm, tn = cdiv(M, BLOCK_M), cdiv(Ntot, BN)
     total = tm * tn * splits
     return Schedule(total, splits, 1, BN, tm, tn, min(total, sms), sms, kbps, swap=swap)
+
+
+def image_slices(N, HW, unit, s, sms):
+    """Three tile-aligned image ranges (first, middle, last round) whose launch has at most `sms` tiles."""
+    tiles_per_img = lambda n: cdiv(n * HW, s.BM) * s.tiles_n * s.phases
+    ni = unit
+    while ni + unit <= N and tiles_per_img(ni + unit) <= sms:
+        ni += unit
+    mid = (N // 2) // unit * unit
+    last = -(-(N - ni) // unit) * unit
+    return [(0, ni), (mid, min(N, mid + ni)), (last, N)]
+
+
+def rows_by_tile(out, kind, N, H, Cn, tiles_m):
+    """The stored output as [tiles_m * phases, 128, Cn] float64: the rows each statistics partial row covers (rows past the
+    end are zeros).  Kind 2: partial row (mt, ph) covers phase ph's output pixels of the small-map pixels of tile mt."""
+    o = out.double()
+    if kind == 2:
+        o = o.view(N, H, 2, H, 2, Cn).permute(2, 4, 0, 1, 3, 5).reshape(4, N * H * H, Cn)
+    else:
+        o = o.reshape(1, N * H * H, Cn)
+    P = o.shape[0]
+    pad = torch.zeros(P, tiles_m * 128, Cn, dtype=torch.float64, device=o.device)
+    pad[:, :o.shape[1]] = o
+    return pad.view(P, tiles_m, 128, Cn).transpose(0, 1).reshape(tiles_m * P, 128, Cn)
 
 
 # ------------------------------------------------------------------ float64 references on the kernels' own (bf16-rounded) operands

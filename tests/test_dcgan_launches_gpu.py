@@ -20,51 +20,26 @@
      every conv_gemm variant of the derived list, the skip addends read through plan.skip_src, and a step bit-identical to
      the same step on plain CudaKernels with its concurrent lanes.
 """
-import inspect
 import math
-import time
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import p2p_oracle as O
-from p2pvg_b200.engine import StepPlan
-from tests.dcgan_ref import (ACT_LRELU, ACT_TANH, EPS, bn_group_ref64, check_conv4_sums, check_stat_rows, check_wgrad_c1, conv4_ref64_elem,
-                             conv_variant, forward_launches, key, step_launches, wgrad4_ref64, wgrad_c1_ref64)
+from p2pvg_b200.engine import StepPlan, TrainEngine
+from tests.dcgan_ref import (ACT_LRELU, ACT_TANH, check_conv4_sums, check_stat_rows, check_wgrad_c1, conv4_ref64_elem, conv_variant,
+                             forward_launches, key, step_launches, wgrad4_ref64, wgrad_c1_ref64)
+from tests.launch_audit import K, memory_per_test, sms  # noqa: F401  (fixtures)
+from tests.launch_audit import (ALPHA_BN, BENCH_OPT, NAN, SKIP_OPT, AuditKernels, RecordingKernels, addend_index, audit_step,
+                                bn_inputs, bn_stats, randn, slices_with_boundary)
+from tests.ref64 import (EPS, assert_exact, binary01, bn_group_ref64, bound_check, check_finalize_vs_output, finalize_ref,
+                         gemm_ref64)
 from tests.tc_schedule import BETA, assert_within, cdiv, conv_tiles, gemm_tc_tiles, sm_count
-from tests.test_tc_schedule_gpu import image_slices
-from tests.vgg_ref import assert_exact, binary01, bound_check, check_finalize_vs_output, finalize_ref, gemm_ref64
 
 pytestmark = pytest.mark.gpu
 
 CONFIGS = {"C2": dict(T=30, B=256, nc=1, W0=64), "C4": dict(T=30, B=64, nc=3, W0=128)}
-BENCH_OPT = dict(skip_prob=0.0, n_past=1, last_frame_skip=False)
-NAN = float("nan")
-# BatchNorm sums: fp32 per-thread running sums, combined in float64 (test_bn_backward_gpu.py ALPHA)
-ALPHA_BN = 2.0 ** -14
-
-
-@pytest.fixture(scope="module")
-def K():
-    from p2pvg_b200._lib import CudaKernels
-    return CudaKernels("cuda")
-
-
-@pytest.fixture(autouse=True)
-def memory_per_test(request):
-    if torch.cuda.is_available():
-        torch.cuda.reset_peak_memory_stats()
-        t0 = time.time()
-    yield
-    if torch.cuda.is_available():
-        _release()
-        print(f"\n[memory] {request.node.name}: {time.time() - t0:.1f} s, peak {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB")
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return sm_count()
 
 
 def plan_for(cfg):
@@ -77,76 +52,35 @@ def launches(name):
     return step_launches(c["T"], c["B"], p.S, p.nskip, c["nc"], c["W0"], p.has_cpc)
 
 
-def randn(*shape, scale=1.0, dtype=torch.bfloat16):
-    return (torch.randn(*shape, device="cuda") * scale).to(dtype)
-
-
-def _release():
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
 # ------------------------------------------------------------------ A. the launch lists
 
-def _recording_class():
-    from p2pvg_b200._lib import CudaKernels
+def _bn_key(op, C=None, act=None):
+    """What dcgan_ref.key gives a BatchNorm entry point; C / act: the value listed where the entry point takes no such
+    argument (None: the entry has none)."""
+    def f(k, x):
+        return (op, x["G"], x["R"] if "R" in x else None, x["C"] if "C" in x else C, x["act"] if "act" in x else act, x.get("F"),
+                x["dout"] is not None if op == "bn_bwd_group_sum" else False)
+    return f
 
-    def bound(meth, a, kw):
-        ba = inspect.signature(getattr(CudaKernels, meth)).bind(None, *a, **kw)
-        ba.apply_defaults()
-        return ba.arguments
 
-    class RecordingKernels(CudaKernels):
-        """CudaKernels that logs the shapes and flags of every conv_gemm, bf16 gemm and BatchNorm launch, then calls through."""
-
-        def __init__(self, *a, **kw):
-            super().__init__(*a, **kw)
-            self.calls = []
-            self.muted = False   # set while the engine runs the LSTM weight gradients (bf16 copies of fp32 operands)
-
-        def conv_gemm(self, *a, **kw):
-            x = bound("conv_gemm", a, kw)
-            self.calls.append(("conv_gemm", x["kind"], x["N"], x["H"], x["Ck"], x["Cn"], x["Cm"], x["bias"] is not None,
-                               x["addend"].dtype if x["addend"] is not None else None, x["imgs_per_group"], x["stat_partial"] is not None))
-            super().conv_gemm(*a, **kw)
-
-        def gemm(self, *a, **kw):
-            x = bound("gemm", a, kw)
-            if x["A"].dtype == torch.bfloat16 and not self.muted:   # the LSTM / latent GEMMs take fp32 operands
-                self.calls.append(("gemm", x["M"], x["N"], x["K"], x["a_mn"], x["b_mn"], x["bias"] is not None))
-            super().gemm(*a, **kw)
-
-        def _bn(self, op, a, kw, R=True, C=True, act=True):
-            x = bound(op, a, kw)
-            self.calls.append((op, x["G"], x["R"] if R else None, (x["C"] if C else 64) if C is not None else None,
-                               (x["act"] if act else ACT_LRELU) if act is not None else None, x.get("F"),
-                               x.get("dout") is not None if op == "bn_bwd_group_sum" else False))
-            getattr(super(), op)(*a, **kw)
-
-        def bn_fwd_stats(self, *a, **kw):
-            self._bn("bn_fwd_stats", a, kw, act=None)
-
-        def bn_fwd_finalize_tiles(self, *a, **kw):
-            self._bn("bn_fwd_finalize_tiles", a, kw, act=None)
-
-        def bn_act(self, *a, **kw):
-            self._bn("bn_act", a, kw)
-
-        def bn_bwd(self, *a, **kw):
-            self._bn("bn_bwd", a, kw)
-
-        def bn_bwd_group_sum(self, *a, **kw):
-            self._bn("bn_bwd_group_sum", a, kw, act=False)
-
-        def bn_bwd_wgrad_c1(self, *a, **kw):
-            self._bn("bn_bwd_wgrad_c1", a, kw, C=False, act=False)
-
-        def bn_param_grad(self, *a, **kw):
-            x = bound("bn_param_grad", a, kw)
-            self.calls.append(("bn_param_grad", x["G"], None, x["C"], None, None, False))
-            super().bn_param_grad(*a, **kw)
-
-    return RecordingKernels
+class DcganRecording(RecordingKernels):
+    """Logs the shapes and flags of every conv_gemm, bf16 gemm and BatchNorm launch."""
+    muted = False   # set while the engine runs the LSTM weight gradients (bf16 copies of fp32 operands)
+    RECORD = {
+        "conv_gemm": lambda k, x: ("conv_gemm", x["kind"], x["N"], x["H"], x["Ck"], x["Cn"], x["Cm"], x["bias"] is not None,
+                                   x["addend"].dtype if x["addend"] is not None else None, x["imgs_per_group"],
+                                   x["stat_partial"] is not None),
+        # the LSTM / latent GEMMs take fp32 operands
+        "gemm": lambda k, x: ("gemm", x["M"], x["N"], x["K"], x["a_mn"], x["b_mn"], x["bias"] is not None)
+        if x["A"].dtype == torch.bfloat16 and not k.muted else None,
+        "bn_fwd_stats": _bn_key("bn_fwd_stats"),
+        "bn_fwd_finalize_tiles": _bn_key("bn_fwd_finalize_tiles"),
+        "bn_act": _bn_key("bn_act"),
+        "bn_bwd": _bn_key("bn_bwd"),
+        "bn_bwd_group_sum": _bn_key("bn_bwd_group_sum", act=ACT_LRELU),
+        "bn_bwd_wgrad_c1": _bn_key("bn_bwd_wgrad_c1", C=64, act=ACT_LRELU),
+        "bn_param_grad": _bn_key("bn_param_grad"),
+    }
 
 
 def _cfg(c):
@@ -163,7 +97,7 @@ def test_launch_list_matches_an_eager_step(name):
     T, B = c["T"], c["B"]
     opt = O.default_opt(**BENCH_OPT)
     opt["batch_size"] = B
-    eng = TrainEngine(O.build_state(_cfg(c), seed=1), _cfg(c), opt, _recording_class()("cuda"), act_dtype=torch.bfloat16)
+    eng = TrainEngine(O.build_state(_cfg(c), seed=1), _cfg(c), opt, DcganRecording("cuda"), act_dtype=torch.bfloat16)
     lin_wgrad = eng.lin_wgrad
 
     def muted_lin_wgrad(*a, **kw):   # TrainEngine.lin_wgrad: the LSTM / head weight gradients, not part of the lists
@@ -244,19 +178,6 @@ def _dedup(Ls):
 CONV = [(n, L) for n in CONFIGS for L in _dedup(launches(n))]
 
 
-def slices_with_boundary(N, HW, s, sms, B):
-    """Tile-aligned image ranges of the first, middle and last round, each a launch of <= SMs tiles; the middle one straddles
-    the boundary between two groups of B images."""
-    unit = max(1, s.BM // HW)
-    first, _, last = image_slices(N, HW, unit, s, sms)
-    ni = first[1]
-    if ni < 2:
-        return [first, last]
-    b = (N // 2) // B * B
-    i0 = max(unit, (b - ni // 2) // unit * unit)
-    return [first, (i0, min(N, i0 + ni)), last]
-
-
 @pytest.mark.parametrize("cfg,L", CONV, ids=[f"{n}-{L['name'].replace(' ', '_')}-N{L['N']}" for n, L in CONV])
 def test_conv_launch(K, sms, cfg, L):
     kind, N, H, Ck, Cn, B = L["kind"], L["N"], L["H"], L["Ck"], L["Cn"], CONFIGS[cfg]["B"]
@@ -274,8 +195,7 @@ def test_conv_launch(K, sms, cfg, L):
         nsrc = 3   # more sources than the bench plan's one: every group reads another source than its neighbours
         G = cdiv(N, ipg)
         src = torch.tensor([(g + 1) % nsrc for g in range(G)], dtype=torch.int32, device="cuda")
-        srcl = src.tolist()
-        idx = torch.tensor([srcl[n // ipg] * ipg + n % ipg for n in range(N)], device="cuda")
+        idx = addend_index(src.tolist(), ipg, N)
         add = randn(nsrc * ipg, Ho, Ho, Cn)
     st = L["stat"]
     s = conv_tiles(kind, N, H, H, Ck, Cn, 0, sms, stat=st is not None)
@@ -400,20 +320,6 @@ def test_weight_gradient_gemm(K, sms, cfg, L):
 
 # ------------------------------------------------------------------ D. BatchNorm at the launch shapes
 
-def _bn_inputs(G, R, C, seed, dt=torch.bfloat16):
-    gen = torch.Generator(device="cuda").manual_seed(seed)
-    raw = (torch.randn(G * R * C, device="cuda", generator=gen) * 1.5 + 0.3).to(dt)
-    gamma = torch.rand(C, device="cuda", generator=gen) + 0.5
-    beta = torch.randn(C, device="cuda", generator=gen) * 0.5
-    return raw, gamma, beta, gen
-
-
-def _stats(K, raw, G, R, C, gamma, beta):
-    st = {k: torch.full((G * C,), NAN, device="cuda") for k in ("mean", "invstd", "varu", "scale", "shift", "sdz", "sdzx")}
-    K.bn_fwd_stats(raw, G, R, C, gamma, beta, st["mean"], st["invstd"], st["varu"], st["scale"], st["shift"])
-    return st
-
-
 def _check_stats(st, raw, G, R, C, gamma, beta, name):
     """bn_fwd_stats against float64 group by group (finalize_ref's bounds with sums known within ALPHA_BN)."""
     x = raw.view(G, R, C)
@@ -445,8 +351,8 @@ def test_bn_forward_at_launch_shape(K, case):
     within the float64 bound, y = act(fmaf(x, scale, shift)) within one fp32 and one bf16 rounding."""
     cfg, G, R, C, act, nm = case
     name = f"{cfg} {nm} G={G} R={R} C={C}"
-    raw, gamma, beta, _ = _bn_inputs(G, R, C, seed=G * 7 + C)
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    raw, gamma, beta, _ = bn_inputs(G, R, C, seed=G * 7 + C)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     w = _check_stats(st, raw, G, R, C, gamma, beta, f"bn_fwd_stats {name}")
     y = torch.full_like(raw, NAN)
     K.bn_act(raw, y, st["scale"], st["shift"], G, R, C, act)
@@ -514,8 +420,8 @@ def test_bn_bwd_at_launch_shape(K, case):
     """bn_bwd as the step calls it (in place; LeakyReLU: y = None, slope from scale / shift; tanh: y given) and bn_param_grad."""
     cfg, G, R, C, act, nm = case
     name = f"bn_bwd {cfg} {nm} G={G} R={R} C={C}"
-    raw, gamma, beta, gen = _bn_inputs(G, R, C, seed=G * 11 + C)
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    raw, gamma, beta, gen = bn_inputs(G, R, C, seed=G * 11 + C)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     x64 = raw.view(G, R, C)
     # dy correlated with xhat, so that the xhat term of dx carries weight
     dy = torch.empty_like(raw)
@@ -566,10 +472,10 @@ def test_bn_bwd_group_sum_at_launch_shape(K, case, plan):
     if plan == "four_sources":
         assert len(set(srcl)) == 3 and 2 not in srcl
     name = f"bn_bwd_group_sum {cfg} {nm} G={G} R={R} C={C} {plan}"
-    raw, gamma, beta, gen = _bn_inputs(G, R, C, seed=G * 13 + C)
+    raw, gamma, beta, gen = bn_inputs(G, R, C, seed=G * 13 + C)
     if with_dout:   # beta >= 0.5: y = lrelu(gamma xhat + beta) has a positive mean in every channel, so y * dout does not cancel
         beta = beta.abs() + 0.5
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     dy = (torch.randn(G * R * C, device="cuda", generator=gen) * 1e-2).to(torch.bfloat16)
     refs = _refs(raw, dy, st, gamma, beta, G, R, C, ACT_LRELU)
     grp = torch.tensor(srcl, dtype=torch.int32, device="cuda")
@@ -624,8 +530,8 @@ def test_bn_bwd_wgrad_c1_c2_enc0(K):
     G, Ho, C = c["T"], c["W0"] // 2, 64
     R = c["B"] * Ho * Ho
     name = f"bn_bwd_wgrad_c1 C2 enc0 G={G} R={R}"
-    raw, gamma, beta, gen = _bn_inputs(G, R, C, seed=41)
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    raw, gamma, beta, gen = bn_inputs(G, R, C, seed=41)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     # dx is orthogonal to 1 (and to xhat) per group and channel, so against an arbitrary input map its weight gradient cancels.
     # Here dy has the sign s = +1 on even images and -1 on odd ones: dx then has about that sign (its mean terms are small),
     # and the input map is zero on the odd images, so the weight gradient sums |dx| * taps without cancelling
@@ -654,157 +560,60 @@ def test_bn_bwd_wgrad_c1_c2_enc0(K):
 
 # ------------------------------------------------------------------ E. audit of real steps
 
-def _make_audit_class():
-    from p2pvg_b200._lib import CudaKernels
+class DcganAudit(AuditKernels):
+    """AuditKernels for a dcgan step: its conv_gemm launches (kinds 0, 1, 2), the bf16 GEMMs only, and the skip sums of
+    bn_bwd_group_sum.  The data-movement kernels of the 1- / 3-channel ends (im2col, col2im, convt_c1_loss, nchw_to_nhwc_dual)
+    and the other BatchNorm entry points are not audited here: parts B-D and tests/test_bn_*_gpu.py check them at the step's
+    shapes.  The fp32 LSTM / latent GEMMs: tests/test_lstm_scan_gpu.py, test_tc_schedule_gpu.py."""
+    GEMM_FP32 = False
+    GEMM_ACCUMULATE = False
+    GEMM_PROBE_K = 1 << 12
 
-    class AuditKernels(CudaKernels):
-        """CudaKernels whose conv_gemm launches (kinds 0, 1, 2), bf16 GEMMs, skip-frame sums (group_sum, the skip sums of
-        bn_bwd_group_sum) and add_indexed are each checked against float64 on their own operands right after they run (device
-        synchronised around each call; inputs a call overwrites are cloned first; nothing the step reads is changed).  The
-        data-movement kernels of the 1- / 3-channel ends (im2col, col2im, convt_c1_loss, nchw_to_nhwc_dual) and the other
-        BatchNorm entry points are not audited here: parts B-D and tests/test_bn_*_gpu.py check them at the step's shapes."""
+    def conv_gemm(self, kind, a, b, c, N, H, W, Ck, Cn, Cm=0, ldb=None, ldc=None, bias=None, addend=None, grp_src=None,
+                  imgs_per_group=0, accumulate=False, stat_partial=None, eval_scale=None, eval_shift=None, act=0):
+        assert kind in (0, 1, 2) and H == W and eval_scale is None and not accumulate, f"unexpected conv_gemm launch kind {kind}"
+        self._sync("conv_gemm", kind, a, b, c, N, H, W, Ck, Cn, Cm, ldb, ldc, bias, addend, grp_src, imgs_per_group, accumulate,
+                   stat_partial, eval_scale, eval_shift, act)
+        if kind == 1:
+            s = conv_tiles(1, N, H, W, 0, Cn, Cm, self._sms)
+            x = a.view(-1)[:N * H * H * Cm].view(N, H, H, Cm)
+            g = b.view(-1)[:N * 4 * H * H * Cn].view(N, 2 * H, 2 * H, Cn)
+            ref, absref = wgrad4_ref64(x, g, N, H, Cm, Cn)
+            w = assert_within(c.view(-1)[:Cm * 16 * Cn].view(Cm, 16 * Cn), ref, absref, s.kb_per_split * 64 + 16 * s.splits,
+                              torch.float32, quiet=True, name=f"audit kind 1 N={N} {H}x{H} {Cm}x{Cn}")
+            # the step's gradients cancel over these K, so the bound above is loose: the same launch on the 0 / 1 pattern
+            # of its operands must be exact
+            x01, g01 = (x > 0).bfloat16(), (g > 0).bfloat16()
+            probe = torch.full((Cm, 16 * Cn), NAN, device=c.device)
+            super().conv_gemm(1, x01, g01, probe, N, H, H, 0, Cn, Cm=Cm)
+            assert_exact(probe, wgrad4_ref64(x01, g01, N, H, Cm, Cn)[0], N * H * H, f"audit kind 1 N={N} {H}x{H} 0/1 probe")
+            self._rec(f"conv_gemm kind 1 N={N} {H}x{H} {Cm}x{Cn}", ("k1",), w)
+            return
+        Ha, Ho = (2 * H, H) if kind == 0 else (H, 2 * H)
+        x = a.view(-1)[:N * Ha * Ha * Ck].view(N, Ha, Ha, Ck)
+        wt = b.view(-1)[:16 * Ck * Cn].view(*((Cn, 16 * Ck) if kind == 0 else (Ck, 16 * Cn)))
+        out = c.view(-1)[:N * Ho * Ho * Cn].view(N, Ho, Ho, Cn)
+        add, idx = self._addend(addend, grp_src, imgs_per_group, N, Ho, Cn) if addend is not None else (None, None)
+        nm = f"conv_gemm kind {kind} N={N} {H}x{H} {Ck}->{Cn}"
+        w = check_conv4_sums(out, kind, x, wt, N, H, Ck, Cn, bias, add, idx, name="audit " + nm)
+        for i0 in sorted({0, N // 2, N - 1}):   # three images element-wise
+            ref, absref = conv4_ref64_elem(kind, x[i0:i0 + 1], wt, H, Ck, Cn, bias, add[idx[i0:i0 + 1]] if add is not None else None)
+            w = max(w, assert_within(out[i0:i0 + 1], ref, absref, 16 * Ck, out.dtype, quiet=True, name=f"audit {nm} image {i0}"))
+        if stat_partial is not None:
+            rows = cdiv(N * H * H, 128) * (4 if kind == 2 else 1)
+            w = max(w, check_stat_rows(stat_partial.view(-1)[:rows * Cn * 2].view(rows, Cn, 2), out, kind, N, H, Cn, name="audit " + nm))
+        self._rec(nm, conv_variant(kind, Cn, stat_partial is not None, addend.dtype if addend is not None else None, H, c.dtype), w)
 
-        def __init__(self, *a, **kw):
-            super().__init__(*a, **kw)
-            self.log = []          # (what, variant, worst ratio)
-            self.seen = set()
-            self.skip_reads = []   # grp_src of every launch with a skip addend
-            self._sms = sm_count()
-
-        def _rec(self, what, v, worst):
-            self.log.append((what, v, worst))
-            self.seen.add(v)
-
-        def conv_gemm(self, kind, a, b, c, N, H, W, Ck, Cn, Cm=0, ldb=None, ldc=None, bias=None, addend=None, grp_src=None,
-                      imgs_per_group=0, accumulate=False, stat_partial=None, eval_scale=None, eval_shift=None, act=0):
-            assert kind in (0, 1, 2) and H == W and eval_scale is None and not accumulate, f"unexpected conv_gemm launch kind {kind}"
-            torch.cuda.synchronize()
-            super().conv_gemm(kind, a, b, c, N, H, W, Ck, Cn, Cm, ldb, ldc, bias, addend, grp_src, imgs_per_group, accumulate,
-                              stat_partial, eval_scale, eval_shift, act)
-            torch.cuda.synchronize()
-            if kind == 1:
-                s = conv_tiles(1, N, H, W, 0, Cn, Cm, self._sms)
-                x = a.view(-1)[:N * H * H * Cm].view(N, H, H, Cm)
-                g = b.view(-1)[:N * 4 * H * H * Cn].view(N, 2 * H, 2 * H, Cn)
-                ref, absref = wgrad4_ref64(x, g, N, H, Cm, Cn)
-                w = assert_within(c.view(-1)[:Cm * 16 * Cn].view(Cm, 16 * Cn), ref, absref, s.kb_per_split * 64 + 16 * s.splits,
-                                  torch.float32, quiet=True, name=f"audit kind 1 N={N} {H}x{H} {Cm}x{Cn}")
-                # the step's gradients cancel over these K, so the bound above is loose: the same launch on the 0 / 1 pattern
-                # of its operands must be exact
-                x01, g01 = (x > 0).bfloat16(), (g > 0).bfloat16()
-                probe = torch.full((Cm, 16 * Cn), NAN, device=c.device)
-                super().conv_gemm(1, x01, g01, probe, N, H, H, 0, Cn, Cm=Cm)
-                assert_exact(probe, wgrad4_ref64(x01, g01, N, H, Cm, Cn)[0], N * H * H, f"audit kind 1 N={N} {H}x{H} 0/1 probe")
-                self._rec(f"conv_gemm kind 1 N={N} {H}x{H} {Cm}x{Cn}", ("k1",), w)
-                return
-            Ha, Ho = (2 * H, H) if kind == 0 else (H, 2 * H)
-            x = a.view(-1)[:N * Ha * Ha * Ck].view(N, Ha, Ha, Ck)
-            wt = b.view(-1)[:16 * Ck * Cn].view(*((Cn, 16 * Ck) if kind == 0 else (Ck, 16 * Cn)))
-            out = c.view(-1)[:N * Ho * Ho * Cn].view(N, Ho, Ho, Cn)
-            add = idx = None
-            if addend is not None:
-                srcl = grp_src.tolist()
-                ipg = max(1, imgs_per_group)
-                self.skip_reads.append(srcl[:cdiv(N, ipg)])
-                nimg = (max(srcl[:cdiv(N, ipg)]) + 1) * ipg
-                add = addend.view(-1)[:nimg * Ho * Ho * Cn].view(nimg, Ho, Ho, Cn)
-                idx = torch.tensor([srcl[n // ipg] * ipg + n % ipg for n in range(N)], device=a.device)
-            nm = f"conv_gemm kind {kind} N={N} {H}x{H} {Ck}->{Cn}"
-            w = check_conv4_sums(out, kind, x, wt, N, H, Ck, Cn, bias, add, idx, name="audit " + nm)
-            for i0 in sorted({0, N // 2, N - 1}):   # three images element-wise
-                ref, absref = conv4_ref64_elem(kind, x[i0:i0 + 1], wt, H, Ck, Cn, bias, add[idx[i0:i0 + 1]] if add is not None else None)
-                w = max(w, assert_within(out[i0:i0 + 1], ref, absref, 16 * Ck, out.dtype, quiet=True, name=f"audit {nm} image {i0}"))
-            if stat_partial is not None:
-                rows = cdiv(N * H * H, 128) * (4 if kind == 2 else 1)
-                w = max(w, check_stat_rows(stat_partial.view(-1)[:rows * Cn * 2].view(rows, Cn, 2), out, kind, N, H, Cn, name="audit " + nm))
-            self._rec(nm, conv_variant(kind, Cn, stat_partial is not None, addend.dtype if addend is not None else None, H, c.dtype), w)
-
-        def gemm(self, A, B, C, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldc=None, accumulate=False, bias=None,
-                 addend=None, ldd=None):
-            if A.dtype != torch.bfloat16:   # the fp32 LSTM / latent GEMMs: tests/test_lstm_scan_gpu.py, test_tc_schedule_gpu.py
-                return super().gemm(A, B, C, M, N, K, a_mn, b_mn, lda, ldb, ldc, accumulate, bias, addend, ldd)
-            torch.cuda.synchronize()
-            lda_ = lda if lda is not None else (M if a_mn else K)
-            ldb_ = ldb if ldb is not None else (N if b_mn else K)
-            ldc_ = ldc if ldc is not None else N
-            cv = C.as_strided((M, N), (ldc_, 1))
-            assert not accumulate and addend is None
-            super().gemm(A, B, C, M, N, K, a_mn, b_mn, lda, ldb, ldc, accumulate, bias, addend, ldd)
-            torch.cuda.synchronize()
-            w, step = 0.0, max(1, (1 << 22) // N)
-            for m0 in range(0, M, step):
-                m1 = min(M, m0 + step)
-                ref, absref = gemm_ref64(A, B, M, N, K, a_mn, b_mn, lda_, ldb_, bias=bias, rows=(m0, m1))
-                w = max(w, assert_within(cv[m0:m1], ref, absref, K, C.dtype, quiet=True,
-                                         name=f"audit gemm {M}x{N}x{K} a_mn={a_mn} b_mn={b_mn} rows {m0}"))
-            if K >= 1 << 12 and C.dtype == torch.float32:
-                # weight gradients: cancelling sums, so the same launch on the 0 / 1 pattern of the operands must be exact
-                A01, B01 = (A > 0).to(A.dtype), (B > 0).to(B.dtype)
-                probe = torch.full((M, N), NAN, device=C.device)
-                super().gemm(A01, B01, probe, M, N, K, a_mn, b_mn, lda, ldb)
-                assert_exact(probe, gemm_ref64(A01, B01, M, N, K, a_mn, b_mn, lda_, ldb_)[0], K, f"audit gemm {M}x{N}x{K} 0/1 probe")
-            self._rec(f"gemm {M}x{N}x{K}", ("gemm",), w)
-
-        def _skip_sums(self, inp, out, srcl, G, F_, n, what):
-            iv = inp.view(-1)[:G * n].view(G, n)
-            w = 0.0
-            for f in range(F_):
-                gs = [g for g in range(G) if srcl[g] == f]
-                ref = iv[gs].double().sum(0) if gs else torch.zeros(n, dtype=torch.float64, device=inp.device)
-                mag = iv[gs].double().abs().sum(0) if gs else torch.zeros_like(ref)
-                w = max(w, bound_check(out.view(-1)[f * n:(f + 1) * n], ref, len(gs) * 2.0 ** -24 * mag + BETA[out.dtype] * ref.abs(),
-                                        f"audit {what} source {f}"))
-            return w
-
-        def group_sum(self, inp, out, grp_src, G, F_, n):
-            torch.cuda.synchronize()
-            super().group_sum(inp, out, grp_src, G, F_, n)
-            torch.cuda.synchronize()
-            self._rec(f"group_sum G={G} F={F_}", ("group_sum",), self._skip_sums(inp, out, grp_src.tolist()[:G], G, F_, n, "group_sum"))
-
-        def bn_bwd_group_sum(self, dy, x, mean, invstd, gamma, G, R, C, dx, sum_dz, sum_dzx, scale, shift, grp_src, F, dx_sum,
-                             dout=None, Ho=0, wpart=None, dw=None):
-            torch.cuda.synchronize()
-            super().bn_bwd_group_sum(dy, x, mean, invstd, gamma, G, R, C, dx, sum_dz, sum_dzx, scale, shift, grp_src, F, dx_sum,
-                                     dout, Ho, wpart, dw)
-            torch.cuda.synchronize()
-            w = self._skip_sums(dx, dx_sum, grp_src.tolist()[:G], G, F, R * C, "bn_bwd_group_sum skip sums")
-            self._rec(f"bn_bwd_group_sum G={G} R={R} C={C}", ("bn_bwd_group_sum", dout is not None), w)
-
-        def add_indexed(self, dst, src, dst_idx, F_, n):
-            torch.cuda.synchronize()
-            di = dst_idx.tolist()[:F_]
-            d0 = [dst.view(-1)[d * n:(d + 1) * n].clone() for d in di]
-            super().add_indexed(dst, src, dst_idx, F_, n)
-            torch.cuda.synchronize()
-            w = 0.0
-            for f, d in enumerate(di):
-                ref = d0[f].double() + src.view(-1)[f * n:(f + 1) * n].double()
-                w = max(w, bound_check(dst.view(-1)[d * n:(d + 1) * n], ref, BETA[dst.dtype] * ref.abs(), "audit add_indexed"))
-            self._rec(f"add_indexed F={F_}", ("add_indexed",), w)
-
-    return AuditKernels
+    def bn_bwd_group_sum(self, dy, x, mean, invstd, gamma, G, R, C, dx, sum_dz, sum_dzx, scale, shift, grp_src, F, dx_sum,
+                         dout=None, Ho=0, wpart=None, dw=None):
+        self._sync("bn_bwd_group_sum", dy, x, mean, invstd, gamma, G, R, C, dx, sum_dz, sum_dzx, scale, shift, grp_src, F, dx_sum,
+                   dout, Ho, wpart, dw)
+        w = self._skip_sums(dx, dx_sum, grp_src.tolist()[:G], G, F, R * C, "bn_bwd_group_sum skip sums")
+        self._rec(f"bn_bwd_group_sum G={G} R={R} C={C}", ("bn_bwd_group_sum", dout is not None), w)
 
 
-def _step(kernels, c, optkw, T, B, np_seed):
-    from p2pvg_b200.engine import TrainEngine
-    opt = O.default_opt(**optkw)
-    opt["batch_size"] = B
-    eng = TrainEngine(O.build_state(_cfg(c), seed=1), _cfg(c), opt, kernels, act_dtype=torch.bfloat16)
-    x = torch.rand(T, B, c["nc"], c["W0"], c["W0"], generator=torch.Generator().manual_seed(5))
-    probs = np.random.RandomState(np_seed).uniform(0, 1, T - 1)
-    plan = StepPlan(T, probs, opt)
-    eps = O.draw_eps(plan.S, B, 10, seed=11)
-    losses = eng.step(x.cuda(), probs=probs, eps=eps.cuda())
-    torch.cuda.synchronize()
-    grads = {m: {k: v.detach().clone() for k, v in eng.arena[m].g.items()} for m in eng.arena}
-    params = {m: {k: v.detach().clone() for k, v in eng.arena[m].p.items()} for m in eng.arena}
-    return plan, np.asarray(losses), grads, params, eng
-
-
-SKIP_OPT = dict(skip_prob=0.5, n_past=2, last_frame_skip=True)
-AUDIT_CASES = [("dcgan64_bench_options", "C2", BENCH_OPT, 64, None), ("dcgan64_skip_lfs", "C2", SKIP_OPT, 64, "search"),
-               ("dcgan128_bench_options", "C4", BENCH_OPT, 16, None)]
+AUDIT_CASES = [("dcgan64_bench_options", "C2", BENCH_OPT, 64), ("dcgan64_skip_lfs", "C2", SKIP_OPT, 64),
+               ("dcgan128_bench_options", "C4", BENCH_OPT, 16)]
 
 
 @pytest.mark.parametrize("case", AUDIT_CASES, ids=[c[0] for c in AUDIT_CASES])
@@ -812,35 +621,16 @@ def test_audit_dcgan_step(case):
     """One eager bf16 step at T = 30 with the audited launches checked as they run.  Every conv_gemm variant of the derived
     launch list must occur, every skip addend must be read through plan.skip_src, and losses, gradients and parameters must
     equal (torch.equal) the same step on plain CudaKernels with its concurrent lanes (so the side lanes share no scratch)."""
-    from p2pvg_b200._lib import CudaKernels
-    from tests.test_vgg_launches_gpu import _skip_seed
-    name, cfg, optkw, B, seed = case
+    name, cfg, optkw, B = case
     c, T = CONFIGS[cfg], 30
-    seed = _skip_seed(T) if seed == "search" else 0
-    plan, losses, grads, params, eng = _step(CudaKernels("cuda"), c, optkw, T, B, seed)
-    del eng
-    _release()
-    if seed:
-        assert len(set(plan.skip_src)) >= 3
-    plan_a, losses_a, grads_a, params_a, eng = _step(_make_audit_class()("cuda"), c, optkw, T, B, seed)
-    log, seen, skip_reads = eng.K.log, eng.K.seen, eng.K.skip_reads
-    del eng
-    _release()
-    want = {L["variant"] for L in step_launches(T, B, plan.S, plan.nskip, c["nc"], c["W0"], plan.has_cpc) if L["op"] == "conv_gemm"}
-    # the explicit last layer sums its skip columns with group_sum; a 1-channel one defers its weight gradient to `dout`
-    want |= {("gemm",), ("bn_bwd_group_sum", False), ("add_indexed",), ("group_sum",)}
-    if c["nc"] == 1:
-        want.add(("bn_bwd_group_sum", True))
-    assert conv_variant(2, 64, False, torch.bfloat16, 16) in want, "the derived list lost the 256-row addend launch"
-    missing = want - seen
-    assert not missing, f"launch variants that did not occur in the step: {sorted(missing)}"
-    fwd = forward_launches(T, B, plan.S, plan.nskip, c["nc"], c["W0"])
-    assert len(skip_reads) == sum(1 for L in fwd if L["op"] == "conv_gemm" and L["addend"] is not None)
-    for r in skip_reads:
-        assert r == plan.skip_src, f"skip addend read through {r}, the schedule says {plan.skip_src}"
-    print(f"[audit] {name}: {len(log)} launches checked, worst error/bound {max(w for _, _, w in log):.3g}")
-    assert np.array_equal(losses, losses_a), (losses, losses_a)
-    for m in grads:
-        for k in grads[m]:
-            assert torch.equal(grads[m][k], grads_a[m][k]), f"grad {m}.{k} differs under the audit"
-            assert torch.equal(params[m][k], params_a[m][k]), f"param {m}.{k} differs under the audit"
+
+    def expect(plan):
+        want = {L["variant"] for L in step_launches(T, B, plan.S, plan.nskip, c["nc"], c["W0"], plan.has_cpc) if L["op"] == "conv_gemm"}
+        # the explicit last layer sums its skip columns with group_sum; a 1-channel one defers its weight gradient to `dout`
+        want |= {("gemm", "bfloat16", "-"), ("bn_bwd_group_sum", False), ("add_indexed",), ("group_sum",)}
+        if c["nc"] == 1:
+            want.add(("bn_bwd_group_sum", True))
+        assert conv_variant(2, 64, False, torch.bfloat16, 16) in want, "the derived list lost the 256-row addend launch"
+        fwd = forward_launches(T, B, plan.S, plan.nskip, c["nc"], c["W0"])
+        return want, [plan.skip_src] * sum(1 for L in fwd if L["op"] == "conv_gemm" and L["addend"] is not None)
+    audit_step(TrainEngine, _cfg(c), optkw, T, B, DcganAudit("cuda"), expect, name)

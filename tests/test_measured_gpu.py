@@ -18,6 +18,7 @@ import torch
 
 from oracle import p2p_oracle as O
 from p2pvg_b200.engine import StepPlan, TrainEngine
+from tests.launch_audit import restore, snapshot
 from tests.test_engine_emu import CFG64, bn_cancelled_bias
 
 pytestmark = pytest.mark.gpu
@@ -27,23 +28,6 @@ LR = 1e-3
 # bf16-rounded tensor, so the first encoder layer sits lowest.  The exact-fp32 mode holds 1 - 1e-4 (tests/test_vgg_gpu.py).
 VGG_MIN_COS = 0.90
 VGG_MEDIAN_COS = 0.975
-
-
-def snapshot(eng):
-    return {m: (eng.arena[m].flat.clone(), {k: v.clone() for k, v in eng.buffers[m].items()}) for m in O.MODULES}
-
-
-def restore(eng, snap):
-    """Back to the initial state IN PLACE (captured graphs keep pointing at the same arenas)."""
-    for m in O.MODULES:
-        A = eng.arena[m]
-        A.flat.copy_(snap[m][0])
-        A.grad.zero_()
-        A.m.zero_()
-        A.v.zero_()
-        A.step_t.zero_()
-        for k, v in snap[m][1].items():
-            eng.buffers[m][k].copy_(v)
 
 
 def adam_reference(w0, g, lr=LR, b1=0.9, b2=0.999, eps=1e-8):

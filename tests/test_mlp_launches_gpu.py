@@ -27,14 +27,19 @@ import pytest
 import torch
 
 from oracle import p2p_oracle as O
+from p2pvg_b200._lib import CudaKernels, KernelError
 from p2pvg_b200.engine import StepPlan
+from p2pvg_b200.engine_mlp import TrainEngineMLP
+from tests.launch_audit import K, memory_per_test  # noqa: F401  (fixtures)
+from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, RecordingKernels, assert_concurrent, assert_equal_steps,
+                                audit_step, release, run_step, skip_seed, step_inputs)
 from tests.loss_ref import (ACT_RELU, ACT_TANH, TINY, act_bwd_ref, act_fwd_ref, build_concat_ref, check_gather_add_cols,
                             check_layernorm_bwd, check_layernorm_fwd)
 from tests.lstm_schedule import U
 from tests.mlp_ref import (POSE, TF32_FLAG, TF32_REQUIRE, backbone_launches, entry_kernel, gemm_alpha, gemm_variant, kernel_for,
                            key, simt_alpha)
-from tests.tc_schedule import alpha_for, assert_within, gemm_tc_tiles, sm_count
-from tests.vgg_ref import assert_exact, bound_check, gemm_ref64
+from tests.ref64 import assert_exact, bound_check, gemm_ref64
+from tests.tc_schedule import alpha_for, assert_within, gemm_tc_tiles
 
 pytestmark = pytest.mark.gpu
 
@@ -42,53 +47,12 @@ C5 = dict(T=60, B=256, R=512)
 CFG = dict(g_dim=128, z_dim=10, rnn_size=512, backbone="mlp", predictor_rnn_layers=2, posterior_rnn_layers=1, prior_rnn_layers=1)
 H = 128                      # h_dim = g_dim (engine_mlp.py:130)
 LD = 2 * H + 2               # pitch of the skip matrix (engine_mlp.py:167)
-BENCH_OPT = dict(skip_prob=0.0, n_past=1, last_frame_skip=False)
-SKIP_OPT = dict(skip_prob=0.5, n_past=2, last_frame_skip=True)
-NAN = float("nan")
 SENTINEL = -777.0
 BACKBONE = ("encode", "decode", "losses_fwd", "decoder_backward", "encoder_backward")
 
 
-@pytest.fixture(autouse=True)
-def memory_per_test(request):
-    if torch.cuda.is_available():
-        torch.cuda.reset_peak_memory_stats()
-        t0 = time.time()
-    yield
-    if torch.cuda.is_available():
-        _release()
-        print(f"\n[memory] {request.node.name}: {time.time() - t0:.1f} s, peak {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB")
-
-
-def _release():
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
-def _skip_seed(T):
-    """The first probability seed whose skip plan reads at least three skip sources."""
-    opt = O.default_opt(**SKIP_OPT)
-    for seed in range(100):
-        p = StepPlan(T, np.random.RandomState(seed).uniform(0, 1, T - 1), opt)
-        if len(set(p.skip_src)) >= 3:
-            return seed
-    raise AssertionError("no seed gives three skip sources")
-
-
-def _inputs(T, B, optkw):
-    opt = O.default_opt(**optkw)
-    opt["batch_size"] = B
-    seed = _skip_seed(T) if optkw.get("skip_prob") else 0
-    probs = np.random.RandomState(seed).uniform(0, 1, T - 1)
-    plan = StepPlan(T, probs, opt)
-    x = 3 * torch.randn(T, B, 17, 3, generator=torch.Generator().manual_seed(5))   # bench.py synth_batch: poses of std 3
-    eps = O.draw_eps(plan.S, B, CFG["z_dim"], seed=11)
-    return opt, probs, plan, x, eps
-
-
-def _engine(kernels, opt, adt):
-    from p2pvg_b200.engine_mlp import TrainEngineMLP
-    return TrainEngineMLP(O.build_state(CFG, seed=1), CFG, opt, kernels, act_dtype=adt)
+def _np_seed(T, optkw):
+    return skip_seed(T) if optkw.get("skip_prob") else 0
 
 
 def _watch(eng):
@@ -103,20 +67,6 @@ def _watch(eng):
             finally:
                 eng.K.on = False
         setattr(eng, nm, w)
-
-
-def _results(eng, losses):
-    torch.cuda.synchronize()
-    return (np.asarray(losses), {m: {k: v.detach().clone() for k, v in eng.arena[m].g.items()} for m in eng.arena},
-            {m: {k: v.detach().clone() for k, v in eng.arena[m].p.items()} for m in eng.arena})
-
-
-def _assert_equal_steps(a, b, what):
-    assert np.array_equal(a[0], b[0]), f"{what}: losses {a[0]} vs {b[0]}"
-    for i, kind in ((1, "grad"), (2, "param")):
-        for m in a[i]:
-            for k in a[i][m]:
-                assert torch.equal(a[i][m][k], b[i][m][k]), f"{what}: {kind} {m}.{k} differs"
 
 
 # ------------------------------------------------------------------ A. the launch lists
@@ -144,101 +94,70 @@ class _Locator:
         return ("?", p)
 
 
-def _recording_class():
-    from p2pvg_b200._lib import CudaKernels, KernelError
+def _on(f):
+    return lambda k, x: f(k.loc, x) if k.on else None
 
-    class RecordingKernels(CudaKernels):
-        """CudaKernels that logs every launch of the backbone (while `on`), with its operands located by buffer and offset.
-        rerun=True: each fp32 GEMM is also rerun on copies of its output through a view with P2PVG_GEMM_TF32 |
-        P2PVG_GEMM_TF32_REQUIRE and through one with flags 0, logging (ran on TF32, TF32 rerun identical, flags-0 rerun
-        identical)."""
 
-        def __init__(self, *a, rerun=False, **kw):
-            super().__init__(*a, **kw)
-            self.calls, self.reruns = [], []
-            self.on, self.rerun, self.loc = False, rerun, None
+class MlpRecording(RecordingKernels):
+    """Logs every launch of the backbone (while `on`), with its operands located by buffer and offset.  rerun=True: each
+    fp32 GEMM is also rerun on copies of its output through a view with P2PVG_GEMM_TF32 | P2PVG_GEMM_TF32_REQUIRE and through
+    one with flags 0, logging (ran on TF32, TF32 rerun identical, flags-0 rerun identical) in `reruns`."""
+    RECORD = {
+        "gemm": _on(lambda L, x: ("gemm", x["M"], x["N"], x["K"], x["a_mn"], x["b_mn"],
+                                  x["lda"] if x["lda"] is not None else (x["M"] if x["a_mn"] else x["K"]),
+                                  x["ldb"] if x["ldb"] is not None else (x["N"] if x["b_mn"] else x["K"]),
+                                  x["ldc"] if x["ldc"] is not None else x["N"], bool(x["accumulate"]), x["bias"] is not None,
+                                  L(x["A"]), L(x["B"]), L(x["C"]))),
+        "act_fwd": _on(lambda L, x: ("act_fwd", L(x["x"]), x["n"], x["act"])),
+        "act_bwd": _on(lambda L, x: ("act_bwd", L(x["dy"]), L(x["y"]), L(x["dx"]), x["n"], x["act"])),
+        "permute4": _on(lambda L, x: ("permute4", L(x["src"]), L(x["dst"]), tuple(x["dims"]), tuple(x["strides"]),
+                                      bool(x["accumulate"]))),
+        "layernorm_fwd": _on(lambda L, x: ("layernorm_fwd", L(x["x"]), L(x["y"]), x["rows"], x["C"])),
+        "layernorm_bwd": _on(lambda L, x: ("layernorm_bwd", L(x["dy"]), L(x["x"]), L(x["dx"]), x["dgamma"] is not None, x["rows"],
+                                           x["C"])),
+        "build_concat": _on(lambda L, x: ("build_concat", L(x["dst"]), L(x["A"]), L(x["ia"]), x["ga"], L(x["Bm"]), L(x["ib"]),
+                                          x["gb"], x["S"], x["B"], x["ld"])),
+        "gather_add_cols": _on(lambda L, x: ("gather_add_cols", L(x["dst"]), L(x["src"]), L(x["idx"]), x["S"], x["T"], x["B"],
+                                             x["g"], x["W"], x["col0"])),
+        "colsum": _on(lambda L, x: ("colsum", L(x["x"]), x["rows"], x["cols"], x["ld"], L(x["out"]))),
+        "mse_plain": _on(lambda L, x: ("mse_plain", L(x["pred"]), L(x["x"]), L(x["tgt"]), x["G"], x["E"])),
+    }
 
-        def _log(self, *t):
-            if self.on:
-                self.calls.append(t)
+    def __init__(self, *a, rerun=False, **kw):
+        super().__init__(*a, **kw)
+        self.reruns = []
+        self.on, self.rerun, self.loc = False, rerun, None
 
-        def gemm(self, A, B, C, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldc=None, accumulate=False, bias=None,
-                 addend=None, ldd=None):
-            args = (A, B, C, M, N, K, a_mn, b_mn, lda, ldb, ldc, accumulate, bias, addend, ldd)
-            if not self.on:
-                return super().gemm(*args)
-            L = self.loc
-            self.calls.append(("gemm", M, N, K, a_mn, b_mn, lda if lda is not None else (M if a_mn else K),
-                               ldb if ldb is not None else (N if b_mn else K), ldc if ldc is not None else N, bool(accumulate),
-                               bias is not None, L(A), L(B), L(C)))
-            if not self.rerun:
-                return super().gemm(*args)
-            torch.cuda.synchronize()
-            C0 = C.clone()
-            super().gemm(*args)
-            torch.cuda.synchronize()
-            req, plain = copy.copy(self), copy.copy(self)
-            req.gemm_flags, plain.gemm_flags = TF32_FLAG | TF32_REQUIRE, 0
-            C1, C2 = C0.clone(), C0.clone()
-            try:
-                CudaKernels.gemm(req, A, B, C1, *args[3:])
-                ran = True
-            except KernelError:
-                ran = False
-            CudaKernels.gemm(plain, A, B, C2, *args[3:])
-            torch.cuda.synchronize()
-            self.reruns.append((ran, ran and torch.equal(C1, C), torch.equal(C2, C)))
-
-        def act_fwd(self, x, n, act):
-            self._log("act_fwd", self.loc(x), n, act) if self.on else None
-            super().act_fwd(x, n, act)
-
-        def act_bwd(self, dy, y, dx, n, act):
-            self._log("act_bwd", self.loc(dy), self.loc(y), self.loc(dx), n, act) if self.on else None
-            super().act_bwd(dy, y, dx, n, act)
-
-        def permute4(self, src, dst, dims, strides, accumulate=False):
-            self._log("permute4", self.loc(src), self.loc(dst), tuple(dims), tuple(strides), bool(accumulate)) if self.on else None
-            super().permute4(src, dst, dims, strides, accumulate)
-
-        def layernorm_fwd(self, x, gamma_, beta, y, mean, rstd, rows, C, eps=1e-5):
-            self._log("layernorm_fwd", self.loc(x), self.loc(y), rows, C) if self.on else None
-            super().layernorm_fwd(x, gamma_, beta, y, mean, rstd, rows, C, eps)
-
-        def layernorm_bwd(self, dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C):
-            self._log("layernorm_bwd", self.loc(dy), self.loc(x), self.loc(dx), dgamma is not None, rows, C) if self.on else None
-            super().layernorm_bwd(dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C)
-
-        def build_concat(self, dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld=None):
-            L = self.loc
-            self._log("build_concat", L(dst), L(A), L(ia), ga, L(Bm), L(ib), gb, S, B, ld) if self.on else None
-            super().build_concat(dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld)
-
-        def gather_add_cols(self, dst, src, idx, S, T, B, g, W, col0, init=False):
-            self._log("gather_add_cols", self.loc(dst), self.loc(src), self.loc(idx), S, T, B, g, W, col0) if self.on else None
-            super().gather_add_cols(dst, src, idx, S, T, B, g, W, col0, init)
-
-        def colsum(self, x, rows, cols, ld, out, accumulate=False):
-            self._log("colsum", self.loc(x), rows, cols, ld, self.loc(out)) if self.on else None
-            super().colsum(x, rows, cols, ld, out, accumulate)
-
-        def mse_plain(self, pred, x, tgt, coef, G, E, d_pred, partial):
-            self._log("mse_plain", self.loc(pred), self.loc(x), self.loc(tgt), G, E) if self.on else None
-            super().mse_plain(pred, x, tgt, coef, G, E, d_pred, partial)
-
-    return RecordingKernels
+    def launch(self, op, args):
+        if op != "gemm" or not (self.on and self.rerun):
+            return super().launch(op, args)
+        C = args["C"]
+        torch.cuda.synchronize()
+        C0 = C.clone()
+        super().launch(op, args)
+        torch.cuda.synchronize()
+        req, plain = copy.copy(self), copy.copy(self)
+        req.gemm_flags, plain.gemm_flags = TF32_FLAG | TF32_REQUIRE, 0
+        C1, C2 = C0.clone(), C0.clone()
+        try:
+            CudaKernels.gemm(**{**args, "self": req, "C": C1})
+            ran = True
+        except KernelError:
+            ran = False
+        CudaKernels.gemm(**{**args, "self": plain, "C": C2})
+        torch.cuda.synchronize()
+        self.reruns.append((ran, ran and torch.equal(C1, C), torch.equal(C2, C)))
 
 
 def _recorded_step(T, B, optkw, adt, rerun=False):
-    opt, probs, plan, x, eps = _inputs(T, B, optkw)
-    eng = _engine(_recording_class()("cuda", rerun=rerun), opt, adt)
-    _watch(eng)
-    xd = x.cuda()
-    eng.K.loc = _Locator(eng, xd)
-    losses = eng.step(xd, probs=probs, eps=eps.cuda())
-    torch.cuda.synchronize()
+    rec = MlpRecording("cuda", rerun=rerun)
+
+    def prepare(eng, x):   # eng.K is the engine's view of rec (CudaKernels.with_mode): same logs, its own flags
+        _watch(eng)
+        eng.K.loc = _Locator(eng, x)
+    plan, (losses, _, _) = run_step(TrainEngineMLP, CFG, optkw, rec, T, B, _np_seed(T, optkw), act_dtype=adt, prepare=prepare)
     assert np.all(np.isfinite(losses))
-    return plan, eng
+    return plan, rec
 
 
 LIST_CASES = [("C5-bf16", BENCH_OPT, torch.bfloat16, C5["B"]), ("C5-fp32", BENCH_OPT, torch.float32, C5["B"]),
@@ -250,10 +169,10 @@ def test_launch_list_matches_an_eager_step(case):
     """The derived list equals, call for call and in order, the backbone launches of one eager step (the recurrent phase
     muted): shapes, flags, pitches, and the buffer and offset of every operand."""
     name, optkw, adt, B = case
-    plan, eng = _recorded_step(C5["T"], B, optkw, adt)
+    plan, rec = _recorded_step(C5["T"], B, optkw, adt)
     if optkw is SKIP_OPT:
         assert len(set(plan.skip_src)) >= 3 and plan.has_cpc
-    got = eng.K.calls
+    got = rec.calls
     derived = backbone_launches(plan, B)
     want = [key(e) for e in derived]
     for i, (g, w) in enumerate(zip(got, want)):
@@ -268,9 +187,9 @@ def test_dispatch_of_every_c5_gemm():
     """Each fp32 GEMM of the bf16-mode C5 step, rerun on its real operands: where the list says tf32 it must run on the TF32
     kernel when a fallback is an error, bit-identically to the step; where it says simt it must be refused there, and a rerun
     with flags 0 (the exact kernel) must be bit-identical."""
-    plan, eng = _recorded_step(C5["T"], C5["B"], BENCH_OPT, torch.bfloat16, rerun=True)
+    plan, rec = _recorded_step(C5["T"], C5["B"], BENCH_OPT, torch.bfloat16, rerun=True)
     derived = [e for e in backbone_launches(plan, C5["B"]) if e["op"] == "gemm"]
-    reruns = eng.K.reruns
+    reruns = rec.reruns
     assert len(reruns) == len(derived)
     n_tf32 = 0
     for e, (ran, same_req, same_plain) in zip(derived, reruns):
@@ -352,12 +271,6 @@ def _run_gemm(K, e, gen, tf32, values="randn"):
     assert (Cbuf[~mask] == SENTINEL).all(), f"{e['name']}: elements outside the output segment were written"
     ref, absref = gemm_ref64(Abuf[e["A"][1]:], Bbuf[e["B"][1]:], M, N, Kd, e["a_mn"], e["b_mn"], e["lda"], e["ldb"], bias=bias, c0=c0)
     return Cv, ref, absref, bias, c0
-
-
-@pytest.fixture(scope="module")
-def K():
-    from p2pvg_b200._lib import CudaKernels
-    return CudaKernels("cuda")
 
 
 @pytest.mark.parametrize("e,tf32", DISTINCT, ids=[f"{e['name'].replace(' ', '_')}-{e['M']}x{e['N']}x{e['K']}-"
@@ -487,7 +400,7 @@ def test_permute4_copy_and_sum(K):
 def _skip_plan():
     T = C5["T"]
     opt = O.default_opt(**SKIP_OPT)
-    p = StepPlan(T, np.random.RandomState(_skip_seed(T)).uniform(0, 1, T - 1), opt)
+    p = StepPlan(T, np.random.RandomState(skip_seed(T)).uniform(0, 1, T - 1), opt)
     assert len(set(p.skip_src)) >= 3
     return p
 
@@ -530,156 +443,93 @@ def test_build_concat_skipsel(K):
 
 # ------------------------------------------------------------------ E. audit of real steps
 
-def _make_audit_class():
-    from p2pvg_b200._lib import CudaKernels
+class MlpAudit(AuditKernels):
+    """AuditKernels for an mlp step: GEMMs of every dtype on the kernel mlp_ref names, act_fwd / act_bwd, permute4,
+    gather_add_cols, build_concat and LayerNorm.  GEMMs outside the backbone methods (`on` unset) are the recurrent ones."""
+    REPORT_GEMMS_ONLY = True
+    GEMM_PROBE_K = 4096
+    GEMM_PROBE_ACCUMULATING = False
 
-    class AuditKernels(CudaKernels):
-        """CudaKernels whose GEMMs (every dtype), act_fwd / act_bwd, permute4, gather_add_cols, build_concat and LayerNorm
-        launches are each checked against float64 on their own operands right after they run (device synchronised around each
-        call; inputs a call overwrites are cloned first; nothing the step reads is changed)."""
+    def __init__(self, *a, **kw):
+        super().__init__(*a, **kw)
+        self.on, self.eng = False, None
 
-        def __init__(self, *a, **kw):
-            super().__init__(*a, **kw)
-            self.log, self.seen, self.skip_reads = [], set(), []
-            self.on, self.eng = False, None
-            self._sms = sm_count()
+    def _is(self, t, name):
+        b = self.eng._bufs.get(name) if self.eng is not None else None
+        return b is not None and b.data_ptr() == t.data_ptr()
 
-        def _rec(self, what, v, worst):
-            self.log.append((what, v, worst))
-            self.seen.add(v)
+    def gemm_bound(self, A, B, M, N, K, a_mn, b_mn, lda, ldb, extra):
+        if A.dtype == torch.bfloat16:
+            s = gemm_tc_tiles(M, N, K, self._sms)
+            return alpha_for(s.kb_per_split * 64 + 16 * s.splits), "tc"
+        kern = kernel_for(M, N, K, a_mn, b_mn, lda, ldb, A.data_ptr() % 16 // 4, B.data_ptr() % 16 // 4, bool(self.gemm_flags & TF32_FLAG))
+        return gemm_alpha(K, kern, extra), kern
 
-        def _is(self, t, name):
-            b = self.eng._bufs.get(name) if self.eng is not None else None
-            return b is not None and b.data_ptr() == t.data_ptr()
+    def gemm_variant(self, A, kern, a_mn, b_mn, accumulate, bias, strided):
+        v = ("gemm", kern if isinstance(kern, str) else kern[0], a_mn, b_mn, bool(accumulate), bias is not None, strided)
+        return v if self.on else ("gemm-recurrent", A.dtype, v[1])
 
-        def gemm(self, A, B, C, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldc=None, accumulate=False, bias=None,
-                 addend=None, ldd=None):
-            torch.cuda.synchronize()
-            lda_ = lda if lda is not None else (M if a_mn else K)
-            ldb_ = ldb if ldb is not None else (N if b_mn else K)
-            ldc_ = ldc if ldc is not None else N
-            ldd_ = ldd if ldd is not None else N
-            cv = C.as_strided((M, N), (ldc_, 1))
-            c0 = cv.clone() if accumulate else None
-            super().gemm(A, B, C, M, N, K, a_mn, b_mn, lda, ldb, ldc, accumulate, bias, addend, ldd)
-            torch.cuda.synchronize()
-            extra = int(bias is not None) + int(addend is not None) + int(accumulate)
-            if A.dtype == torch.bfloat16:
-                s = gemm_tc_tiles(M, N, K, self._sms)
-                alpha, kern = alpha_for(s.kb_per_split * 64 + 16 * s.splits), "tc"
-            else:
-                kern = kernel_for(M, N, K, a_mn, b_mn, lda_, ldb_, A.data_ptr() % 16 // 4, B.data_ptr() % 16 // 4,
-                                  bool(self.gemm_flags & TF32_FLAG))
-                alpha = gemm_alpha(K, kern, extra)
-            dv = addend.as_strided((M, N), (ldd_, 1)) if addend is not None else None
-            w, step = 0.0, max(1, (1 << 22) // max(N, 1))
-            for m0 in range(0, M, step):
-                m1 = min(M, m0 + step)
-                ref, absref = gemm_ref64(A, B, M, N, K, a_mn, b_mn, lda_, ldb_, bias=bias, addend=dv[m0:m1] if dv is not None else None,
-                                         c0=c0[m0:m1] if c0 is not None else None, rows=(m0, m1))
-                w = max(w, assert_within(cv[m0:m1], ref, absref, K, C.dtype, alpha=alpha, quiet=True,
-                                         name=f"audit gemm {M}x{N}x{K} {A.dtype} a_mn={a_mn} b_mn={b_mn} on {kern} rows {m0}"))
-            if K >= 4096 and C.dtype == torch.float32 and not accumulate:
-                # weight gradients: cancelling sums, so the same launch on the 0 / 1 pattern of the operands must be exact
-                A01, B01 = (A > 0).to(A.dtype), (B > 0).to(B.dtype)
-                probe = torch.full((M, N), NAN, device=C.device)
-                super().gemm(A01, B01, probe, M, N, K, a_mn, b_mn, lda, ldb)
-                assert_exact(probe, gemm_ref64(A01, B01, M, N, K, a_mn, b_mn, lda_, ldb_)[0], K, f"audit gemm {M}x{N}x{K} 0/1 probe")
-            v = ("gemm", kern if isinstance(kern, str) else kern[0], a_mn, b_mn, bool(accumulate), bias is not None, ldc_ != N)
-            self._rec(f"gemm {M}x{N}x{K}", v if self.on else ("gemm-recurrent", A.dtype, v[1]), w)
+    def act_fwd(self, x, n, act):
+        torch.cuda.synchronize()
+        x0 = x[:n].clone()
+        self._sync("act_fwd", x, n, act)
+        ref, err = act_fwd_ref(x0, act)
+        self._rec(f"act_fwd {act} n={n}", ("act_fwd", act), bound_check(x[:n], ref, err + (TINY if act != ACT_RELU else 0), f"audit act_fwd {act}"))
 
-        def act_fwd(self, x, n, act):
-            torch.cuda.synchronize()
-            x0 = x[:n].clone()
-            super().act_fwd(x, n, act)
-            torch.cuda.synchronize()
-            ref, err = act_fwd_ref(x0, act)
-            self._rec(f"act_fwd {act} n={n}", ("act_fwd", act), bound_check(x[:n], ref, err + (TINY if act != ACT_RELU else 0), f"audit act_fwd {act}"))
+    def act_bwd(self, dy, y, dx, n, act):
+        torch.cuda.synchronize()
+        d0, y0 = dy[:n].clone(), y[:n].clone()
+        self._sync("act_bwd", dy, y, dx, n, act)
+        ref, err = act_bwd_ref(d0, y0, act)
+        aliased = dy.data_ptr() == dx.data_ptr()
+        self._rec(f"act_bwd {act} n={n}", ("act_bwd", act, aliased),
+                  bound_check(dx[:n], ref, err + (TINY if act != ACT_RELU else 0), f"audit act_bwd {act}"))
 
-        def act_bwd(self, dy, y, dx, n, act):
-            torch.cuda.synchronize()
-            d0, y0 = dy[:n].clone(), y[:n].clone()
-            super().act_bwd(dy, y, dx, n, act)
-            torch.cuda.synchronize()
-            ref, err = act_bwd_ref(d0, y0, act)
-            aliased = dy.data_ptr() == dx.data_ptr()
-            self._rec(f"act_bwd {act} n={n}", ("act_bwd", act, aliased),
-                      bound_check(dx[:n], ref, err + (TINY if act != ACT_RELU else 0), f"audit act_bwd {act}"))
+    def permute4(self, src, dst, dims, strides, accumulate=False):
+        torch.cuda.synchronize()
+        n = dims[0] * dims[1] * dims[2] * dims[3]
+        d0 = dst.reshape(-1)[:n].clone() if accumulate else None
+        self._sync("permute4", src, dst, dims, strides, accumulate)
+        s = src.as_strided(tuple(dims), tuple(strides)).reshape(-1).double()
+        got = dst.reshape(-1)[:n]
+        if accumulate:
+            ref = d0.double() + s
+            w = bound_check(got, ref, U * ref.abs() if dst.dtype == torch.float32 else 2.0 ** -8 * ref.abs(), "audit permute4 sum")
+        else:
+            ref = s.to(dst.dtype).double()
+            w = bound_check(got, ref, torch.zeros_like(ref), "audit permute4 copy")
+        self._rec(f"permute4 {tuple(dims)}", ("permute4", bool(accumulate)), w)
 
-        def permute4(self, src, dst, dims, strides, accumulate=False):
-            torch.cuda.synchronize()
-            n = dims[0] * dims[1] * dims[2] * dims[3]
-            d0 = dst.reshape(-1)[:n].clone() if accumulate else None
-            super().permute4(src, dst, dims, strides, accumulate)
-            torch.cuda.synchronize()
-            s = src.as_strided(tuple(dims), tuple(strides)).reshape(-1).double()
-            got = dst.reshape(-1)[:n]
-            if accumulate:
-                ref = d0.double() + s
-                w = bound_check(got, ref, U * ref.abs() if dst.dtype == torch.float32 else 2.0 ** -8 * ref.abs(), "audit permute4 sum")
-            else:
-                ref = s.to(dst.dtype).double()
-                w = bound_check(got, ref, torch.zeros_like(ref), "audit permute4 copy")
-            self._rec(f"permute4 {tuple(dims)}", ("permute4", bool(accumulate)), w)
+    def gather_add_cols(self, dst, src, idx, S, T, B, g, W, col0, init=False):
+        torch.cuda.synchronize()
+        d0 = dst.reshape(-1)[:T * B * g].clone()
+        self._sync("gather_add_cols", dst, src, idx, S, T, B, g, W, col0, init)
+        if self._is(src, "dskipsel"):
+            self.skip_reads.append(("gather_add_cols", col0, idx.tolist()[:S]))
+        check_gather_add_cols(dst, d0, src, idx, S, T, B, g, W, col0, init)
+        self._rec(f"gather_add_cols W={W} col0={col0}", ("gather_add_cols", self._is(src, "dskipsel")), 0.0)
 
-        def gather_add_cols(self, dst, src, idx, S, T, B, g, W, col0, init=False):
-            torch.cuda.synchronize()
-            d0 = dst.reshape(-1)[:T * B * g].clone()
-            super().gather_add_cols(dst, src, idx, S, T, B, g, W, col0, init)
-            torch.cuda.synchronize()
-            if self._is(src, "dskipsel"):
-                self.skip_reads.append(("gather_add_cols", col0, idx.tolist()[:S]))
-            check_gather_add_cols(dst, d0, src, idx, S, T, B, g, W, col0, init)
-            self._rec(f"gather_add_cols W={W} col0={col0}", ("gather_add_cols", self._is(src, "dskipsel")), 0.0)
+    def build_concat(self, dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld=None):
+        self._sync("build_concat", dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld)
+        ld_ = ld if ld is not None else ga + gb + 2
+        if self._is(dst, "skipsel"):
+            self.skip_reads.append(("build_concat", 0, ia.tolist()[:S]))
+            self.skip_reads.append(("build_concat", ga, ib.tolist()[:S]))
+        ref = build_concat_ref(A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld_)
+        assert torch.equal(dst.reshape(-1)[:S * B * ld_], ref), f"audit build_concat S={S} ld={ld_}"
+        self._rec(f"build_concat ld={ld_}", ("build_concat", self._is(dst, "skipsel")), 0.0)
 
-        def build_concat(self, dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld=None):
-            super().build_concat(dst, A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld)
-            torch.cuda.synchronize()
-            ld_ = ld if ld is not None else ga + gb + 2
-            if self._is(dst, "skipsel"):
-                self.skip_reads.append(("build_concat", 0, ia.tolist()[:S]))
-                self.skip_reads.append(("build_concat", ga, ib.tolist()[:S]))
-            ref = build_concat_ref(A, ia, ga, Bm, ib, gb, tuc, dt, S, B, ld_)
-            assert torch.equal(dst.reshape(-1)[:S * B * ld_], ref), f"audit build_concat S={S} ld={ld_}"
-            self._rec(f"build_concat ld={ld_}", ("build_concat", self._is(dst, "skipsel")), 0.0)
+    def layernorm_fwd(self, x, gamma_, beta, y, mean, rstd, rows, C, eps=1e-5):
+        self._sync("layernorm_fwd", x, gamma_, beta, y, mean, rstd, rows, C, eps)
+        check_layernorm_fwd(x, gamma_, beta, y, mean, rstd, rows, C, eps)
+        self._rec(f"layernorm_fwd rows={rows}", ("layernorm_fwd",), 0.0)
 
-        def layernorm_fwd(self, x, gamma_, beta, y, mean, rstd, rows, C, eps=1e-5):
-            super().layernorm_fwd(x, gamma_, beta, y, mean, rstd, rows, C, eps)
-            torch.cuda.synchronize()
-            check_layernorm_fwd(x, gamma_, beta, y, mean, rstd, rows, C, eps)
-            self._rec(f"layernorm_fwd rows={rows}", ("layernorm_fwd",), 0.0)
-
-        def layernorm_bwd(self, dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C):
-            torch.cuda.synchronize()
-            d0 = dy.reshape(-1)[:rows * C].clone()
-            super().layernorm_bwd(dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C)
-            torch.cuda.synchronize()
-            check_layernorm_bwd(d0, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C)
-            self._rec(f"layernorm_bwd rows={rows}", ("layernorm_bwd", dgamma is not None), 0.0)
-
-    return AuditKernels
-
-
-def _plain_step(T, B, optkw, adt=torch.bfloat16, use_graph=False):
-    from p2pvg_b200._lib import CudaKernels
-    opt, probs, plan, x, eps = _inputs(T, B, optkw)
-    eng = _engine(CudaKernels("cuda"), opt, adt)
-    xd, ed = x.cuda(), eps.cuda()
-    if use_graph:
-        from tests.test_measured_gpu import restore, snapshot
-        snap = snapshot(eng)
-        for _ in range(2):
-            eng.step(xd, probs=probs, eps=ed, use_graph=True)
-        restore(eng, snap)
-        losses = eng.step(xd, probs=probs, eps=ed, use_graph=True)
-        assert any(v != "warm" for v in eng._graphs.values()), "the step was not graph-replayed"
-    else:
-        losses = eng.step(xd, probs=probs, eps=ed)
-    out = _results(eng, losses)
-    assert eng.concurrent
-    del eng
-    _release()
-    return out
+    def layernorm_bwd(self, dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C):
+        torch.cuda.synchronize()
+        d0 = dy.reshape(-1)[:rows * C].clone()
+        self._sync("layernorm_bwd", dy, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C)
+        check_layernorm_bwd(d0, x, mean, rstd, gamma_, dx, dgamma, dbeta, rows, C)
+        self._rec(f"layernorm_bwd rows={rows}", ("layernorm_bwd", dgamma is not None), 0.0)
 
 
 AUDIT_CASES = [("C5_bench_options", BENCH_OPT, C5["B"]), ("skip_lfs_B32", SKIP_OPT, 32)]
@@ -691,39 +541,31 @@ def test_audit_mlp_step(case):
     must occur, the skip matrix must be built and its gradients gathered through plan.skip_src, and losses, gradients and
     parameters must equal (torch.equal) the same step on plain CudaKernels with its concurrent lanes."""
     name, optkw, B = case
-    T = C5["T"]
-    plain = _plain_step(T, B, optkw)
-    opt, probs, plan, x, eps = _inputs(T, B, optkw)
-    eng = _engine(_make_audit_class()("cuda"), opt, torch.bfloat16)
-    eng.K.eng = eng
-    _watch(eng)
-    losses = eng.step(x.cuda(), probs=probs, eps=eps.cuda())
-    audited = _results(eng, losses)
-    log, seen, reads = eng.K.log, eng.K.seen, eng.K.skip_reads
-    del eng
-    _release()
-    want = {gemm_variant(e, entry_kernel(e, True)) for e in backbone_launches(plan, B) if e["op"] == "gemm"}
-    want |= {("act_fwd", ACT_RELU), ("act_fwd", ACT_TANH), ("act_bwd", ACT_RELU, True), ("act_bwd", ACT_RELU, False),
-             ("act_bwd", ACT_TANH, False), ("permute4", False), ("permute4", True), ("gather_add_cols", True),
-             ("build_concat", True), ("layernorm_fwd",), ("layernorm_bwd", True), ("layernorm_bwd", False)}
-    missing = want - seen
-    assert not missing, f"launch variants that did not occur in the step: {sorted(missing, key=str)}"
-    rec = {v for v in seen if v[0] == "gemm-recurrent"}
+    audit = MlpAudit("cuda")
+
+    def expect(plan):
+        want = {gemm_variant(e, entry_kernel(e, True)) for e in backbone_launches(plan, B) if e["op"] == "gemm"}
+        want |= {("act_fwd", ACT_RELU), ("act_fwd", ACT_TANH), ("act_bwd", ACT_RELU, True), ("act_bwd", ACT_RELU, False),
+                 ("act_bwd", ACT_TANH, False), ("permute4", False), ("permute4", True), ("gather_add_cols", True),
+                 ("build_concat", True), ("layernorm_fwd",), ("layernorm_bwd", True), ("layernorm_bwd", False)}
+        # the skip matrix [h1 | h2 | ..] is built for the S + 1 decoder calls, its gradients gathered over the S reconstructions
+        src = plan.skip_src
+        return want, [("build_concat", 0, src[:plan.S + 1]), ("build_concat", H, src[:plan.S + 1]),
+                      ("gather_add_cols", 0, src[:plan.S]), ("gather_add_cols", H, src[:plan.S])]
+
+    def watched(eng, x):
+        eng.K.eng = eng
+        _watch(eng)
+    audit_step(TrainEngineMLP, CFG, optkw, C5["T"], B, audit, expect, name, prepare=watched)
+    rec = {v for v in audit.seen if v[0] == "gemm-recurrent"}
     assert ("gemm-recurrent", torch.float32, "tf32") in rec and ("gemm-recurrent", torch.bfloat16, "tc") in rec, rec
-    assert sorted(r[:2] for r in reads) == [("build_concat", 0), ("build_concat", H), ("gather_add_cols", 0), ("gather_add_cols", H)]
-    for what, col, idx in reads:
-        n = plan.S + 1 if what == "build_concat" else plan.S
-        assert idx == plan.skip_src[:n], f"{what} (column {col}) read {idx}, the plan's skip_src is {plan.skip_src}"
-    worst = max((w for _, v, w in log if v[0].startswith("gemm")), default=0.0)
-    print(f"[audit] {name}: {len(log)} launches checked, worst GEMM error/bound {worst:.3g}")
-    _assert_equal_steps(plain, audited, f"{name} audited vs plain")
 
 
 def test_graph_replay_equals_eager_c5():
     """The C5 step replayed from a captured CUDA graph (restored to the initial state in place) equals the eager step."""
-    eager = _plain_step(C5["T"], C5["B"], BENCH_OPT)
-    graph = _plain_step(C5["T"], C5["B"], BENCH_OPT, use_graph=True)
-    _assert_equal_steps(eager, graph, "C5 graph replay vs eager")
+    eager, graph = (run_step(TrainEngineMLP, CFG, BENCH_OPT, CudaKernels("cuda"), C5["T"], C5["B"], 0, use_graph=g,
+                             prepare=assert_concurrent)[1] for g in (False, True))
+    assert_equal_steps(eager, graph, "C5 graph replay vs eager")
 
 
 # ------------------------------------------------------------------ F. the whole C5 step against the float64 oracle
@@ -732,7 +574,7 @@ def test_graph_replay_equals_eager_c5():
 def oracle_c5():
     """The oracle's C5 step (reference models/p2p_model.py, Mode A) in float64 on the device, from the engine's initial weights
     and inputs."""
-    opt, probs, plan, x, eps = _inputs(C5["T"], C5["B"], BENCH_OPT)
+    opt, probs, plan, x, eps = step_inputs(CFG, BENCH_OPT, C5["T"], C5["B"], 0)
     state = {m: {k: v.cuda() for k, v in sd.items()} for m, sd in O.build_state(CFG, seed=1, dtype=torch.float64).items()}
     adam = {m: O.new_adam_state(state[m]) for m in O.MODULES}
     t0 = time.time()
@@ -741,7 +583,7 @@ def oracle_c5():
     print(f"[oracle] float64 C5 step on the device: {time.time() - t0:.1f} s")
     grads = {m: {k: g.cpu() for k, g in gm.items()} for m, gm in ref["grads"].items()}
     del state, adam
-    _release()
+    release()
     return ref["losses"], grads
 
 
@@ -753,11 +595,10 @@ def test_c5_step_vs_float64_oracle(oracle_c5, mode):
     """Losses and every gradient tensor of one C5 step against the float64 oracle: fp32 mode to rtol 1e-4 and cosine
     >= 1 - 1e-5 (the thresholds of test_mlp_gpu.py), bf16 mode to rtol 1e-2, cosine >= 0.995 and norm ratio within 5 %
     (test_measured_gpu.py's thresholds for h36m at rnn_size 512)."""
-    from p2pvg_b200._lib import CudaKernels
     name, adt, rtol, mincos, norm_tol = mode
     ref_losses, ref_grads = oracle_c5
-    opt, probs, plan, x, eps = _inputs(C5["T"], C5["B"], BENCH_OPT)
-    eng = _engine(CudaKernels("cuda"), opt, adt)
+    opt, probs, plan, x, eps = step_inputs(CFG, BENCH_OPT, C5["T"], C5["B"], 0)
+    eng = TrainEngineMLP(O.build_state(CFG, seed=1), CFG, opt, CudaKernels("cuda"), act_dtype=adt)
     got = eng.step(x.cuda(), probs=probs, eps=eps.cuda())
     torch.cuda.synchronize()
     np.testing.assert_allclose(got, np.array(ref_losses), rtol=rtol, atol=1e-7, err_msg=name)

@@ -18,8 +18,8 @@ import math
 import pytest
 import torch
 
-from tests.tc_schedule import (alpha_for, assert_multi_round, assert_within, cdiv, conv_ref64, conv_tiles, gemm_tc_tiles, ref64,
-                               sm_count)
+from tests.tc_schedule import (alpha_for, assert_multi_round, assert_within, cdiv, conv_ref64, conv_tiles, fit, gemm_tc_tiles,
+                               image_slices, ref64, rows_by_tile, sm_count)
 
 pytestmark = pytest.mark.gpu
 
@@ -36,18 +36,6 @@ def K():
 @pytest.fixture(scope="module")
 def sms():
     return sm_count()
-
-
-def fit(cands, sched, need_n_change=True, min_tiles=None):
-    """The first candidate shape whose schedule meets the multi-round invariants (fails loudly if none does)."""
-    for shape in cands:
-        s = sched(*shape)
-        try:
-            assert_multi_round(s, need_n_change, min_tiles)
-        except AssertionError:
-            continue
-        return shape, s
-    raise AssertionError("no candidate shape reaches the rounds this case is meant to test on this device")
 
 
 def randn(*shape, scale=1.0, dtype=torch.float32):
@@ -184,17 +172,6 @@ def conv_locate(kind, H, s):
     return loc
 
 
-def image_slices(N, HW, unit, s, sms):
-    """Three tile-aligned image ranges (first, middle, last round) whose launch has at most `sms` tiles."""
-    tiles_per_img = lambda n: cdiv(n * HW, s.BM) * s.tiles_n * s.phases
-    ni = unit
-    while ni + unit <= N and tiles_per_img(ni + unit) <= sms:
-        ni += unit
-    mid = (N // 2) // unit * unit
-    last = -(-(N - ni) // unit) * unit
-    return [(0, ni), (mid, min(N, mid + ni)), (last, N)]
-
-
 CONV_CASES = [
     # id, kind, H (small map), Ck, Cn candidates, starting N, image step, kind-2 images per addend group
     ("k0_hw256_cn576", 0, 16, 128, (576, 640), 40, 1, 0),        # 2 tiles per image; Cn tail: the last column tile is half
@@ -311,20 +288,6 @@ STAT_CASES = [
     ("k2_hw256_cn256", 2, 16, 128, (256, 640), 25, 5),
     ("k2_hw16_bn64", 2, 4, 256, (64,), 800, 16),
 ]
-
-
-def rows_by_tile(out, kind, N, H, Cn, tiles_m):
-    """The stored output as [tiles_m * phases, 128, Cn] float64: the rows each statistics partial row covers (rows past the
-    end are zeros).  Kind 2: partial row (mt, ph) covers phase ph's output pixels of the small-map pixels of tile mt."""
-    o = out.double()
-    if kind == 2:
-        o = o.view(N, H, 2, H, 2, Cn).permute(2, 4, 0, 1, 3, 5).reshape(4, N * H * H, Cn)
-    else:
-        o = o.reshape(1, N * H * H, Cn)
-    P = o.shape[0]
-    pad = torch.zeros(P, tiles_m * 128, Cn, dtype=torch.float64, device=o.device)
-    pad[:, :o.shape[1]] = o
-    return pad.view(P, tiles_m, 128, Cn).transpose(0, 1).reshape(tiles_m * P, 128, Cn)
 
 
 @pytest.mark.parametrize("cdt", [torch.bfloat16, torch.float32])

@@ -7,7 +7,7 @@ runs at twice the map size of its vgg_64 counterpart: the 64-channel layers at 1
 
   A. the launch lists tests/vgg_ref.py derives, against the conv_gemm launches one eager bf16 step records, at this shape and
      at C3 (vgg_64, T = 30, B = 128);
-  B. every distinct kind-3 / kind-5 launch at its vgg_128 shape (tests/test_vgg_launches_gpu.py run_conv): no element left
+  B. every distinct kind-3 / kind-5 launch at its vgg_128 shape (tests/vgg_ref.py run_conv): no element left
      unwritten, float64 on slices of the first, middle and last round (the middle one straddling a group of B images),
      bit-identity against a launch of just those images, per-(image, channel) sums of the whole output, every fused
      statistics row and the finalized statistics;
@@ -21,7 +21,6 @@ runs at twice the map size of its vgg_64 counterpart: the 64-channel layers at 1
      checked as it runs, coverage of the derived list, skip addends read through plan.skip_src, and a step bit-identical to
      the unaudited step with its concurrent lanes and to a CUDA-graph replay of it.
 """
-import inspect
 import math
 
 import numpy as np
@@ -29,45 +28,23 @@ import pytest
 import torch
 
 from oracle import p2p_oracle as O
+from p2pvg_b200._lib import CudaKernels
 from p2pvg_b200.engine import ACT_LRELU, StepPlan
+from p2pvg_b200.engine_vgg import TrainEngineVGG
 from p2pvg_b200.layouts import up8
-from tests.dcgan_ref import EPS, bn_group_ref64
-from tests.tc_schedule import BETA, assert_within, gemm_tc_tiles, sm_count
-from tests.test_dcgan_launches_gpu import ALPHA_BN, _bn_inputs, _stats
-from tests.test_vgg_launches_gpu import (AUDIT_CASES, BENCH_OPT, _dedup, _release, _skip_seed, assert_equal_steps, audit_step, randn, run_conv,
-                                         run_end_gemms, run_im2col3_col2im3, run_maxpool, run_skip_index, run_upsample, run_wgrad,
-                                         vgg_step, wgrad_classes)
-from tests.vgg_ref import (assert_exact, backward_launches, binary01, bound_check, finalize_ref, forward_launches, gemm_ref64,
-                           launch_key)
+from tests.launch_audit import K, memory_per_test, sms  # noqa: F401  (fixtures)
+from tests.launch_audit import (ALPHA_BN, BENCH_OPT, NAN, RecordingKernels, assert_equal_steps, bn_inputs, bn_stats, randn, run_step,
+                                skip_seed)
+from tests.ref64 import EPS, assert_exact, binary01, bn_group_ref64, bound_check, finalize_ref, gemm_ref64
+from tests.tc_schedule import BETA, assert_within, gemm_tc_tiles
+from tests.vgg_ref import (AUDIT_CASES, audit_vgg_step, backward_launches, distinct_convs, forward_launches, launch_key, run_conv,
+                           run_end_gemms, run_im2col3_col2im3, run_maxpool, run_skip_index, run_upsample, run_wgrad, vgg_cfg,
+                           wgrad_classes)
 
 pytestmark = pytest.mark.gpu
 
 SHAPES = {"vgg128": dict(T=30, B=32, W0=128), "C3": dict(T=30, B=128, W0=64)}
 V128 = SHAPES["vgg128"]
-NAN = float("nan")
-
-
-@pytest.fixture(scope="module")
-def K():
-    from p2pvg_b200._lib import CudaKernels
-    return CudaKernels("cuda")
-
-
-@pytest.fixture(autouse=True)
-def memory_per_test(request):
-    import time
-    if torch.cuda.is_available():
-        torch.cuda.reset_peak_memory_stats()
-        t0 = time.time()
-    yield
-    if torch.cuda.is_available():
-        _release()
-        print(f"\n[memory] {request.node.name}: {time.time() - t0:.1f} s, peak {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB")
-
-
-@pytest.fixture(scope="module")
-def sms():
-    return sm_count()
 
 
 def bench_plan(c):
@@ -83,27 +60,15 @@ def launches(name):
 
 # ------------------------------------------------------------------ A. the launch lists against a recorded step
 
-def _recording_class():
-    from p2pvg_b200._lib import CudaKernels
+def _conv_key(k, x):
+    assert x["H"] == x["W"]
+    return (x["kind"], x["N"], x["H"], x["Ck"], x["Cn"], x["Cm"], x["bias"] is not None,
+            x["addend"].dtype if x["addend"] is not None else None, x["imgs_per_group"], x["stat_partial"] is not None)
 
-    class RecordingKernels(CudaKernels):
-        """CudaKernels that logs what every conv_gemm launch is (vgg_ref.launch_key), then calls through."""
 
-        def __init__(self, *a, **kw):
-            super().__init__(*a, **kw)
-            self.calls = []
-
-        def conv_gemm(self, *a, **kw):
-            x = inspect.signature(CudaKernels.conv_gemm).bind(None, *a, **kw)
-            x.apply_defaults()
-            x = x.arguments
-            assert x["H"] == x["W"]
-            self.calls.append((x["kind"], x["N"], x["H"], x["Ck"], x["Cn"], x["Cm"], x["bias"] is not None,
-                               x["addend"].dtype if x["addend"] is not None else None, x["imgs_per_group"],
-                               x["stat_partial"] is not None))
-            super().conv_gemm(*a, **kw)
-
-    return RecordingKernels
+class VggRecording(RecordingKernels):
+    """Logs what every conv_gemm launch is (vgg_ref.launch_key)."""
+    RECORD = {"conv_gemm": _conv_key}
 
 
 @pytest.mark.parametrize("name", list(SHAPES))
@@ -113,10 +78,9 @@ def test_launch_list_matches_a_recorded_step(name):
     launches run over S B images (and B for the CPC decode), not over the forward's (S + 1) B."""
     c = SHAPES[name]
     T, B, W0 = c["T"], c["B"], c["W0"]
-    plan, losses, _, eng = vgg_step(_recording_class()("cuda"), BENCH_OPT, T, B, 0, W0)
-    got = eng.K.calls
-    del eng
-    _release()
+    rec = VggRecording("cuda")
+    plan, (losses, _, _) = run_step(TrainEngineVGG, vgg_cfg(W0), BENCH_OPT, rec, T, B, 0)
+    got = rec.calls
     assert np.all(np.isfinite(losses))
     assert (plan.S, plan.nskip, plan.has_cpc) == (29, 1, True)
     fwd, bwd = launches(name)
@@ -130,7 +94,7 @@ def test_launch_list_matches_a_recorded_step(name):
 
 # ------------------------------------------------------------------ B. every distinct kind-3 / kind-5 launch
 
-CONV = _dedup([L for L in sum(launches("vgg128"), []) if L["kind"] != 4])
+CONV = distinct_convs(sum(launches("vgg128"), []))
 
 
 @pytest.mark.parametrize("L", CONV, ids=[f"{L['name'].replace(' ', '_')}-N{L['N']}" for L in CONV])
@@ -240,8 +204,8 @@ def test_bn_forward_at_launch_shape(K, case):
     finalize_ref's bound on sums known within ALPHA_BN, y within one fp32 and one bf16 rounding."""
     cfg, G, R, C, nm = case
     name = f"{cfg} {nm} G={G} R={R} C={C}"
-    raw, gamma, beta, _ = _bn_inputs(G, R, C, seed=G * 7 + C + R)
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    raw, gamma, beta, _ = bn_inputs(G, R, C, seed=G * 7 + C + R)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     y = torch.full_like(raw, NAN)
     K.bn_act(raw, y, st["scale"], st["shift"], G, R, C, ACT_LRELU)
     x, yv = raw.view(G, R, C), y.view(G, R, C)
@@ -263,12 +227,12 @@ def test_bn_forward_at_launch_shape(K, case):
 @pytest.mark.parametrize("case", BN, ids=[f"{c[0]}-{c[4]}-G{c[1]}_R{c[2]}_C{c[3]}" for c in BN])
 def test_bn_bwd_at_launch_shape(K, case):
     """bn_bwd as the step calls it (in place, LeakyReLU slope recomputed from scale / shift) and bn_param_grad, every group
-    against float64 (dcgan_ref.bn_group_ref64): dx within one bf16 rounding, the per-group sums and dgamma / dbeta within
+    against float64 (ref64.bn_group_ref64): dx within one bf16 rounding, the per-group sums and dgamma / dbeta within
     ALPHA_BN of their magnitudes."""
     cfg, G, R, C, nm = case
     name = f"bn_bwd {cfg} {nm} G={G} R={R} C={C}"
-    raw, gamma, beta, gen = _bn_inputs(G, R, C, seed=G * 11 + C + R)
-    st = _stats(K, raw, G, R, C, gamma, beta)
+    raw, gamma, beta, gen = bn_inputs(G, R, C, seed=G * 11 + C + R)
+    st = bn_stats(K, raw, G, R, C, gamma, beta)
     x = raw.view(G, R, C)
     # dy correlated with xhat, so that the xhat term of dx carries weight
     dy = torch.empty_like(raw)
@@ -330,15 +294,13 @@ def test_skip_index_kernels_vgg128(K):
 
 @pytest.mark.parametrize("case", AUDIT_CASES, ids=[c[0] for c in AUDIT_CASES])
 def test_audit_vgg128_step(case):
-    """One eager bf16 vgg_128 step at T = 30, B = 8 with every launch checked as it runs (audit_step: coverage of the derived
-    list, skip addends through plan.skip_src, equal to the plain step), and the plain step equal to a CUDA-graph replay."""
-    from p2pvg_b200._lib import CudaKernels
-    name, optkw, seed = case
+    """One eager bf16 vgg_128 step at T = 30, B = 8 with every launch checked as it runs (vgg_ref.audit_vgg_step: coverage of
+    the derived list, skip addends through plan.skip_src, equal to the plain step), and the plain step equal to a CUDA-graph
+    replay."""
+    name, optkw = case
     T, B = 30, 8
-    eager = audit_step(name, optkw, T, B, seed, W0=128)
-    np_seed = _skip_seed(T) if seed == "search" else 0
-    _, losses, grads, eng = vgg_step(CudaKernels("cuda"), optkw, T, B, np_seed, W0=128, use_graph=True)
-    del eng
-    _release()
-    assert_equal_steps(eager, (losses, grads), f"vgg128 {name}: graph replay vs eager")
+    eager = audit_vgg_step(name, optkw, T, B, W0=128)
+    np_seed = skip_seed(T) if optkw.get("skip_prob") else 0
+    _, graph = run_step(TrainEngineVGG, vgg_cfg(128), optkw, CudaKernels("cuda"), T, B, np_seed, use_graph=True)
+    assert_equal_steps(eager, graph, f"vgg128 {name}: graph replay vs eager")
     print(f"[audit] vgg128 {name}: graph replay equals the eager step")

@@ -1,5 +1,6 @@
 """The vgg_64 and vgg_128 training steps' kernel launches, derived from the engine's layer tables, and the float64 statements
-the launch tests check them against (tests/test_vgg_launches_gpu.py, tests/test_vgg128_launches_gpu.py).
+the launch tests check them against (tests/test_vgg_launches_gpu.py, tests/test_vgg128_launches_gpu.py), with the launch
+checks and the audited step both files run.
 
 `forward_launches` / `backward_launches` walk the backbone's layer tables (VGG_ENC / VGG_DEC for 64x64 frames, VGG_ENC_128 /
 VGG_DEC_128 for 128x128) the way TrainEngineVGG.encode / decode / decoder_backward / encoder_backward do and ask the engine's
@@ -12,18 +13,20 @@ The checkers work in image chunks so that float64 references of C3-sized tensors
   * stat rows / finalize: every fused statistics row against the float64 sums of the stored rows it covers, and the
     finalized BatchNorm statistics per group against float64 statistics of the stored output.
 """
+import math
 import types
 
 import torch
 import torch.nn.functional as F
 
 from p2pvg_b200.engine import TrainEngine
-from p2pvg_b200.engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128
+from p2pvg_b200.engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128, TrainEngineVGG
 from p2pvg_b200.layouts import implicit_shape
-from tests.tc_schedule import BETA, alpha_for, assert_within, cdiv
-from tests.test_tc_schedule_gpu import rows_by_tile
-
-CHUNK = 1 << 25     # elements of one float64 chunk (256 MB)
+from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, addend_index, audit_step, randn, release,
+                                slices_with_boundary)
+from tests.ref64 import (A_STAT, CHUNK, assert_exact, binary01, bound_check, check_finalize_vs_output, finalize_ref,
+                         gemm_ref64)
+from tests.tc_schedule import BETA, alpha_for, assert_within, cdiv, conv_tiles, gemm_tc_tiles, rows_by_tile, sm_count
 
 
 # ------------------------------------------------------------------ the launch list
@@ -240,29 +243,7 @@ def conv3_ref64_elem(kind, a, b, H, Ck, Cn, bias=None, addend_rows=None):
     return ref, absref
 
 
-# ------------------------------------------------------------------ exact reductions
-
-def binary01(shape, p=0.25):
-    """bf16 0 / 1 operand, 1 with probability p.  Products are 0 / 1 and a K-long sum of them is an integer <= K: below 2^24 every
-    fp32 partial sum is exact in any order, so a kernel's result must equal the float64 reference bit for bit."""
-    return (torch.rand(*shape, device="cuda") < p).to(torch.bfloat16)
-
-
-def assert_exact(got, ref, K, name):
-    """The fp32 result of a reduction of 0 / 1 products over K < 2^24 terms equals float64 exactly."""
-    assert K < 1 << 24, f"{name}: K = {K} is too long for exact fp32 integer sums"
-    bad = got.double() != ref
-    if bad.any():
-        i = tuple(int(v) for v in torch.unravel_index(torch.nonzero(bad.flatten())[0, 0], got.shape))
-        raise AssertionError(f"{name}: {int(bad.sum())}/{bad.numel()} elements differ from the exact integer sum, first at {i}: "
-                             f"got {got[i].item():.9g}, exact {ref[i].item():.9g}")
-    print(f"[exact] {name}: K={K}, largest sum {ref.max().item():.0f}, exact")
-
-
 # ------------------------------------------------------------------ fused statistics
-
-A_STAT = 2.0 ** -18   # a statistics row: a fixed-order fp32 tree over 128 stored values (see test_tc_schedule_gpu.py)
-
 
 def check_stat_rows(part, out, N, H, Cn, name=""):
     """Every partial row [tile, Cn, (sum, sum of squares)] against the float64 sums of the (up to 128) stored rows it covers,
@@ -285,63 +266,6 @@ def check_stat_rows(part, out, N, H, Cn, name=""):
     return worst
 
 
-def bound_check(got, ref, bound, name):
-    """|got - ref| <= bound element-wise (float64 ref and bound); returns the worst ratio."""
-    diff = (got.double() - ref).abs()
-    ratio = torch.where(bound > 0, diff / bound.clamp_min(1e-300), torch.where(diff > 0, torch.inf, 0.0))
-    ratio = torch.nan_to_num(ratio, nan=torch.inf)
-    worst = ratio.max().item()
-    if worst > 1.0:
-        i = int(ratio.argmax())
-        raise AssertionError(f"{name}: worst ratio {worst:.3g} at {i}: got {got.flatten()[i].item():.8g}, "
-                             f"ref {ref.flatten()[i].item():.8g}, bound {bound.flatten()[i].item():.3g}")
-    return worst
-
-
-def finalize_ref(s1, s2, m1, R, gamma, beta, eps, a_rel):
-    """Float64 mean / invstd / var_unbiased / scale / shift of groups whose sums are (s1, s2) with magnitudes (m1 = sum|x|,
-    s2 = sum x^2), each sum known within a_rel of its magnitude; returns [(ref, bound)] in the kernel's output order."""
-    E1, E2 = m1 / R, s2 / R
-    m = s1 / R
-    var = (s2 / R - m * m).clamp_min(0.0)
-    g, bt = gamma.double(), beta.double()
-    invstd = 1.0 / torch.sqrt(var + eps)
-    u = 2.0 ** -23
-    d_m = a_rel * E1 + u * m.abs()
-    d_var = 3.0 * a_rel * E2 + u * var
-    d_is = invstd * (0.5 * d_var / (var + eps) * 1.01 + u)
-    sc = g * invstd
-    d_sc = g.abs() * d_is + u * sc.abs()
-    sh = bt - m * sc
-    d_sh = m.abs() * d_sc + sc.abs() * d_m + u * (bt.abs() + (m * sc).abs()) * 2
-    varu = var * R / (R - 1)
-    return [(m, d_m), (invstd, d_is), (varu, d_var * R / (R - 1) + u * varu), (sc, d_sc), (sh, d_sh)]
-
-
-def check_finalize_vs_output(K, part, parts_per_group, out, G, rows_per_group, Cn, name=""):
-    """bn_fwd_finalize_tiles with the engine's parts_per_group against float64 statistics of the stored output."""
-    gamma = torch.rand(Cn, device=out.device) + 0.5
-    beta = torch.randn(Cn, device=out.device)
-    outs = [torch.empty(G * Cn, device=out.device) for _ in range(5)]
-    K.bn_fwd_finalize_tiles(part, parts_per_group, Cn, 1, G, rows_per_group, Cn, gamma, beta, *outs)
-    flat = out.reshape(G, rows_per_group, Cn)
-    s1 = torch.empty(G, Cn, dtype=torch.float64, device=out.device)
-    s2, m1 = torch.empty_like(s1), torch.empty_like(s1)
-    per = max(1, CHUNK // Cn)
-    for g in range(G):
-        a = b = c = 0.0
-        for r0 in range(0, rows_per_group, per):
-            x = flat[g, r0:r0 + per].double()
-            a, b, c = a + x.sum(0), b + (x * x).sum(0), c + x.abs().sum(0)
-        s1[g], s2[g], m1[g] = a, b, c
-    worst = 0.0
-    for got, (ref, bound), nm in zip(outs, finalize_ref(s1, s2, m1, rows_per_group, gamma, beta, 1e-5, A_STAT),
-                                     ("mean", "invstd", "var_unbiased", "scale", "shift")):
-        worst = max(worst, bound_check(got.view(G, Cn), ref, bound, f"{name} finalize {nm}"))
-    print(f"[bound] {name} finalize ({G} groups x {parts_per_group} parts): worst error/bound {worst:.3g}")
-    return worst
-
-
 # ------------------------------------------------------------------ kind 4
 
 def wgrad_ref64(a, b, N, H, Cm, Cn):
@@ -361,34 +285,6 @@ def wgrad_ref64(a, b, N, H, Cm, Cn):
                 dst[:, tap] += xa.t() @ bpa[:, kh:kh + H, kw:kw + H].reshape(-1, Cn)
         del x, bp
     return ref.view(Cm, 9 * Cn), absref.view(Cm, 9 * Cn)
-
-
-# ------------------------------------------------------------------ GEMM (p2pvg_gemm)
-
-def gemm_ref64(A, B, M, N, Kd, a_mn, b_mn, lda, ldb, bias=None, addend=None, ldd=None, c0=None, rows=None):
-    """C = opA(A) opB(B) + bias + addend + c0 in float64 (and over |.|) on strided views of the operands, chunked over M and K.
-    rows = (m0, m1): only those rows of C (addend and c0 are then those rows too)."""
-    Av = A.as_strided((Kd, M), (lda, 1)) if a_mn else A.as_strided((M, Kd), (lda, 1))
-    if rows is not None:
-        Av = Av[:, rows[0]:rows[1]] if a_mn else Av[rows[0]:rows[1]]
-        M = rows[1] - rows[0]
-    Bv = B.as_strided((Kd, N), (ldb, 1)) if b_mn else B.as_strided((N, Kd), (ldb, 1))
-    ref = torch.zeros(M, N, dtype=torch.float64, device=A.device)
-    absref = torch.zeros_like(ref)
-    mc = max(1, min(M, CHUNK // max(1, min(Kd, 4096))))
-    kc = max(1, min(Kd, CHUNK // max(mc, N)))
-    for m0 in range(0, M, mc):
-        for k0 in range(0, Kd, kc):
-            a = (Av[k0:k0 + kc, m0:m0 + mc].t() if a_mn else Av[m0:m0 + mc, k0:k0 + kc]).double()
-            b = (Bv[k0:k0 + kc] if b_mn else Bv[:, k0:k0 + kc].t()).double()
-            ref[m0:m0 + mc] += a @ b
-            absref[m0:m0 + mc] += a.abs() @ b.abs()
-    for extra in (bias, addend, c0):
-        if extra is not None:
-            e = extra.double()
-            ref += e
-            absref += e.abs()
-    return ref, absref
 
 
 # ------------------------------------------------------------------ vgg.cu data movement (exact statements, in image chunks)
@@ -495,3 +391,444 @@ def check_col2im3(col, y, N, H, W, C, ld, bias, name):
             mag += t.abs()
         worst = max(worst, bound_check(y[n0:n0 + n], ref, 9 * 2.0 ** -24 * mag + BETA[y.dtype] * ref.abs(), f"{name} col2im3 images [{n0}, ..)"))
     return worst
+
+
+# ------------------------------------------------------------------ launch checks (vgg_64 and vgg_128 shapes)
+
+def run_conv(K, sms, L, cdt, seed, label=""):
+    """Launch kind 3 / 5 as L describes (forward_launches / backward_launches entry, or a part-B case) on seeded operands
+    and run checks 1-4 of the launch list.  Returns the variant it exercised."""
+    kind, N, H, Ck, Cn, B = L["kind"], L["N"], L["H"], L["Ck"], L["Cn"], L["B"]
+    HW = H * H
+    name = f"{label}{L['name']} kind {kind} N={N} {H}x{H} {Ck}->{Cn} out={str(cdt)[6:]}"
+    torch.manual_seed(seed)
+    a = randn(N, H, H, Ck, scale=0.5)
+    b = randn(Cn, 9 * Ck, scale=1.0 / math.sqrt(9 * Ck))
+    bias = randn(Cn, dtype=torch.float32) if L["bias"] else None
+    add = src = idx = None
+    ipg = L["ipg"]
+    if L["addend"]:
+        nsrc = L.get("nsrc", 1)
+        G = cdiv(N, ipg)
+        src = torch.tensor([(g + 1) % nsrc for g in range(G)], dtype=torch.int32, device="cuda")
+        idx = addend_index(src.tolist(), ipg, N)
+        add = randn(nsrc * ipg, H, H, Cn)
+    st = L["stat"]
+    s = conv_tiles(kind, N, H, H, Ck, Cn, 0, sms)
+    part = torch.full((s.tiles_m, Cn, 2), NAN, device="cuda") if st is not None else None
+    out = torch.full((N, H, H, Cn), NAN, device="cuda", dtype=cdt)
+    K.conv_gemm(kind, a, b, out, N, H, H, Ck, Cn, bias=bias, addend=add, grp_src=src, imgs_per_group=ipg, stat_partial=part)
+    torch.cuda.synchronize()
+    assert not torch.isnan(out).any(), f"{name}: unwritten output elements"
+    # 1 + 2: float64 and bit-identity on slices of the first, middle and last round
+    worst = 0.0
+    for i0, i1 in slices_with_boundary(N, HW, s, sms, max(1, ipg or B)):
+        arows = add[idx[i0:i1]] if add is not None else None
+        ref, absref = conv3_ref64_elem(kind, a[i0:i1], b, H, Ck, Cn, bias, arows)
+        worst = max(worst, assert_within(out[i0:i1], ref, absref, 9 * Ck, cdt, quiet=True, name=f"{name} images [{i0}, {i1})",
+                                         locate=lambda ix, i0=i0: s.where(0, ((i0 + ix[0]) * HW + ix[1] * H + ix[2]) // 128, ix[3] // s.BN)))
+        del ref, absref
+        sub = conv_tiles(kind, i1 - i0, H, H, Ck, Cn, 0, sms)
+        assert sub.tiles <= sms
+        o = torch.empty(i1 - i0, H, H, Cn, device="cuda", dtype=cdt)
+        p = torch.full((sub.tiles_m, Cn, 2), NAN, device="cuda") if st is not None else None
+        kw = {}
+        if add is not None:   # the same addend rows, one group per image
+            kw = dict(addend=arows.contiguous(), grp_src=torch.arange(i1 - i0, dtype=torch.int32, device="cuda"), imgs_per_group=1)
+        K.conv_gemm(kind, a[i0:i1], b, o, i1 - i0, H, H, Ck, Cn, bias=bias, stat_partial=p, **kw)
+        assert torch.equal(o, out[i0:i1]), f"{name}: images [{i0}, {i1}) differ from a launch of just those images"
+        if p is not None:
+            t0 = i0 * HW // 128
+            assert torch.equal(p, part[t0:t0 + p.shape[0]]), f"{name}: statistics rows of images [{i0}, {i1}) differ"
+        del o, p, arows
+    print(f"[bound] {name} slices: worst error/bound {worst:.3g}")
+    # 3: every tile, through the per-(image, channel) sums
+    check_conv3_sums(out, kind, a, b, N, H, Ck, Cn, bias, add, idx, name=name)
+    # 4: statistics rows and the finalize per BatchNorm group
+    if st is not None:
+        check_stat_rows(part, out, N, H, Cn, name=name)
+        check_finalize_vs_output(K, part, st["parts_per_group"], out, N // B, B * HW, Cn, name=name)
+    v = variant(kind, Ck, Cn, st is not None, add.dtype if add is not None else None, cdt)
+    del a, b, out, part, add
+    release()
+    return v
+
+
+def distinct_convs(launches):
+    """The first launch of each distinct kind-3 / kind-5 shape of a list."""
+    seen, out = set(), []
+    for L in launches:
+        if L["kind"] == 4:
+            continue
+        key = (L["kind"], L["N"], L["H"], L["Ck"], L["Cn"], L["bias"], L["addend"], L["stat"] is not None)
+        if key not in seen:
+            seen.add(key)
+            out.append(L)
+    return out
+
+
+def encoder_first(backward):
+    """A backward list with the encoder's launches first, in layer order (the engine runs them last, in reverse): each shape
+    is then represented by its longest launch (all T B frames) under the encoder layer's name."""
+    enc = [L for L in backward if L["name"].startswith("enc")]
+    return enc[::-1] + [L for L in backward if not L["name"].startswith("enc")]
+
+
+def wgrad_classes(launches):
+    """The first kind-4 launch of each (map size, swapped roles) class of a backward list, encoder launches first."""
+    sms_ = sm_count() if torch.cuda.is_available() else 132
+    seen, out = set(), []
+    for L in encoder_first(launches):
+        if L["kind"] != 4:
+            continue
+        s = conv_tiles(4, L["N"], L["H"], L["H"], 0, L["Cn"], L["Cm"], sms_)
+        if (L["H"], s.swap) not in seen:
+            seen.add((L["H"], s.swap))
+            out.append(L)
+    return out
+
+
+def run_wgrad(K, sms, L):
+    """A kind-4 launch as L describes.  Zero-mean operands would cancel: over K = N H W the worst-case accumulation bound is
+    larger than the result itself.  So (1) 0 / 1 operands, whose fp32 sums are exact integers: the result must equal float64
+    bit for bit, and one lost 64-pixel block or split changes it; (2) real operands that do not cancel (one positive, one of
+    mean 1/2), so that the bound is a small fraction of the value."""
+    N, H, Cm, Cn = L["N"], L["H"], L["Cm"], L["Cn"]
+    s = conv_tiles(4, N, H, H, 0, Cn, Cm, sms)
+    name = f"wgrad {L['name']} {H}x{H} {Cm}x{Cn} swap={s.swap} splits={s.splits}"
+    torch.manual_seed(22)
+    a, b = binary01((N, H, H, Cm)), binary01((N, H, H, Cn))
+    out = torch.full((Cm, 9 * Cn), NAN, device="cuda")
+    K.conv_gemm(4, a, b, out, N, H, H, 0, Cn, Cm=Cm)
+    assert_exact(out, wgrad_ref64(a, b, N, H, Cm, Cn)[0], N * H * H, name + " 0/1 operands")
+    a = torch.rand(N, H, H, Cm, device="cuda").bfloat16()
+    b = randn(N, H, H, Cn, scale=0.5) + 0.5
+    K.conv_gemm(4, a, b, out, N, H, H, 0, Cn, Cm=Cm)
+    ref, absref = wgrad_ref64(a, b, N, H, Cm, Cn)
+    keff = s.kb_per_split * 64 + 16 * s.splits
+    assert (ref.abs() >= 0.5 * absref).all()
+    assert_within(out, ref, absref, keff, torch.float32, name=f"{name} K={N * H * H} non-cancelling operands")
+    del a, b, out, ref, absref
+    release()
+
+
+def run_end_gemms(K, M):
+    """The explicit GEMMs of the 3-channel ends over M pixels: the first encoder layer ([M, 32] x [64, 32] after im2col3) and
+    the last decoder layer ([M, 64] x [64, 32], MN-major weight), and the [64, 32] weight gradient with K = M that both the
+    first layer (dy^T col) and the last layer (x^T dcol, row pitch up8(27) = 32) launch."""
+    torch.manual_seed(23)
+    col = randn(M, 32)
+    col[:, 27:] = 0
+    w = randn(64, 32, scale=0.3)
+    bias = randn(64, dtype=torch.float32)
+    out = torch.full((M, 64), NAN, device="cuda", dtype=torch.bfloat16)
+    K.gemm(col, w, out, M, 64, 32, bias=bias)
+    for r0 in range(0, M, 1 << 21):
+        r1 = min(M, r0 + (1 << 21))
+        ref, absref = gemm_ref64(col[r0:r1], w, r1 - r0, 64, 32, False, False, 32, 32, bias=bias)
+        assert_within(out[r0:r1], ref, absref, 32, torch.bfloat16, quiet=r0 > 0, name=f"enc first layer GEMM rows {r0}")
+    a = randn(M, 64)
+    wl = randn(64, 32, scale=0.2)
+    colT = torch.full((M, 32), NAN, device="cuda", dtype=torch.bfloat16)
+    K.gemm(a, wl, colT, M, 32, 64, b_mn=True)
+    for r0 in range(0, M, 1 << 21):
+        r1 = min(M, r0 + (1 << 21))
+        ref, absref = gemm_ref64(a[r0:r1], wl, r1 - r0, 32, 64, False, True, 64, 32)
+        assert_within(colT[r0:r1], ref, absref, 64, torch.bfloat16, quiet=r0 > 0, name=f"dec last layer GEMM rows {r0}")
+    del col, out, a, colT
+    # the first layer's weight gradient, K = M: exact on 0 / 1 operands, and within the bound on operands that do not cancel
+    s = gemm_tc_tiles(64, 32, M, sm_count())
+    name = f"enc first layer weight gradient K={M} splits={s.splits}"
+    dy, col = binary01((M, 64)), binary01((M, 32))
+    gw = torch.full((64, 32), NAN, device="cuda")
+    K.set_gemm_impl("tc")
+    try:
+        K.gemm(dy, col, gw, 64, 32, M, a_mn=True, b_mn=True, lda=64, ldb=32)
+        assert_exact(gw, gemm_ref64(dy, col, 64, 32, M, True, True, 64, 32)[0], M, name + " 0/1 operands")
+        dy = torch.rand(M, 64, device="cuda").bfloat16()
+        col = randn(M, 32, scale=0.5) + 0.5
+        K.gemm(dy, col, gw, 64, 32, M, a_mn=True, b_mn=True, lda=64, ldb=32)
+    finally:
+        K.set_gemm_impl("auto")
+    ref, absref = gemm_ref64(dy, col, 64, 32, M, True, True, 64, 32)
+    assert (ref.abs() >= 0.5 * absref).all()
+    assert_within(gw, ref, absref, s.kb_per_split * 64 + 16 * s.splits, torch.float32, name=name)
+    del dy, col
+    release()
+
+
+def misaligned_like(n, dtype):
+    """A flat tensor of n elements whose data pointer is not 16-byte aligned (forces the scalar kernels)."""
+    return torch.empty(n + 1, device="cuda", dtype=dtype)[1:]
+
+
+def run_maxpool(K, N, H, C, dtype, label):
+    """maxpool2_fwd / maxpool2_bwd on an N x H x H x C map with planted ties: equal pairs, four equal values, and -0 / +0.
+    The gradient goes to the first maximum in row-major order; the scalar paths equal the vector ones."""
+    torch.manual_seed(26)
+    x = randn(N, H, H, C, dtype=dtype)
+    w = windows(x, N, H, H, C)
+    # ties, on every 7th / 11th / 13th window channel
+    w[1][..., 0::7].copy_(w[0][..., 0::7])                        # pair (0, 1)
+    w[3][..., 3::11].copy_(w[2][..., 3::11])                      # pair (2, 3)
+    for k in (1, 2, 3):
+        w[k][:, ::5, :, 5::13].copy_(w[0][:, ::5, :, 5::13])      # four equal
+    w[0][:, 1::5, :, 6::13] = -0.0                                 # -0 then +0, the others negative
+    w[1][:, 1::5, :, 6::13] = 0.0
+    w[2][:, 1::5, :, 6::13] = -1.0
+    w[3][:, 1::5, :, 6::13] = -2.0
+    del w
+    y = torch.empty(N, H // 2, H // 2, C, device="cuda", dtype=dtype)
+    K.maxpool2_fwd(x, y, N, H, H, C)
+    ys = misaligned_like(y.numel(), dtype).view_as(y)
+    K.maxpool2_fwd(x, ys, N, H, H, C)
+    dy = randn(N, H // 2, H // 2, C, dtype=dtype)
+    dx = torch.empty_like(x)
+    K.maxpool2_bwd(x, dy, dx, N, H, H, C)
+    dxs = misaligned_like(x.numel(), dtype).view_as(x)
+    K.maxpool2_bwd(x, dy, dxs, N, H, H, C)
+    check_maxpool(x, y, dy, dx, N, H, H, C, f"{label} {dtype}")
+    for n0 in range(0, N, 256):
+        sl = slice(n0, n0 + 256)
+        assert torch.equal(ys[sl], y[sl]) and torch.equal(dxs[sl], dx[sl]), f"scalar and vector paths differ, images [{n0}, ..)"
+    print(f"[exact] maxpool2 fwd/bwd {dtype} N={N} {H}x{H}x{C}: exact, scalar == vector")
+    del x, y, ys, dy, dx, dxs
+    release()
+
+
+def run_upsample(K, N, H, C, dtype, label):
+    """upsample2_fwd / upsample2_bwd from an N x H x H x C map: forward exact; backward bit for bit against torch's fp32
+    (a + b) + (c + d) and within one rounding of float64; the scalar paths equal the vector ones."""
+    torch.manual_seed(27)
+    x = randn(N, H, H, C, dtype=dtype)
+    u = torch.empty(N, 2 * H, 2 * H, C, device="cuda", dtype=dtype)
+    K.upsample2_fwd(x, u, N, H, H, C)
+    us = misaligned_like(u.numel(), dtype).view_as(u)
+    K.upsample2_fwd(x, us, N, H, H, C)
+    check_upsample_fwd(x, u, N, H, H, C, f"{label} {dtype}")
+    for n0 in range(0, N, 256):
+        assert torch.equal(us[n0:n0 + 256], u[n0:n0 + 256]), f"upsample2_fwd scalar and vector paths differ, images [{n0}, ..)"
+    del us
+    dy = u.normal_()   # the 64x64 gradient map, reusing the upsampled buffer
+    dx = torch.empty(N, H, H, C, device="cuda", dtype=dtype)
+    K.upsample2_bwd(dy, dx, N, H, H, C)
+    dxs = misaligned_like(dx.numel(), dtype).view_as(dx)
+    K.upsample2_bwd(dy, dxs, N, H, H, C)
+    worst = check_upsample_bwd(dy, dx, N, H, H, C, f"{label} {dtype}")
+    for n0 in range(0, N, 256):
+        assert torch.equal(dxs[n0:n0 + 256], dx[n0:n0 + 256]), f"upsample2_bwd scalar and vector paths differ, images [{n0}, ..)"
+    print(f"[bound] upsample2 {dtype} N={N} {H}x{H}x{C}: fwd exact, bwd bit-exact, worst error/bound vs float64 {worst:.3g}")
+    del x, u, dy, dx, dxs
+    release()
+
+
+def run_im2col3_col2im3(K, N, H, dtype, label):
+    """The 3-channel ends on N frames of H x H x 3: im2col3's row32 path (ld = 32) against the generic one (ld = 40) and an
+    exact statement for both tap signs, pad columns zero; col2im3 within 9 fp32 adds and one rounding."""
+    C = 3
+    torch.manual_seed(28)
+    x = randn(N, H, H, C, dtype=dtype)
+    for sgn in (1, -1):
+        c32 = torch.full((N * H * H, 32), 7.0, device="cuda", dtype=dtype)
+        c40 = torch.full((N * H * H, 40), 7.0, device="cuda", dtype=dtype)
+        K.im2col3(x, c32, N, H, H, C, 32, sgn)
+        K.im2col3(x, c40, N, H, H, C, 40, sgn)
+        check_im2col3(x, c40, N, H, H, C, 40, sgn, f"{label} generic {dtype}")
+        check_im2col3(x, c32, N, H, H, C, 32, sgn, f"{label} row32 {dtype}")
+        del c32, c40
+    ld = 32
+    col = randn(N * H * H, ld, dtype=dtype)
+    bias = randn(C, dtype=torch.float32)
+    y = torch.full((N, H, H, C), NAN, device="cuda", dtype=dtype)
+    K.col2im3(col, y, N, H, H, C, ld, bias=bias)
+    worst = check_col2im3(col, y, N, H, H, C, ld, bias, f"{label} {dtype}")
+    print(f"[bound] im2col3 exact (row32 == generic), col2im3 {dtype}: worst error/bound {worst:.3g}")
+    del x, col, y
+    release()
+
+
+def run_skip_index(K, G, B, H, C, dtype, gather):
+    """(gather: gather_add,) group_sum and add_indexed over G groups of B images of H x H x C, three distinct skip sources."""
+    nsrc = 3
+    n = B * H * H * C
+    src = torch.tensor([(g + 1) % nsrc for g in range(G)], dtype=torch.int32, device="cuda")
+    srcl = src.tolist()
+    torch.manual_seed(29)
+    big = randn(G * n, dtype=dtype)
+    if gather:
+        small = randn(nsrc * n, dtype=torch.float32)
+        dst0 = big.clone()
+        # gather_add: dst[g] += src[grp_src[g]] (fp32 addend); a bf16 destination rounds twice (fp32, then bf16): one bf16 ulp
+        K.gather_add(big, small, src, G, n)
+        worst = 0.0
+        for g in range(G):
+            ref = dst0[g * n:(g + 1) * n].double() + small[srcl[g] * n:(srcl[g] + 1) * n].double()
+            rel = 2.0 ** -7 if dtype == torch.bfloat16 else 2.0 ** -23
+            worst = max(worst, bound_check(big[g * n:(g + 1) * n], ref, rel * ref.abs(), f"gather_add group {g}"))
+        print(f"[bound] gather_add {dtype} G={G} n={n}: worst error/bound {worst:.3g}")
+        del dst0, small
+    # group_sum: out[f] = sum over the groups reading source f (fp32 in group order, one output rounding)
+    out = torch.full((nsrc * n,), NAN, device="cuda", dtype=dtype)
+    K.group_sum(big, out, src, G, nsrc, n)
+    worst = 0.0
+    for f in range(nsrc):
+        for j0 in range(0, n, 1 << 24):
+            j1 = min(n, j0 + (1 << 24))
+            gs = [g for g in range(G) if srcl[g] == f]
+            ref = sum(big[g * n + j0:g * n + j1].double() for g in gs)
+            mag = sum(big[g * n + j0:g * n + j1].double().abs() for g in gs)
+            worst = max(worst, bound_check(out[f * n + j0:f * n + j1], ref, len(gs) * 2.0 ** -24 * mag + BETA[dtype] * ref.abs(),
+                                            f"group_sum source {f}"))
+    print(f"[bound] group_sum {dtype}: worst error/bound {worst:.3g}")
+    # add_indexed: dst[dst_idx[f]] += src[f]; the other groups untouched
+    dst_idx = torch.tensor([2, 0, 1], dtype=torch.int32, device="cuda")
+    dst0 = big.clone()
+    K.add_indexed(big, out, dst_idx, nsrc, n)
+    worst = 0.0
+    for f, d in enumerate(dst_idx.tolist()):
+        ref = dst0[d * n:(d + 1) * n].double() + out[f * n:(f + 1) * n].double()
+        worst = max(worst, bound_check(big[d * n:(d + 1) * n], ref, BETA[dtype] * ref.abs(), f"add_indexed {f} -> {d}"))
+    assert torch.equal(big[nsrc * n:], dst0[nsrc * n:]), "add_indexed wrote outside its destination groups"
+    print(f"[bound] add_indexed {dtype}: worst error/bound {worst:.3g}")
+    del big, dst0, out
+    release()
+
+
+# ------------------------------------------------------------------ the audited step
+
+AUDIT_CASES = [("bench_options", BENCH_OPT), ("skip_lfs", SKIP_OPT)]
+
+
+class VggAudit(AuditKernels):
+    """AuditKernels for a vgg step: also its convolutions (kinds 3, 4, 5), the 3-channel ends, pooling and upsampling, the
+    fp32 skip gather and the BatchNorm finalize."""
+    PRINT_RECORDS = True
+
+    # ---- convolutions
+    def conv_gemm(self, kind, a, b, c, N, H, W, Ck, Cn, Cm=0, ldb=None, ldc=None, bias=None, addend=None, grp_src=None,
+                  imgs_per_group=0, accumulate=False, stat_partial=None, eval_scale=None, eval_shift=None, act=0):
+        assert kind in (3, 4, 5) and H == W and eval_scale is None, f"unexpected conv_gemm launch kind {kind} in a vgg step"
+        torch.cuda.synchronize()
+        c0 = c.clone() if accumulate else None
+        self._sync("conv_gemm", kind, a, b, c, N, H, W, Ck, Cn, Cm, ldb, ldc, bias, addend, grp_src, imgs_per_group, accumulate,
+                   stat_partial, eval_scale, eval_shift, act)
+        if kind == 4:
+            s = conv_tiles(4, N, H, W, 0, Cn, Cm, self._sms)
+            npx = N * H * W
+            ref, absref = wgrad_ref64(a.view(-1)[:npx * Cm].view(N, H, W, Cm), b.view(-1)[:npx * Cn].view(N, H, W, Cn), N, H, Cm, Cn)
+            if c0 is not None:
+                ref += c0.view(-1)[:Cm * 9 * Cn].view(Cm, 9 * Cn).double()
+                absref += c0.view(-1)[:Cm * 9 * Cn].view(Cm, 9 * Cn).double().abs()
+            got = c.view(-1)[:Cm * 9 * Cn].view(Cm, 9 * Cn)
+            w = assert_within(got, ref, absref, s.kb_per_split * 64 + 16 * s.splits, torch.float32, quiet=True,
+                              name=f"audit kind 4 N={N} {H}x{W} {Cm}x{Cn}")
+            # the step's gradients cancel over these K, so the bound above is loose; the same launch on the 0 / 1 pattern of
+            # its operands (x > 0) must be exact
+            a01 = (a.view(-1)[:npx * Cm] > 0).bfloat16().view(N, H, W, Cm)
+            b01 = (b.view(-1)[:npx * Cn] > 0).bfloat16().view(N, H, W, Cn)
+            probe = torch.full((Cm, 9 * Cn), NAN, device=c.device)
+            super().conv_gemm(4, a01, b01, probe, N, H, W, 0, Cn, Cm=Cm)
+            assert_exact(probe, wgrad_ref64(a01, b01, N, H, Cm, Cn)[0], npx, f"audit kind 4 N={N} {H}x{W} {Cm}x{Cn} 0/1 probe")
+            self._rec(f"conv_gemm kind 4 N={N} {H}x{W} {Cm}x{Cn}", variant(4, 0, Cn, False, None, c.dtype, swap=s.swap), w)
+            return
+        assert not accumulate
+        x = a.view(-1)[:N * H * W * Ck].view(N, H, W, Ck)
+        wt = b.view(-1)[:Cn * 9 * Ck].view(Cn, 9 * Ck)
+        out = c.view(-1)[:N * H * W * Cn].view(N, H, W, Cn)
+        add, idx = self._addend(addend, grp_src, imgs_per_group, N, H, Cn) if addend is not None else (None, None)
+        nm = f"conv_gemm kind {kind} N={N} {H}x{W} {Ck}->{Cn}"
+        w = check_conv3_sums(out, kind, x, wt, N, H, Ck, Cn, bias, add, idx, name="audit " + nm)
+        for i0 in sorted({0, N // 2, N - 1}):   # three images element-wise
+            ref, absref = conv3_ref64_elem(kind, x[i0:i0 + 1], wt, H, Ck, Cn, bias, add[idx[i0:i0 + 1]] if add is not None else None)
+            w = max(w, assert_within(out[i0:i0 + 1], ref, absref, 9 * Ck, out.dtype, quiet=True, name=f"audit {nm} image {i0}"))
+        if stat_partial is not None:
+            tiles = cdiv(N * H * W, 128)
+            w = max(w, check_stat_rows(stat_partial.view(-1)[:tiles * Cn * 2].view(tiles, Cn, 2), out, N, H, Cn, name="audit " + nm))
+        self._rec(nm, variant(kind, Ck, Cn, stat_partial is not None, addend.dtype if addend is not None else None, c.dtype), w)
+
+    # ---- 3-channel ends
+    def im2col3(self, x, col, N, H, W, C, ld, sgn=1):
+        self._sync("im2col3", x, col, N, H, W, C, ld, sgn)
+        check_im2col3(x, col, N, H, W, C, ld, sgn, "audit")
+        self._rec(f"im2col3 N={N} C={C} ld={ld}", ("im2col3", "row32" if ld == 32 and C in (1, 3) else "generic", sgn), 0.0)
+
+    def col2im3(self, col, y, N, H, W, C, ld, bias=None):
+        self._sync("col2im3", col, y, N, H, W, C, ld, bias)
+        self._rec(f"col2im3 N={N}", ("col2im3",), check_col2im3(col, y, N, H, W, C, ld, bias, "audit"))
+
+    # ---- pooling / upsampling
+    def maxpool2_fwd(self, x, y, N, H, W, C):
+        self._sync("maxpool2_fwd", x, y, N, H, W, C)
+        check_maxpool(x, y, None, None, N, H, W, C, "audit")
+        self._rec(f"maxpool2_fwd N={N} {H}x{W}x{C}", ("maxpool2_fwd",), 0.0)
+
+    def maxpool2_bwd(self, x, dy, dx, N, H, W, C):
+        self._sync("maxpool2_bwd", x, dy, dx, N, H, W, C)
+        check_maxpool(x, None, dy, dx, N, H, W, C, "audit")
+        self._rec(f"maxpool2_bwd N={N} {H}x{W}x{C}", ("maxpool2_bwd",), 0.0)
+
+    def upsample2_fwd(self, x, y, N, H, W, C):
+        self._sync("upsample2_fwd", x, y, N, H, W, C)
+        check_upsample_fwd(x, y, N, H, W, C, "audit")
+        self._rec(f"upsample2_fwd N={N} {H}x{W}x{C}", ("upsample2_fwd",), 0.0)
+
+    def upsample2_bwd(self, dy, dx, N, H, W, C):
+        self._sync("upsample2_bwd", dy, dx, N, H, W, C)
+        self._rec(f"upsample2_bwd N={N} {H}x{W}x{C}", ("upsample2_bwd",), check_upsample_bwd(dy, dx, N, H, W, C, "audit"))
+
+    # ---- the fp32 skip gather and the BatchNorm finalize
+    def gather_add(self, dst, src, grp_src, G, n):
+        torch.cuda.synchronize()
+        d0 = dst.view(-1)[:G * n].clone()
+        self._sync("gather_add", dst, src, grp_src, G, n)
+        srcl = grp_src.tolist()
+        ref = d0.double().view(G, n) + src.view(-1).double().view(-1, n)[srcl[:G]]
+        rel = 2.0 ** -7 if dst.dtype == torch.bfloat16 else 2.0 ** -23
+        self._rec(f"gather_add G={G}", ("gather_add",), bound_check(dst.view(-1)[:G * n].view(G, n), ref, rel * ref.abs(), "audit gather_add"))
+
+    def bn_fwd_finalize_tiles(self, partial, parts_per_group, ldp, fold, G, R, C, gamma, beta, mean, invstd, var_unb, scale,
+                              shift, eps=1e-5):
+        self._sync("bn_fwd_finalize_tiles", partial, parts_per_group, ldp, fold, G, R, C, gamma, beta, mean, invstd, var_unb, scale,
+                   shift, eps)
+        assert fold == 1 and ldp == C
+        p = partial.view(-1)[:G * parts_per_group * C * 2].view(G, parts_per_group, C, 2).double()
+        s1, s2, m1 = p[..., 0].sum(1), p[..., 1].sum(1), p[..., 0].abs().sum(1)
+        # the kernel's own operands are exact here: only the float64 combine order and the fp32 outputs differ
+        w = 0.0
+        for got, (ref, _), nm in zip((mean, invstd, var_unb, scale, shift), finalize_ref(s1, s2, m1, R, gamma, beta, eps, 0.0),
+                                     ("mean", "invstd", "var_unbiased", "scale", "shift")):
+            g = got.view(-1)[:G * C].view(G, C)
+            mag = ref.abs() if nm != "shift" else beta.double().abs() + (s1 / R * scale.view(-1)[:G * C].view(G, C).double()).abs()
+            if nm == "mean":
+                mag = mag + 2.0 ** -30 * m1 / R
+            w = max(w, bound_check(g, ref, 2.0 ** -20 * mag + 1e-30, f"audit finalize {nm}"))
+        self._rec(f"bn_fwd_finalize_tiles G={G} C={C}", ("bn_fwd_finalize_tiles",), w)
+
+
+def vgg_cfg(W0):
+    return dict(g_dim=128, z_dim=10, rnn_size=256, channels=3, image_width=W0, backbone="vgg", predictor_rnn_layers=2,
+                posterior_rnn_layers=1, prior_rnn_layers=1)
+
+
+def audit_vgg_step(name, optkw, T, B, W0):
+    """One eager bf16 vgg step (vgg_64 or vgg_128 by W0) with every launch checked as it runs (launch_audit.audit_step): every
+    path of the derived launch list must occur, and every decoder stage entry reads, for decoder call s, the skip frame the
+    reference's schedule names (models/p2p_model.py).  Returns the plain step's results."""
+    def expect(plan):
+        fwd = forward_launches(T, B, plan.S, plan.nskip, W0)
+        want = set()
+        for L in fwd + backward_launches(T, B, plan.S, plan.nskip, W0, plan.has_cpc):
+            if L["kind"] == 4:
+                want.add(variant(4, 0, L["Cn"], False, None, torch.float32, swap=conv_tiles(4, L["N"], L["H"], L["H"], 0, L["Cn"], L["Cm"], sm_count()).swap))
+            else:
+                want.add(variant(L["kind"], L["Ck"], L["Cn"], L["stat"] is not None, torch.bfloat16 if L["addend"] else None, torch.bfloat16))
+        want |= {("maxpool2_fwd",), ("maxpool2_bwd",), ("upsample2_fwd",), ("upsample2_bwd",), ("group_sum",), ("add_indexed",),
+                 ("bn_fwd_finalize_tiles",), ("col2im3",), ("im2col3", "row32", 1)}
+        for v in [("k3", "bres", "-", "add_bf16", "rowcoop"), ("k3", "bn128", "stat", "add_bf16", "perrow"), ("k4", "swap"),
+                  ("k4", "noswap"), ("k3", "bn128", "-", "-", "rowcoop"), ("k5", "bres", "-", "-", "rowcoop")]:
+            assert v in want, f"the derived launch list lost {v}"
+        return want, [plan.skip_src] * sum(1 for L in fwd if L["addend"])
+    audit = VggAudit("cuda")
+    _, plain = audit_step(TrainEngineVGG, vgg_cfg(W0), optkw, T, B, audit, expect, f"{name} {W0}x{W0}")
+    assert any(v[0] == "gemm" for v in audit.seen)
+    return plain
