@@ -17,6 +17,7 @@ device data happens inside those kernels.
 """
 from __future__ import annotations
 
+import gc
 import math
 import os
 import time
@@ -48,6 +49,23 @@ def skip_schedule(seq_len, probs, skip_prob, n_past):
         out.append((i, (cp_ix - i + 1) / cp_ix, (i - prev_i) / cp_ix))
         prev_i = i
     return out
+
+
+def capture_graph(fn, device=None):
+    """fn() captured into a new torch.cuda.CUDAGraph, after a device synchronise.  The garbage collector is paused during
+    the capture: a dropped model and its engine form a reference cycle, and a cached CUDA graph the collector destroys
+    mid-capture invalidates this capture."""
+    torch.cuda.synchronize(device)
+    g = torch.cuda.CUDAGraph()
+    gc_on = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(g):
+            fn()
+    finally:
+        if gc_on:
+            gc.enable()
+    return g
 
 
 class StepPlan:
@@ -420,9 +438,9 @@ class TrainEngine:
         self.coef = cf[:S1]
 
     # ------------------------------------------------------------------ phases
-    def step(self, x, probs=None, eps=None, return_device=False, use_graph=False):
-        """x: [T,B,C,H,W] fp32 on the device.  probs: host numpy uniform draws (None -> np.random.uniform,
-        like models/p2p_model.py:215).  eps: [S,2,B,z] N(0,1) (None -> torch.randn on the device)."""
+    def _prepare(self, x, probs, eps):
+        """What step() and evaluate_losses() do before any kernel runs: the skip draw and eps draw where the caller gave
+        none (in the reference's order), the plan of the executed timesteps and its index tables on the device."""
         T, B = int(x.shape[0]), int(x.shape[1])
         opt = self.opt
         if probs is None:
@@ -436,7 +454,6 @@ class TrainEngine:
             if len(self._plans) > 4096:
                 self._plans.clear()
             plan = self._plans[pkey] = StepPlan(T, probs, opt)
-        self.last_plan = plan
         self.T, self.B, self.S = T, B, plan.S
         if eps is None:
             eps = torch.randn(plan.S, 2, B, self.z, device=self.dev, dtype=torch.float32)
@@ -444,11 +461,35 @@ class TrainEngine:
         if ukey != self._uploaded:
             self.upload_plan(plan)
             self._uploaded = ukey
+        return plan, eps
+
+    def step(self, x, probs=None, eps=None, return_device=False, use_graph=False):
+        """x: [T,B,C,H,W] fp32 on the device.  probs: host numpy uniform draws (None -> np.random.uniform,
+        like models/p2p_model.py:215).  eps: [S,2,B,z] N(0,1) (None -> torch.randn on the device).
+        use_graph: the step as a CUDA-graph replay (_graphed), its inputs staged in static buffers."""
+        plan, eps = self._prepare(x, probs, eps)
+        self.last_plan = plan
         if self.early_loss:
             self._pub_seq = (self._pub_seq + 1) & 0x3FFFFFFF
             self._pub_seq_dev.fill_(self._pub_seq)
         if use_graph:
-            out = self._step_graphed(x, eps, plan)
+            # host scalars that the kernels receive by value are part of the signature: a replay would silently keep
+            # the values seen at capture time (lr, loss weights, configured batch size, Adam beta1)
+            opt = self.opt
+            key = plan.key + (self.B, tuple(x.shape[2:]), float(opt["lr"]), float(opt["beta1"]), float(opt["beta"]),
+                              float(opt["weight_align"]), float(opt["weight_cpc"]), int(opt["batch_size"]), self.mode,
+                              self.dist[2] if self.dist is not None else 1)
+            xs = self._stage("x_static", x)
+            # the caller's batch tensor is not read again by this step: an input pipeline that attached a callback
+            # (p2pvg_b200.data.DevicePrefetcher) may refill its slot from here on instead of after the whole step
+            consumed = getattr(x, "_p2pvg_on_consumed", None)
+            if consumed is not None:
+                ev = torch.cuda.Event()
+                ev.record()
+                consumed(ev)
+            self.eps = self._stage("eps_static", eps)
+            self._graphed(self._graphs, key, lambda: self._run(xs, plan), self.graph_generation)
+            out = self._bufs["loss_out"][:4]
         else:
             self.eps = eps.contiguous()
             out = self._run(x, plan)
@@ -478,52 +519,36 @@ class TrainEngine:
                 time.sleep(0)
         return self._pub_np[:4].copy()
 
-    def _step_graphed(self, x, eps, plan):
-        """CUDA-graph replay of the whole step.  The first call with a new (T,B,S,...) signature runs eagerly
-        (allocating every buffer), the second captures, later ones only replay; index tables, counters and
-        inputs live in static device buffers that are refreshed before each replay."""
-        # host scalars that the kernels receive by value are part of the signature: a replay would silently keep
-        # the values seen at capture time (lr, loss weights, configured batch size, Adam beta1)
-        opt = self.opt
-        key = plan.key + (self.B, tuple(x.shape[2:]), float(opt["lr"]), float(opt["beta1"]), float(opt["beta"]),
-                          float(opt["weight_align"]), float(opt["weight_cpc"]), int(opt["batch_size"]), self.mode,
-                          self.dist[2] if self.dist is not None else 1)
-        xs = self.fbuf("x_static", x.numel()).view(-1)[:x.numel()].view(x.shape)
-        es = self.fbuf("eps_static", eps.numel()).view(-1)[:eps.numel()].view(eps.shape)
-        xs.copy_(x, non_blocking=True)
-        # the caller's batch tensor is not read again by this step: an input pipeline that attached a callback
-        # (p2pvg_b200.data.DevicePrefetcher) may refill its slot from here on instead of after the whole step
-        consumed = getattr(x, "_p2pvg_on_consumed", None)
-        if consumed is not None:
-            ev = torch.cuda.Event()
-            ev.record()
-            consumed(ev)
-        es.copy_(eps, non_blocking=True)
-        self.eps = es
-        st = self._graphs.get(key)
-        if st is not None and st != "warm" and st[2] != self.graph_generation():
+    def _stage(self, name, t):
+        """Copy of t in the static input buffer `name`, whose address a captured graph keeps."""
+        s = self.fbuf(name, t.numel()).view(-1)[:t.numel()].view(t.shape)
+        s.copy_(t, non_blocking=True)
+        return s
+
+    def _graphed(self, table, key, run, generation):
+        """run() as a CUDA-graph replay cached in table[key].  The first call with a key runs eagerly (allocating every
+        buffer), the second captures, later ones only replay; index tables, counters and inputs live in static device
+        buffers that are refreshed before each replay.  generation() names every buffer a graph may have baked in."""
+        st = table.get(key)
+        if st is not None and st != "warm" and st[2] != generation():
             st = None   # some buffer moved since this graph was captured
         if st is None:
             # eager run: allocates / grows every buffer this signature needs
-            gen0 = self.graph_generation()
-            out = self._run(xs, plan)
-            if self.graph_generation() != gen0:
-                self._graphs.clear()   # older graphs point into freed buffers
-            self._graphs[key] = "warm"
-            return out
+            gen0 = generation()
+            run()
+            if generation() != gen0:
+                table.clear()   # older graphs point into freed buffers
+            table[key] = "warm"
+            return
         if st == "warm":
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
             n0 = self.K.launches
-            gen0 = self.graph_generation()
-            with torch.cuda.graph(g):
-                self._run(xs, plan)
-            if self.graph_generation() != gen0:
+            gen0 = generation()
+            g = capture_graph(run, self.dev)
+            if generation() != gen0:
                 raise RuntimeError("a buffer was re-allocated during CUDA-graph capture (the warm-up run must size every buffer)")
-            self._graphs[key] = st = (g, self.K.launches - n0, gen0)
+            table[key] = st = (g, self.K.launches - n0, gen0)
         st[0].replay()
         self.K.launches += st[1]
-        return self._bufs["loss_out"][:4]
 
     # ------------------------------------------------------------------ eval-mode forward (held-out scoring)
     def evaluate_losses(self, x, probs=None, eps=None, use_graph=False):
@@ -532,68 +557,23 @@ class TrainEngine:
         and BatchNorm buffers are left as they are.  x, probs, eps: as for step() (drawn in the same order when None).
         Returns (plan, per_seq, out): per_seq fp64 [4, B] device tensor of every row's (mse, kld, cpc, align), out fp64 [4]
         the four scalars forward returns (p2pvg_seq_losses); both are fresh tensors."""
-        T, B = int(x.shape[0]), int(x.shape[1])
-        opt = self.opt
-        if probs is None:
-            probs = np.random.uniform(0, 1, T - 1)
-        sched = skip_schedule(T, probs, opt["skip_prob"], opt["n_past"])
-        pkey = (T, tuple(i for i, _, _ in sched), bool(opt["last_frame_skip"]), int(opt["n_past"]))
-        plan = self._plans.get(pkey)
-        if plan is None:
-            if len(self._plans) > 4096:
-                self._plans.clear()
-            plan = self._plans[pkey] = StepPlan(T, probs, opt)
-        self.T, self.B, self.S = T, B, plan.S
-        if eps is None:
-            eps = torch.randn(plan.S, 2, B, self.z, device=self.dev, dtype=torch.float32)
-        ukey = (pkey, B, float(opt["weight_cpc"]), self.graph_generation())
-        if ukey != self._uploaded:
-            self.upload_plan(plan)
-            self._uploaded = ukey
+        plan, eps = self._prepare(x, probs, eps)
         fuse_stats, self.fuse_stats = self.fuse_stats, False   # no statistics epilogues: BatchNorm uses running statistics
         self._eval = True
         try:
             if use_graph:
-                self._eval_graphed(x, eps, plan)
+                # a graph table of its own, checked against eval_graph_generation: another skip pattern of the same
+                # signature only refreshes the index tables, and nothing allocated here invalidates the step's graphs
+                key = plan.key + (self.B, tuple(x.shape[2:]), int(self.opt["batch_size"]))
+                xs = self._stage("x_eval_static", x)
+                self.eps = self._stage("eps_eval_static", eps)
+                self._graphed(self._eval_graphs, key, lambda: self._run_eval(xs, plan), self.eval_graph_generation)
             else:
                 self.eps = eps.contiguous()
                 self._run_eval(x, plan)
         finally:
             self._eval, self.fuse_stats = False, fuse_stats
-        return plan, self._seq_per[:4 * B].view(4, B).clone(), self._seq_out[:4].clone()
-
-    def _eval_graphed(self, x, eps, plan):
-        """evaluate_losses as a CUDA-graph replay, managed like _step_graphed (eager run, capture, replays) in a graph table of
-        its own, checked against eval_graph_generation: another skip pattern of the same signature only refreshes the index
-        tables, and nothing allocated here invalidates the step's graphs."""
-        key = plan.key + (self.B, tuple(x.shape[2:]), int(self.opt["batch_size"]))
-        xs = self.fbuf("x_eval_static", x.numel()).view(-1)[:x.numel()].view(x.shape)
-        es = self.fbuf("eps_eval_static", eps.numel()).view(-1)[:eps.numel()].view(eps.shape)
-        xs.copy_(x, non_blocking=True)
-        es.copy_(eps, non_blocking=True)
-        self.eps = es
-        st = self._eval_graphs.get(key)
-        if st is not None and st != "warm" and st[2] != self.eval_graph_generation():
-            st = None
-        if st is None:
-            gen0 = self.eval_graph_generation()
-            self._run_eval(xs, plan)
-            if self.eval_graph_generation() != gen0:
-                self._eval_graphs.clear()
-            self._eval_graphs[key] = "warm"
-            return
-        if st == "warm":
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            n0 = self.K.launches
-            gen0 = self.eval_graph_generation()
-            with torch.cuda.graph(g):
-                self._run_eval(xs, plan)
-            if self.eval_graph_generation() != gen0:
-                raise RuntimeError("a buffer was re-allocated during CUDA-graph capture (the warm-up run must size every buffer)")
-            self._eval_graphs[key] = st = (g, self.K.launches - n0, gen0)
-        st[0].replay()
-        self.K.launches += st[1]
+        return plan, self._seq_per[:4 * self.B].view(4, self.B).clone(), self._seq_out[:4].clone()
 
     def _run_eval(self, x, plan):
         self.pack_weights(backward=False)   # only the copies the forward phases read
@@ -709,12 +689,9 @@ class TrainEngine:
         out = {}
         try:
             self._run(x, plan)   # eager: every buffer exists, activations of this batch are in place
-            torch.cuda.synchronize(self.dev)
             self._serial = True
             for name, fn, _ in self.phases(x, plan):
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    fn()
+                g = capture_graph(fn, self.dev)
                 g.replay()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()

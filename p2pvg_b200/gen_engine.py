@@ -57,13 +57,13 @@ draws are consumed in the reference's order (posterior, then prior, per executed
 """
 from __future__ import annotations
 
-import gc
 from collections import OrderedDict
 
 import numpy as np
 import torch
 
 from ._lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH
+from .engine import capture_graph
 from .layouts import cast, implicit_shape, nchw_to_nhwc, nhwc_to_nchw, pack_conv4, pack_convt4, tile_bias
 
 MAX_GRAPHS = 4
@@ -475,18 +475,7 @@ class GenerateEngine:
             G.cfg = cfg
             self._alloc_io(G)
             self._body(G)
-            torch.cuda.current_stream(dev).synchronize()
-            G.graph = torch.cuda.CUDAGraph()
-            # no garbage collection during the capture: a dropped model and its engine form a reference cycle, and a cached
-            # CUDA graph the collector destroys mid-capture invalidates this capture
-            gc_on = gc.isenabled()
-            gc.disable()
-            try:
-                with torch.cuda.graph(G.graph):
-                    self._body(G)
-            finally:
-                if gc_on:
-                    gc.enable()
+            G.graph = capture_graph(lambda: self._body(G), dev)
             G.ws_gen = K.ws_gen
             self._graphs[sig] = G
             while len(self._graphs) > MAX_GRAPHS:
