@@ -627,6 +627,24 @@ int p2pvg_gif_encode(const int64_t* anims, int n, int rule, void* workspace, siz
  * Host code (no device, no stream); data may be NULL when n == 0. */
 uint32_t p2pvg_crc32c(const void* data, size_t n, uint32_t crc);
 
+/* Human3.6M skeletons as the reference's Skeleton3DVisualizer draws them (data/human36m/human36m.py:290-388), n images in
+ * one launch; the camera, stroke and blend rules are those of p2pvg_b200/skeleton.py's module docstring.
+ *   poses       [n][J][3] fp32 device poses (x, y, z), plotted at (x, z, y)
+ *   views       [n] int32 device camera view per image, 0..3; an image whose view is outside 0..3 is left white
+ *   J           joints, 2..32; limb l = 0..J-2 joins joint l + 1 to parents_host[l + 1], drawn in that order
+ *   parents_host [J] int32, HOST memory: parents[0] = -1 and 0 <= parents[j] < j
+ *   colors_host [J - 1][3] fp32, HOST memory: limb RGB in 0..1
+ *   matrices_host [4][3][4] fp32, HOST memory: per view rows 0, 1 and 3 of M = P . View . W (the plot limits are in W)
+ *   out_f       [n][3][98][98] fp32 or NULL: float32(q / 255.) of the quantised value q
+ *   out_u8      [n][98][98][3] uint8 or NULL: q = min(255, floor(255 c + 0.5)) of the blended fp32 colour c
+ * Projection and coverage are fp64 with one rounding per operation; blend and quantisation fp32, likewise.  A limb shorter
+ * than 1e-6 px or with a non-finite projected end draws nothing.
+ * n == 0 returns P2PVG_OK without a launch.  P2PVG_ERR_BAD_ARG (nothing launched): n < 0, J outside 2..32, a null table,
+ * null poses / views or both outputs when n > 0, misaligned device pointers, bad parents, a colour outside 0..1, a
+ * non-finite matrix value. */
+int p2pvg_skeleton_render(const float* poses, const int32_t* views, int n, int J, const int32_t* parents_host,
+                          const float* colors_host, const float* matrices_host, float* out_f, uint8_t* out_u8, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

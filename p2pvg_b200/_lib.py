@@ -8,6 +8,7 @@ from __future__ import annotations
 import ctypes
 import os
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -539,6 +540,21 @@ class CudaKernels:
                                           _i(len(tiles_host)), _vp(images_host.ctypes.data), _i(len(images_host)), _p(tables_dev),
                                           _p(out_f), ctypes.c_longlong(0 if out_f is None else out_f.numel()), _p(out_u8),
                                           ctypes.c_longlong(0 if out_u8 is None else out_u8.numel()), self._stream()))
+
+    def skeleton_render(self, poses, views, parents_host, colors_host, matrices_host, out_f, out_u8):
+        """p2pvg_skeleton_render: the skeleton pictures of fp32 poses [n, J, 3] seen from int32 views [n] (device), into
+        out_f fp32 [n, 3, 98, 98] and / or out_u8 uint8 [n, 98, 98, 3]; parents_host int32 [J], colors_host fp32 [J - 1, 3]
+        and matrices_host fp32 [4, 3, 4] are host arrays (checked by the library before the launch)."""
+        n, J = int(poses.shape[0]), int(poses.shape[1])
+        assert poses.dtype == torch.float32 and views.dtype == torch.int32 and poses.is_contiguous() and views.is_contiguous()
+        assert views.numel() == n and parents_host.dtype == np.int32 and len(parents_host) == J
+        assert colors_host.dtype == matrices_host.dtype == np.float32 and colors_host.shape == (J - 1, 3)
+        assert matrices_host.shape == (4, 3, 4) and matrices_host.flags.c_contiguous and colors_host.flags.c_contiguous
+        assert out_f is None or (out_f.dtype == torch.float32 and out_f.is_contiguous() and out_f.numel() == n * 3 * 98 * 98)
+        assert out_u8 is None or (out_u8.dtype == torch.uint8 and out_u8.is_contiguous() and out_u8.numel() == n * 3 * 98 * 98)
+        self._ck(self.lib.p2pvg_skeleton_render(_p(poses), _p(views), _i(n), _i(J), _vp(parents_host.ctypes.data),
+                                                _vp(colors_host.ctypes.data), _vp(matrices_host.ctypes.data), _p(out_f),
+                                                _p(out_u8), self._stream()))
 
     # -- TensorBoard histograms ------------------------------------------------------------
     def histograms_workspace_bytes(self, segs_host, n_edges):

@@ -98,7 +98,7 @@ def check_generate(model, seq, gen_lengths, nsamples, ndisplays):
     1 <= ndisplays <= nsamples.  Makes no draw and no launch."""
     from .gen_engine import check_lengths
     if getattr(model, "is_pose", False):
-        raise ValueError("generate_video draws image frames; h36m poses need the host renderer (misc/visualize.py)")
+        raise ValueError("generate_video draws image frames; h36m poses are drawn by vis_seq (p2pvg_b200.skeleton)")
     if not hasattr(model, "_graphed_engine"):
         raise ValueError("generate_video needs a p2pvg_b200 P2PModel")
     model._graphed_engine()._check_model()
@@ -192,8 +192,8 @@ def read_video(vid_name):
 def backbone_of(opt):
     """The backbone module generate.py picks from a checkpoint's options (:52-66); ValueError for h36m."""
     if opt.dataset == "h36m":
-        raise ValueError("h36m checkpoints are not supported: their pictures need the host pose renderer (the reference's "
-                         "generate.py has no h36m path either)")
+        raise ValueError("h36m checkpoints are not supported: the reference's generate.py reads an mp4 video and has no "
+                         "pose path")
     from .models import dcgan_64, dcgan_128, vgg_64, vgg_128
     nets = {("dcgan", 64): dcgan_64, ("dcgan", 128): dcgan_128, ("vgg", 64): vgg_64, ("vgg", 128): vgg_128}
     net = nets.get((opt.backbone, int(opt.image_width)))

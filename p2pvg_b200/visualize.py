@@ -18,9 +18,12 @@ With skip_frame=True every reference call has its own skip pattern, so the sampl
 Afterwards ``.hidden`` of the LSTMs holds the graph's nsample * n_block rows (the last call's n_block rows with
 skip_frame=True); the reference's leaves the last call's B rows.  ``P2PModel.forward`` does not read it.
 
-Poses (h36m): the n_block displayed sequences are generated graphed, then drawn by ``h36m_visualizer.set_data`` in the
+Poses (h36m): the n_block displayed sequences are generated graphed.  When ``h36m_visualizer`` is a
+``p2pvg_b200.skeleton.Skeleton3DVisualizer`` the pose store (every sample's frames, then the ground truth padded to
+output_len) and each image's camera view are assembled on the device and drawn by ONE p2pvg_skeleton_render launch straight
+into the fp32 frame store, with no pose copied to the host.  Any other visualizer draws them with ``set_data`` in the
 reference's order and with its arguments; the rendered images, scaled as the reference scales them, are uploaded as one
-frame store and composed by the same kernel.
+frame store.  Either store is composed by the same kernel, with the same tile table and the same random draws.
 
 ``check_vis_seq`` raises ValueError, before any draw or launch, for anything this path does not take.
 """
@@ -29,7 +32,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from . import gen_engine, infer
+from . import gen_engine, infer, skeleton
 
 NROW = 6        # rows per block: the ground truth and five samples (misc/visualize.py:105)
 ORANGE, RED = 1, 2
@@ -240,15 +243,21 @@ def vis_seq(model, x, epoch, output_len, model_mode='full', recon_mode=None, ski
             sample_ref = lambda s, t: (1, (s * L + t) * nb)   # noqa: E731
         if pose:
             # the reference's set_data order: every sample's sequences, then the ground truth padded to output_len
-            sp = samples.view(nsample, L, nb, 17, 3)
-            imgs = [_render(h36m_visualizer, sp[s], camera_view, nb) for s in range(nsample)]
             gt = torch.cat([frames, frames[-1:].expand(max(L - seq_len, 0), *frames.shape[1:])])
-            imgs.append(_render(h36m_visualizer, gt, camera_view, nb))
-            C, H, W = imgs[0].shape[2:]
-            if C not in (1, 3) or H != W or H > 128:
-                raise ValueError(f"vis_seq composes 1- or 3-channel square images of at most 128 pixels; the visualizer drew "
-                                 f"{C}x{H}x{W}")
-            store = torch.cat([i.reshape(-1, C, H, W) for i in imgs]).to(dev).contiguous()
+            if isinstance(h36m_visualizer, skeleton.Skeleton3DVisualizer):
+                # the same store drawn on the device: sample s frame t row b at (s L + t) nb + b, then the ground truth
+                poses = torch.cat([samples.reshape(-1, *samples.shape[-2:]), gt.reshape(-1, *gt.shape[-2:]).float()])
+                views = camera_view[:nb].repeat(poses.shape[0] // nb)
+                store, C, H = h36m_visualizer.render_device(poses, views), 3, skeleton.SIZE
+            else:
+                sp = samples.view(nsample, L, nb, 17, 3)
+                imgs = [_render(h36m_visualizer, sp[s], camera_view, nb) for s in range(nsample)]
+                imgs.append(_render(h36m_visualizer, gt, camera_view, nb))
+                C, H, W = imgs[0].shape[2:]
+                if C not in (1, 3) or H != W or H > 128:
+                    raise ValueError(f"vis_seq composes 1- or 3-channel square images of at most 128 pixels; the visualizer "
+                                     f"drew {C}x{H}x{W}")
+                store = torch.cat([i.reshape(-1, C, H, W) for i in imgs]).to(dev).contiguous()
             g0 = nsample * L * nb
             tiles = plan_tiles(seq_len, L, nb, nsample, lambda t: (0, g0 + t * nb), lambda s, t: (0, (s * L + t) * nb))
             canvas, video, gif = compose(store, None, tiles, C, H)
