@@ -27,6 +27,7 @@ import numpy as np
 import torch
 
 from .layouts import cast, implicit_shape, nchw_to_nhwc, pack_conv4, pack_convt4, tile_bias, unpack_conv4, unpack_convt4, up8
+from .models.backbone import STAGE_CHANNELS
 
 ACT_NONE, ACT_LRELU, ACT_TANH = 0, 1, 2
 BN_MOMENTUM = 0.1
@@ -176,10 +177,11 @@ class TrainEngine:
             self.nc, self.W0 = cfg["channels"], cfg["image_width"]
             if self.backbone == "vgg" and self.W0 not in (64, 128):
                 self.W0 = cfg.get("vgg_width", 64)  # fixtures name the backbone in image_width
-            self.chans = [64, 128, 256, 512] if self.W0 == 64 else [64, 128, 256, 512, 512]
-            if self.W0 not in (64, 128):
+            if self.W0 not in STAGE_CHANNELS:
                 raise ValueError("dcgan backbones exist for 64 and 128 pixel frames")
+            self.chans = STAGE_CHANNELS[self.W0]
             self.n = len(self.chans)
+            self.top = f"c{self.n + 1}"   # state-dict prefix of the encoder's 4x4 top layer
             self.frame_elems = self.nc * self.W0 * self.W0
         else:
             self.frame_elems = 51  # h36m pose: 17 joints x 3
@@ -322,14 +324,10 @@ class TrainEngine:
 
     # ------------------------------------------------------------------ weights
     def enc_names(self, l):
-        if l < self.n:
-            return f"c{l + 1}.main.0", f"c{l + 1}.main.1"
-        return f"c{self.n + 1}.0", f"c{self.n + 1}.1"
+        return f"c{l + 1}.main.0", f"c{l + 1}.main.1"
 
     def dec_names(self, k):
-        """k = -1: upc1;  k in [0, n-1]: the stride-2 stages (the last one has no BatchNorm)."""
-        if k < 0:
-            return "upc1.0", "upc1.1"
+        """The stride-2 stages k in [0, n-1] (the last one has no BatchNorm)."""
         if k < self.n - 1:
             return f"upc{k + 2}.main.0", f"upc{k + 2}.main.1"
         return f"upc{self.n + 1}.0", None
@@ -340,7 +338,7 @@ class TrainEngine:
         K = self.K
         if "encoder" in which:
             P = self.arena["encoder"].p
-            for l in range(self.n + 1):
+            for l in range(self.n):
                 w = P[self.enc_names(l)[0] + ".weight"]
                 co, ci = w.shape[0], w.shape[1]
                 wp = self.buf(f"wp_enc{l}", co * 16 * ci)
@@ -352,9 +350,11 @@ class TrainEngine:
                     b4 = self.fbuf("bias4_enc0", 4 * co)
                     tile_bias(K, P[self.enc_names(l)[0] + ".bias"], b4, 4)
                     self._packed["enc0.bd"], self._packed["enc0.bias4"] = bd, b4
+            self.pack_enc_top()
         if "decoder" in which:
+            self.pack_dec_head()
             P = self.arena["decoder"].p
-            for k in range(-1, self.n):
+            for k in range(self.n):
                 cn = self.dec_names(k)[0]
                 w = P[cn + ".weight"]
                 ci, co = w.shape[0], w.shape[1]
@@ -367,10 +367,22 @@ class TrainEngine:
                         bd = self.buf(f"wbd_dec_last{half}", 4 * cd * 64 * co)
                         K.blockdiag(wp[off:], bd, cd, 16 * co, 4)
                         self._packed[f"dec_last.bd{half}"] = bd
-                if k == -1:  # bias of the 1x1 -> 4x4 ConvTranspose, repeated over the 16 taps
-                    b16 = self.fbuf("bias16_upc1", 16 * co)
-                    tile_bias(K, P[cn + ".bias"], b16, 16)
-                    self._packed["dec-1.bias16"] = b16
+
+    def pack_enc_top(self):
+        """pack_conv4 of the encoder's top layer Conv2d(512, g, 4, 1, 0)."""
+        wp = self.buf("wp_enc_top", self.g * 16 * 512)
+        pack_conv4(self.K, self.arena["encoder"].p[self.top + ".0.weight"], wp)
+        self._packed["enc_top"] = wp
+
+    def pack_dec_head(self):
+        """pack_convt4 of the decoder's head upc1 = ConvTranspose2d(g, 512, 4, 1, 0), and its bias repeated over the 16 taps."""
+        P = self.arena["decoder"].p
+        wp = self.buf("wp_dec-1", self.g * 16 * 512)
+        pack_convt4(self.K, P["upc1.0.weight"], wp)
+        self._packed["dec-1"] = wp
+        b16 = self.fbuf("bias16_upc1", 16 * 512)
+        tile_bias(self.K, P["upc1.0.bias"], b16, 16)
+        self._packed["dec-1.bias16"] = b16
 
     def pack_lstm_weights(self, backward=True):
         """Tensor-core (TF32) mode only: K-major fp32 copies of the LSTM weights for the GEMMs whose natural
@@ -767,27 +779,35 @@ class TrainEngine:
             st = self.bn_forward("enc", l, raw, y, T, B * Ho * Ho, cout, P[bn + ".weight"], P[bn + ".bias"], ACT_LRELU, tiles=sp)
             self.enc.append(dict(col=col, raw=raw, y=y, st=st, cin=cin, cout=cout, Hin=H, Hout=Ho, M=M, imp=imp, inp=a))
             a, H = y, Ho
-        # final 4x4 valid conv == GEMM over the flattened 4x4xC map
-        ctop = self.chans[-1]
-        cn, bn = self.enc_names(n)
-        raw = self.buf("enc_rawf", N * self.g)
-        y = self.buf("enc_yf", N * self.g)
-        K.gemm(a, self._packed[f"enc{n}"], raw, N, self.g, 16 * ctop, bias=P[cn + ".bias"])
-        st = self.bn_forward("enc", n, raw, y, T, B, self.g, P[bn + ".weight"], P[bn + ".bias"], ACT_TANH)
+        self.encode_top(a)
+        self.update_running_stats("encoder", "enc_order", [(self.enc_names(l)[1], rec["st"]) for l, rec in enumerate(self.enc)]
+                                  + [(self.top + ".1", self.enc_final["st"])])
+
+    def encode_top(self, a):
+        """The encoder's top layer Conv2d(512, g, 4, 1, 0) + BatchNorm + Tanh on the 4x4x512 maps `a` of all T*B frames, as one
+        GEMM over the flattened map; sets enc_final and the fp32 latents Hlat."""
+        K, N, g = self.K, self.T * self.B, self.g
+        P = self.arena["encoder"].p
+        raw = self.buf("enc_rawf", N * g)
+        y = self.buf("enc_yf", N * g)
+        K.gemm(a, self._packed["enc_top"], raw, N, g, 16 * 512, bias=P[self.top + ".0.bias"])
+        st = self.bn_forward("enc", "top", raw, y, self.T, self.B, g, P[self.top + ".1.weight"], P[self.top + ".1.bias"], ACT_TANH)
         self.enc_final = dict(inp=a, raw=raw, y=y, st=st)
         if self.adt == torch.float32:
             self.Hlat = y
         else:
-            self.Hlat = self.fbuf("Hlat", N * self.g)
-            cast(K, y, self.Hlat, N * self.g)
-        # running statistics: one EMA update per reference call, in call order (training mode only)
-        ncalls = len(plan.enc_order)
-        Bf = self.buffers["encoder"]
-        for l in range(0 if self._eval else n + 1):
-            st = self.enc[l]["st"] if l < n else self.enc_final["st"]
-            bn = self.enc_names(l)[1]
-            K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], st["mean"], st["varu"], self.ix["enc_order"], ncalls,
-                     st["C"], BN_MOMENTUM)
+            self.Hlat = self.fbuf("Hlat", N * g)
+            cast(K, y, self.Hlat, N * g)
+
+    def update_running_stats(self, m, order, bns):
+        """BatchNorm running statistics of module m: for every (layer prefix, bn_forward statistics) in bns, in that order, one
+        EMA update per reference call in the call order self.ix[order].  Nothing in eval mode."""
+        if self._eval:
+            return
+        K, Bf, idx = self.K, self.buffers[m], self.ix[order]
+        ncalls = idx.numel()
+        for bn, st in bns:
+            K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], st["mean"], st["varu"], idx, ncalls, st["C"], BN_MOMENTUM)
             Bf[bn + ".num_batches_tracked"] += ncalls
 
     def stat_buf(self, tag, rows, phases, C, rows_per_group, kred=1 << 30):
@@ -919,22 +939,11 @@ class TrainEngine:
 
     # -- Phase D ----------------------------------------------------------------------------
     def decode(self, plan):
-        K, B, S, n, g = self.K, self.B, self.S, self.n, self.g
+        K, B, S, n = self.K, self.B, self.S, self.n
         G = S + 1
         P = self.arena["decoder"].p
         N = G * B
-        if self.adt == torch.float32:
-            hp = self.h_pred
-        else:
-            hp = self.buf("hp_act", N * g)
-            cast(K, self.h_pred, hp, N * g)
-        ctop = self.chans[-1]
-        cn, bn = self.dec_names(-1)
-        raw = self.buf("dec_raw_1", N * 16 * ctop)
-        d = self.buf("dec_d_1", N * 16 * ctop)
-        K.gemm(hp, self._packed["dec-1"], raw, N, 16 * ctop, g, b_mn=True, bias=self._packed["dec-1.bias16"])
-        st = self.bn_forward("dec", -1, raw, d, G, B * 16, ctop, P[bn + ".weight"], P[bn + ".bias"], ACT_LRELU)
-        self.dec_first = dict(inp=hp, raw=raw, d=d, st=st)
+        d = self.decode_head()
         self.dec = []
         Hi = 4
         nskip = plan.nskip
@@ -980,12 +989,26 @@ class TrainEngine:
                 d = dn
             self.dec.append(rec)
             Hi *= 2
-        Bf = self.buffers["decoder"]
-        for k in range(-1, -1 if self._eval else n - 1):
-            st = self.dec_first["st"] if k < 0 else self.dec[k]["st"]
-            bn = self.dec_names(k)[1]
-            K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], st["mean"], st["varu"], self.ix["dec_order"], G, st["C"], BN_MOMENTUM)
-            Bf[bn + ".num_batches_tracked"] += G
+        self.update_running_stats("decoder", "dec_order", [("upc1.1", self.dec_first["st"])]
+                                  + [(self.dec_names(k)[1], self.dec[k]["st"]) for k in range(n - 1)])
+
+    def decode_head(self):
+        """The decoder's head upc1 = ConvTranspose2d(g, 512, 4, 1, 0) + BatchNorm + LeakyReLU on the latents h_pred of all S+1
+        calls, as one GEMM; sets dec_first and returns the 4x4x512 maps."""
+        K, B, g, G = self.K, self.B, self.g, self.S + 1
+        P = self.arena["decoder"].p
+        N = G * B
+        if self.adt == torch.float32:
+            hp = self.h_pred
+        else:
+            hp = self.buf("hp_act", N * g)
+            cast(K, self.h_pred, hp, N * g)
+        raw = self.buf("dec_raw_1", N * 16 * 512)
+        d = self.buf("dec_d_1", N * 16 * 512)
+        K.gemm(hp, self._packed["dec-1"], raw, N, 16 * 512, g, b_mn=True, bias=self._packed["dec-1.bias16"])
+        st = self.bn_forward("dec", -1, raw, d, G, B * 16, 512, P["upc1.1.weight"], P["upc1.1.bias"], ACT_LRELU)
+        self.dec_first = dict(inp=hp, raw=raw, d=d, st=st)
+        return d
 
     def losses_fwd(self, plan):
         K, B, S = self.K, self.B, self.S
@@ -1009,7 +1032,7 @@ class TrainEngine:
     def decoder_backward(self, g0, g1, want_wgrad, want_skip):
         """Backward of the decoder calls [g0, g1).  Seeds: d_rawout.  Produces d_hpred[g0:g1] (fp32) and,
         if requested, weight gradients (into the decoder grad arena) and the skip gradients."""
-        K, B, n, g = self.K, self.B, self.n, self.g
+        K, B, n = self.K, self.B, self.n
         Gn = g1 - g0
         N = Gn * B
         A = self.arena["decoder"]
@@ -1102,26 +1125,32 @@ class TrainEngine:
                 elif want_wgrad:
                     unpack_convt4(K, gw, A.g[cn + ".weight"])
             dy = dd
-        # upc1: BatchNorm + LeakyReLU, then the g -> 4x4xCtop GEMM
-        ctop = self.chans[-1]
-        cn, bn = self.dec_names(-1)
+        self.decode_head_backward(dy, g0, g1, want_wgrad)
+
+    def decode_head_backward(self, dy, g0, g1, want_wgrad):
+        """Backward of upc1 for the decoder calls [g0, g1): dy (gradient of its 4x4x512 output maps, overwritten) -> d_hpred[g0:g1]
+        (fp32) and, with want_wgrad, its parameter gradients."""
+        K, B, g = self.K, self.B, self.g
+        Gn = g1 - g0
+        N = Gn * B
+        A = self.arena["decoder"]
         st = self.dec_first["st"]
-        sl = slice(g0 * B * 16 * ctop, g1 * B * 16 * ctop)
-        c0, c1 = g0 * ctop, g1 * ctop
-        self.bn_backward(dy, self.dec_first["raw"][sl], self.dec_first["d"][sl], st, c0, c1, Gn, B * 16, ctop, ACT_LRELU)
+        sl = slice(g0 * B * 16 * 512, g1 * B * 16 * 512)
+        c0, c1 = g0 * 512, g1 * 512
+        self.bn_backward(dy, self.dec_first["raw"][sl], self.dec_first["d"][sl], st, c0, c1, Gn, B * 16, 512, ACT_LRELU)
         hp = self.dec_first["inp"][g0 * B * g:g1 * B * g]
         if want_wgrad:
-            K.bn_param_grad(st["sdz"][c0:c1], st["sdzx"][c0:c1], Gn, ctop, A.g[bn + ".weight"], A.g[bn + ".bias"])
-            A.g[cn + ".bias"].zero_()
-            gw = self.fbuf("gwp_dec-1", g * 16 * ctop)
-            K.gemm(hp, dy, gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-            unpack_convt4(K, gw, A.g[cn + ".weight"])
+            K.bn_param_grad(st["sdz"][c0:c1], st["sdzx"][c0:c1], Gn, 512, A.g["upc1.1.weight"], A.g["upc1.1.bias"])
+            A.g["upc1.0.bias"].zero_()   # bias feeding a training-mode BatchNorm: gradient is exactly zero
+            gw = self.fbuf("gwp_dec-1", g * 16 * 512)
+            K.gemm(hp, dy, gw, g, 16 * 512, N, a_mn=True, b_mn=True, lda=g, ldb=16 * 512)
+            unpack_convt4(K, gw, A.g["upc1.0.weight"])
         dhp = self.d_hpred[g0 * B * g:g1 * B * g]
         if self.adt == torch.float32:
-            K.gemm(dy, self._packed["dec-1"], dhp, N, g, 16 * ctop)
+            K.gemm(dy, self._packed["dec-1"], dhp, N, g, 16 * 512)
         else:
             tmp = self.buf("dhp_act", N * g)
-            K.gemm(dy, self._packed["dec-1"], tmp, N, g, 16 * ctop)
+            K.gemm(dy, self._packed["dec-1"], tmp, N, g, 16 * 512)
             cast(K, tmp, dhp, N * g)
 
     def bn_backward(self, dy, raw, y, st, c0, c1, G, R, C, act):
@@ -1261,28 +1290,13 @@ class TrainEngine:
         K.gather_add_cols(self.dH, dXpred, ix["in_idx"], S, T, B, g, wp, 0)
 
     def encoder_backward(self, plan):
-        K, T, B, n, g = self.K, self.T, self.B, self.n, self.g
+        K, T, B, n = self.K, self.T, self.B, self.n
         A = self.arena["encoder"]
         N = T * B
         nskip = plan.nskip
         self.join(self.LANE_WGRAD)   # the lane-2 weight-gradient work is ordered before the encoder backward
-        if self.adt == torch.float32:
-            dy = self.dH
-        else:
-            dy = self.buf("dH_act", N * g)
-            cast(K, self.dH, dy, N * g)
-        cn, bn = self.enc_names(n)
-        fin = self.enc_final
-        st = fin["st"]
-        K.bn_bwd(dy, fin["raw"], fin["y"], st["mean"], st["invstd"], st["gamma"], T, B, g, ACT_TANH, dy, st["sdz"], st["sdzx"])
-        K.bn_param_grad(st["sdz"], st["sdzx"], T, g, A.g[bn + ".weight"], A.g[bn + ".bias"])
-        A.g[cn + ".bias"].zero_()
-        ctop = self.chans[-1]
-        gw = self.fbuf(f"gwp_enc{n}", g * 16 * ctop)
-        K.gemm(dy, fin["inp"], gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-        unpack_conv4(K, gw, A.g[cn + ".weight"])
-        gy = self.buf(f"enc_gy{n - 1}", N * 16 * ctop)
-        K.gemm(dy, self._packed[f"enc{n}"], gy, N, 16 * ctop, g, b_mn=True)
+        gy = self.buf(f"enc_gy{n - 1}", N * 16 * 512)
+        self.encode_top_backward(gy)
         for l in range(n - 1, -1, -1):
             rec = self.enc[l]
             cin, cout, M, Ho = rec["cin"], rec["cout"], rec["M"], rec["Hout"]
@@ -1319,6 +1333,26 @@ class TrainEngine:
                     K.gemm(gy, self._packed[f"enc{l}"], dcol, M, 16 * cin, cout, b_mn=True)
                     K.col2im(dcol, gprev, N, Ho, Ho, cin)
                 gy = gprev
+
+    def encode_top_backward(self, gy):
+        """Backward of the encoder's top layer: dH -> its parameter gradients and gy, the gradient of its 4x4x512 input maps."""
+        K, T, B, g = self.K, self.T, self.B, self.g
+        N = T * B
+        A = self.arena["encoder"]
+        if self.adt == torch.float32:
+            dy = self.dH
+        else:
+            dy = self.buf("dH_act", N * g)
+            cast(K, self.dH, dy, N * g)
+        fin = self.enc_final
+        st = fin["st"]
+        K.bn_bwd(dy, fin["raw"], fin["y"], st["mean"], st["invstd"], st["gamma"], T, B, g, ACT_TANH, dy, st["sdz"], st["sdzx"])
+        K.bn_param_grad(st["sdz"], st["sdzx"], T, g, A.g[self.top + ".1.weight"], A.g[self.top + ".1.bias"])
+        A.g[self.top + ".0.bias"].zero_()
+        gw = self.fbuf("gwp_enc_top", g * 16 * 512)
+        K.gemm(dy, fin["inp"], gw, g, 16 * 512, N, a_mn=True, b_mn=True, lda=g, ldb=16 * 512)
+        unpack_conv4(K, gw, A.g[self.top + ".0.weight"])
+        K.gemm(dy, self._packed["enc_top"], gy, N, 16 * 512, g, b_mn=True)
 
     def backward_prior(self, plan):
         """prior_loss = kld + weight_cpc*cpc (models/p2p_model.py:266-268): CPC chain through decoder and

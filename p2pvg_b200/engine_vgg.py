@@ -17,9 +17,8 @@ from __future__ import annotations
 
 import torch
 
-from .engine import ACT_LRELU, ACT_TANH, BN_MOMENTUM, TrainEngine
-from .layouts import cast, implicit_shape, pack_conv3, pack_conv3_t, pack_conv4, pack_convt4, tile_bias, unpack_conv3, \
-    unpack_conv4, unpack_convt4, up8
+from .engine import ACT_LRELU, TrainEngine
+from .layouts import implicit_shape, pack_conv3, pack_conv3_t, unpack_conv3, up8
 
 VGG_ENC = [[(None, 64), (64, 64)], [(64, 128), (128, 128)], [(128, 256), (256, 256), (256, 256)], [(256, 512), (512, 512), (512, 512)]]
 VGG_DEC = [[(1024, 512), (512, 512), (512, 256)], [(512, 256), (256, 256), (256, 128)], [(256, 128), (128, 64)], [(128, 64)]]
@@ -28,27 +27,33 @@ VGG_ENC_128 = VGG_ENC + [[(512, 512), (512, 512), (512, 512)]]
 VGG_DEC_128 = [[(1024, 512), (512, 512), (512, 512)]] + VGG_DEC
 
 
+def vgg_tables(width):
+    """(encoder, decoder) stage tables of the vgg backbone for width x width frames (vgg_64 or vgg_128)."""
+    if width not in (64, 128):
+        raise ValueError("vgg backbones exist for 64x64 (vgg_64) and 128x128 (vgg_128) frames")
+    return (VGG_ENC_128, VGG_DEC_128) if width == 128 else (VGG_ENC, VGG_DEC)
+
+
+def vgg_layers(width, nc):
+    """The 3x3 layers of the vgg backbone as two lists of (stage, index, cin, cout, state-dict prefix of the vgg_layer's
+    ``main``): the encoder's, then the decoder's (cin of a decoder stage's first layer counts both torch.cat halves)."""
+    ENC, DEC = vgg_tables(width)
+    enc = [(i, j, nc if cin is None else cin, cout, f"c{i + 1}.{j}.main")
+           for i, stage in enumerate(ENC) for j, (cin, cout) in enumerate(stage)]
+    dec = [(k, j, cin, cout, f"upc{k + 2}.{j}.main") for k, stage in enumerate(DEC) for j, (cin, cout) in enumerate(stage)]
+    return enc, dec
+
+
 class TrainEngineVGG(TrainEngine):
     def __init__(self, *a, **kw):
         super().__init__(*a, **kw)
-        if self.W0 not in (64, 128):
-            raise ValueError("vgg backbones exist for 64x64 (vgg_64) and 128x128 (vgg_128) frames")
-        self.ENC, self.DEC = (VGG_ENC_128, VGG_DEC_128) if self.W0 == 128 else (VGG_ENC, VGG_DEC)
+        self.ENC, self.DEC = vgg_tables(self.W0)
+        self.enc_layers, self.dec_layers = vgg_layers(self.W0, self.nc)
         self.nst = len(self.ENC)                 # stages; the final 4x4 conv is c{nst+1}, the last decoder block upc{nst+1}
         self.top, self.last = f"c{self.nst + 1}", f"upc{self.nst + 1}"
         self.ldl = up8(9 * self.nc)  # row pitch of the last layer's [pix, 9*nc] matrix
 
     # ------------------------------------------------------------------ weights
-    def enc_layers(self):
-        for i, stage in enumerate(self.ENC):
-            for j, (cin, cout) in enumerate(stage):
-                yield i, j, (self.nc if cin is None else cin), cout, f"c{i + 1}.{j}.main"
-
-    def dec_layers(self):
-        for k, stage in enumerate(self.DEC):
-            for j, (cin, cout) in enumerate(stage):
-                yield k, j, cin, cout, f"upc{k + 2}.{j}.main"
-
     def _pack_conv3(self, key, w, c0, cin, want_t=True):
         """pack_conv3 and (want_t) pack_conv3_t of input channels [c0, c0+cin); thin inputs are packed via the wp_ scratch."""
         K = self.K
@@ -68,22 +73,13 @@ class TrainEngineVGG(TrainEngine):
         K = self.K
         if "encoder" in which:
             P = self.arena["encoder"].p
-            for i, j, cin, cout, pre in self.enc_layers():
+            for i, j, cin, cout, pre in self.enc_layers:
                 self._pack_conv3(f"enc.{i}.{j}", P[pre + ".0.weight"], 0, cin, want_t=backward and not (i == 0 and j == 0))
-            w = P[self.top + ".0.weight"]
-            wp = self.buf("wp_enc_c5", self.g * 16 * 512)
-            pack_conv4(K, w, wp)
-            self._packed["enc.c5"] = wp
+            self.pack_enc_top()
         if "decoder" in which:
+            self.pack_dec_head()
             P = self.arena["decoder"].p
-            w = P["upc1.0.weight"]
-            wp = self.buf("wp_dec-1", self.g * 16 * 512)
-            pack_convt4(K, w, wp)
-            self._packed["dec-1"] = wp
-            b16 = self.fbuf("bias16_upc1", 16 * 512)
-            tile_bias(K, P["upc1.0.bias"], b16, 16)
-            self._packed["dec-1.bias16"] = b16
-            for k, j, cin, cout, pre in self.dec_layers():
+            for k, j, cin, cout, pre in self.dec_layers:
                 w = P[pre + ".0.weight"]
                 if j == 0:
                     C = cin // 2
@@ -140,7 +136,7 @@ class TrainEngineVGG(TrainEngine):
         a = self.frames_nhwc(x)
         self.venc = [[] for _ in self.ENC]
         H, C = self.W0, nc
-        for i, j, cin, cout, pre in self.enc_layers():
+        for i, j, cin, cout, pre in self.enc_layers:
             if j == 0 and i > 0:
                 pooled = self.buf(f"venc_pool{i}", N * (H // 2) * (H // 2) * C)
                 K.maxpool2_fwd(a, pooled, N, H, H, C)
@@ -155,44 +151,22 @@ class TrainEngineVGG(TrainEngine):
             a, C = y, cout
         pooled = self.buf("venc_pool_top", N * 16 * 512)
         K.maxpool2_fwd(a, pooled, N, 8, 8, 512)
-        raw = self.buf("enc_rawf", N * self.g)
-        y = self.buf("enc_yf", N * self.g)
-        K.gemm(pooled, self._packed["enc.c5"], raw, N, self.g, 16 * 512, bias=P[self.top + ".0.bias"])
-        st = self.bn_forward("venc", "f", raw, y, T, B, self.g, P[self.top + ".1.weight"], P[self.top + ".1.bias"], ACT_TANH)
-        self.enc_final = dict(inp=pooled, raw=raw, y=y, st=st)
-        if self.adt == torch.float32:
-            self.Hlat = y
-        else:
-            self.Hlat = self.fbuf("Hlat", N * self.g)
-            cast(K, y, self.Hlat, N * self.g)
-        ncalls = len(plan.enc_order)
-        Bf = self.buffers["encoder"]
-        bns = [(rec["pre"] + ".1", rec["st"]) for recs in self.venc for rec in recs] + [(self.top + ".1", st)]
-        for bn, s in ([] if self._eval else bns):   # running statistics: training mode only
-            K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], s["mean"], s["varu"], self.ix["enc_order"], ncalls, s["C"], BN_MOMENTUM)
-            Bf[bn + ".num_batches_tracked"] += ncalls
+        self.encode_top(pooled)
+        self.update_running_stats("encoder", "enc_order", [(rec["pre"] + ".1", rec["st"]) for recs in self.venc for rec in recs]
+                                  + [(self.top + ".1", self.enc_final["st"])])
 
     # ------------------------------------------------------------------ Phase D
     def decode(self, plan):
-        K, B, S, g, nc = self.K, self.B, self.S, self.g, self.nc
+        K, B, S, nc = self.K, self.B, self.S, self.nc
         G = S + 1
         P = self.arena["decoder"].p
         N = G * B
-        if self.adt == torch.float32:
-            hp = self.h_pred
-        else:
-            hp = self.buf("hp_act", N * g)
-            cast(K, self.h_pred, hp, N * g)
-        raw = self.buf("dec_raw_1", N * 16 * 512)
-        d = self.buf("dec_d_1", N * 16 * 512)
-        K.gemm(hp, self._packed["dec-1"], raw, N, 16 * 512, g, b_mn=True, bias=self._packed["dec-1.bias16"])
-        st = self.bn_forward("dec", -1, raw, d, G, B * 16, 512, P["upc1.1.weight"], P["upc1.1.bias"], ACT_LRELU)
-        self.dec_first = dict(inp=hp, raw=raw, d=d, st=st)
+        d = self.decode_head()
         nskip = plan.nskip
         self.vdec = [[] for _ in self.DEC]
         H, C = 4, 512
         a = d
-        for k, j, cin, cout, pre in self.dec_layers():
+        for k, j, cin, cout, pre in self.dec_layers:
             M = N * (2 * H if j == 0 else H) ** 2
             if j == 0:
                 H *= 2
@@ -226,15 +200,12 @@ class TrainEngineVGG(TrainEngine):
         K.col2im3(colT, raw_out, N, W0, W0, nc, ldl, bias=P[self.last + ".1.bias"])
         self.vlast = dict(inp=a)
         self.dec = [dict(raw=raw_out)]
-        Bf = self.buffers["decoder"]
-        bns = [("upc1.1", st)] + [(rec["pre"] + ".1", rec["st"]) for recs in self.vdec for rec in recs]
-        for bn, s in ([] if self._eval else bns):
-            K.bn_ema(Bf[bn + ".running_mean"], Bf[bn + ".running_var"], s["mean"], s["varu"], self.ix["dec_order"], G, s["C"], BN_MOMENTUM)
-            Bf[bn + ".num_batches_tracked"] += G
+        self.update_running_stats("decoder", "dec_order", [("upc1.1", self.dec_first["st"])]
+                                  + [(rec["pre"] + ".1", rec["st"]) for recs in self.vdec for rec in recs])
 
     # ------------------------------------------------------------------ backward
     def decoder_backward(self, g0, g1, want_wgrad, want_skip):
-        K, B, g, nc = self.K, self.B, self.g, self.nc
+        K, B, nc = self.K, self.B, self.nc
         Gn = g1 - g0
         N = Gn * B
         A = self.arena["decoder"]
@@ -298,47 +269,15 @@ class TrainEngineVGG(TrainEngine):
                         self.conv3_wgrad(dy, x_in, gw, N, H, cout, cin)
                         unpack_conv3(K, gw, A.g[pre + ".0.weight"])
                     dy = dprev
-        # upc1: BatchNorm + LeakyReLU, then the g -> 4x4x512 GEMM
-        ctop = 512
-        st = self.dec_first["st"]
-        sl = slice(g0 * B * 16 * ctop, g1 * B * 16 * ctop)
-        c0, c1 = g0 * ctop, g1 * ctop
-        self.bn_backward(dy, self.dec_first["raw"][sl], self.dec_first["d"][sl], st, c0, c1, Gn, B * 16, ctop, ACT_LRELU)
-        hp = self.dec_first["inp"][g0 * B * g:g1 * B * g]
-        if want_wgrad:
-            K.bn_param_grad(st["sdz"][c0:c1], st["sdzx"][c0:c1], Gn, ctop, A.g["upc1.1.weight"], A.g["upc1.1.bias"])
-            A.g["upc1.0.bias"].zero_()
-            gw = self.fbuf("gwp_dec-1", g * 16 * ctop)
-            K.gemm(hp, dy, gw, g, 16 * ctop, N, a_mn=True, b_mn=True, lda=g, ldb=16 * ctop)
-            unpack_convt4(K, gw, A.g["upc1.0.weight"])
-        dhp = self.d_hpred[g0 * B * g:g1 * B * g]
-        if self.adt == torch.float32:
-            K.gemm(dy, self._packed["dec-1"], dhp, N, g, 16 * ctop)
-        else:
-            tmp = self.buf("dhp_act", N * g)
-            K.gemm(dy, self._packed["dec-1"], tmp, N, g, 16 * ctop)
-            cast(K, tmp, dhp, N * g)
+        self.decode_head_backward(dy, g0, g1, want_wgrad)
 
     def encoder_backward(self, plan):
-        K, T, B, g = self.K, self.T, self.B, self.g
+        K, T, B = self.K, self.T, self.B
         A = self.arena["encoder"]
         N = T * B
         nskip = plan.nskip
-        if self.adt == torch.float32:
-            dy = self.dH
-        else:
-            dy = self.buf("dH_act", N * g)
-            cast(K, self.dH, dy, N * g)
-        fin = self.enc_final
-        st = fin["st"]
-        K.bn_bwd(dy, fin["raw"], fin["y"], st["mean"], st["invstd"], st["gamma"], T, B, g, ACT_TANH, dy, st["sdz"], st["sdzx"])
-        K.bn_param_grad(st["sdz"], st["sdzx"], T, g, A.g[self.top + ".1.weight"], A.g[self.top + ".1.bias"])
-        A.g[self.top + ".0.bias"].zero_()
-        gw = self.fbuf("gwp_enc_c5", g * 16 * 512)
-        K.gemm(dy, fin["inp"], gw, g, 16 * 512, N, a_mn=True, b_mn=True, lda=g, ldb=16 * 512)
-        unpack_conv4(K, gw, A.g[self.top + ".0.weight"])
         gy = self.buf("venc_gpool4", N * 16 * 512)
-        K.gemm(dy, self._packed["enc.c5"], gy, N, 16 * 512, g, b_mn=True)
+        self.encode_top_backward(gy)
         for i in range(self.nst - 1, -1, -1):
             recs = self.venc[i]
             top = recs[-1]

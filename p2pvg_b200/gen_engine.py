@@ -682,33 +682,18 @@ class GenerateEngine:
         adt = G.cfg["adt"]
         enc, dec = model.encoder, model.decoder
         self.chans = infer._stages(enc)
-        chans, n, g = self.chans, len(self.chans), model.g_dim
+        n = len(self.chans)
         self.wp, self.bn = {}, {}
-
-        def coeffs(tag, bn):
-            C = bn.weight.numel()
-            sc, sh = self._buf(G, f"bn_{tag}_scale", C), self._buf(G, f"bn_{tag}_shift", C)
-            K.bn_eval_coeffs(bn.weight.data, bn.bias.data, bn.running_mean, bn.running_var, C, sc, sh, eps=bn.eps)
-            self.bn[tag] = (sc, sh)
-
         cin = enc.nc
-        for l in range(n + 1):
-            blk = getattr(enc, f"c{l + 1}")
-            conv, bn = (blk.main[0], blk.main[1]) if l < n else (blk[0], blk[1])
+        for l in range(n):
+            conv, bn = getattr(enc, f"c{l + 1}").main[:2]
             cout = conv.weight.shape[0]
             wp = self._buf(G, f"wp_enc{l}", cout * 16 * cin, adt)
             pack_conv4(K, conv.weight.data, wp)
             self.wp[f"enc{l}"] = wp
-            coeffs(f"enc{l}", bn)
+            self._bn_coeffs(f"enc{l}", bn)
             cin = cout
-        ctop = chans[-1]
-        convt, bn = dec.upc1[0], dec.upc1[1]
-        wp = self._buf(G, "wp_dec-1", g * 16 * ctop, adt)
-        pack_convt4(K, convt.weight.data, wp)
-        b16 = self._buf(G, "bias16_dec-1", 16 * ctop)
-        tile_bias(K, convt.bias.data, b16, 16)
-        self.wp["dec-1"], self.wp["dec-1.bias16"] = wp, b16
-        coeffs("dec-1", bn)
+        self._prepare_latent(getattr(enc, f"c{n + 1}"), dec.upc1)
         for k in range(n):
             last = k == n - 1
             blk = getattr(dec, f"upc{k + 2}")
@@ -718,7 +703,31 @@ class GenerateEngine:
             pack_convt4(K, convt.weight.data, wp)
             self.wp[f"dec{k}"] = wp
             if not last:
-                coeffs(f"dec{k}", blk.main[1])
+                self._bn_coeffs(f"dec{k}", blk.main[1])
+
+    def _bn_coeffs(self, tag, bn):
+        """Eval-mode scale / shift of BatchNorm module bn from its running statistics, into self.bn[tag]."""
+        G, C = self.G, bn.weight.numel()
+        sc, sh = self._buf(G, f"bn_{tag}_scale", C), self._buf(G, f"bn_{tag}_shift", C)
+        self.K.bn_eval_coeffs(bn.weight.data, bn.bias.data, bn.running_mean, bn.running_var, C, sc, sh, eps=bn.eps)
+        self.bn[tag] = (sc, sh)
+
+    def _prepare_latent(self, top, upc1):
+        """Weights and eval-BatchNorm coefficients of the two latent layers both image backbones share: the encoder's top
+        ``top`` = Conv2d(512, g, 4, 1, 0) + BatchNorm + Tanh and the decoder's head ``upc1`` = ConvTranspose2d(g, 512, 4, 1, 0) +
+        BatchNorm + LeakyReLU."""
+        K, G, g = self.K, self.G, self.model.g_dim
+        adt = G.cfg["adt"]
+        wp = self._buf(G, "wp_enc_top", g * 16 * 512, adt)
+        pack_conv4(K, top[0].weight.data, wp)
+        self.wp["enc_top"] = wp
+        self._bn_coeffs("enc_top", top[1])
+        wp = self._buf(G, "wp_dec-1", g * 16 * 512, adt)
+        pack_convt4(K, upc1[0].weight.data, wp)
+        b16 = self._buf(G, "bias16_dec-1", 16 * 512)
+        tile_bias(K, upc1[0].bias.data, b16, 16)
+        self.wp["dec-1"], self.wp["dec-1.bias16"] = wp, b16
+        self._bn_coeffs("dec-1", upc1[1])
 
     # ------------------------------------------------------------------ encoder / decoder
     def _encode(self, tag, frames, N, h_out):
@@ -747,16 +756,20 @@ class GenerateEngine:
                 K.bn_act(raw, y, sc, sh, 1, M, cout, ACT_LRELU)
             skips.append(y)
             a, H, cin = y, Ho, cout
-        conv = getattr(enc, f"c{len(self.chans) + 1}")[0]
-        g = model.g_dim
-        sc, sh = self.bn[f"enc{len(self.chans)}"]
+        self._encode_top(tag, a, N, h_out, getattr(enc, f"c{len(self.chans) + 1}")[0].bias)
+        return skips
+
+    def _encode_top(self, tag, a, N, h_out, bias):
+        """The encoder's top layer (bias: its conv bias) on the 4x4x512 maps a [N, 4, 4, 512] -> h_out fp32 [N, g]."""
+        K, G, g = self.K, self.G, self.model.g_dim
+        adt = G.cfg["adt"]
+        sc, sh = self.bn["enc_top"]
         raw = self._buf(G, f"{tag}_enc_rawf", N * g, adt)
         y = h_out if adt == torch.float32 else self._buf(G, f"{tag}_enc_yf", N * g, adt)
-        K.gemm(a, self.wp[f"enc{len(self.chans)}"], raw, N, g, 16 * cin, bias=conv.bias.data)
+        K.gemm(a, self.wp["enc_top"], raw, N, g, 16 * 512, bias=bias.data)
         K.bn_act(raw, y, sc, sh, 1, N, g, ACT_TANH)
         if y is not h_out:
             cast(K, y, h_out, N * g)
-        return skips
 
     def _skip_halves(self, tag, skips, nsrc):
         """The skip half of every decoder stage's torch.cat([d, skip]) ConvTranspose for one skip source of nsrc images:
@@ -786,19 +799,10 @@ class GenerateEngine:
         """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied), on the first rows rows."""
         K, G, model = self.K, self.G, self.model
         adt = G.cfg["adt"]
-        dec, g = model.decoder, model.g_dim
+        dec = model.decoder
         n = len(self.chans)
-        ctop = self.chans[-1]
-        if adt == torch.float32:
-            hp = h_pred
-        else:
-            hp = self._buf(G, "dec_hp", rows * g, adt)
-            cast(K, h_pred, hp, rows * g)
-        raw = self._buf(G, "dec_raw-1", rows * 16 * ctop, adt)
-        d = self._buf(G, "dec_d-1", rows * 16 * ctop, adt)
-        K.gemm(hp, self.wp["dec-1"], raw, rows, 16 * ctop, g, b_mn=True, bias=self.wp["dec-1.bias16"])
-        sc, sh = self.bn["dec-1"]
-        K.bn_act(raw, d, sc, sh, 1, rows * 16, ctop, ACT_LRELU)
+        d = self._buf(G, "dec_d-1", rows * 16 * 512, adt)
+        self._decode_head(h_pred, rows, self._buf(G, "dec_raw-1", rows * 16 * 512, adt), d)
         Hi = 4
         for k in range(n):
             last = k == n - 1
@@ -830,6 +834,20 @@ class GenerateEngine:
         cast(K, d, out32, rows * W * W * nc)
         K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
         nhwc_to_nchw(K, out32, frame_out, rows, W * W, nc)
+
+    def _decode_head(self, h_pred, rows, raw, d):
+        """The decoder's head upc1 on the first rows rows of h_pred fp32 [rows, g] -> d [rows, 4, 4, 512] (raw: its
+        pre-BatchNorm scratch of the same size)."""
+        K, G, g = self.K, self.G, self.model.g_dim
+        adt = G.cfg["adt"]
+        if adt == torch.float32:
+            hp = h_pred
+        else:
+            hp = self._buf(G, "dec_hp", rows * g, adt)
+            cast(K, h_pred, hp, rows * g)
+        K.gemm(hp, self.wp["dec-1"], raw, rows, 16 * 512, g, b_mn=True, bias=self.wp["dec-1.bias16"])
+        sc, sh = self.bn["dec-1"]
+        K.bn_act(raw, d, sc, sh, 1, rows * 16, 512, ACT_LRELU)
 
     # ------------------------------------------------------------------ recurrent modules
     def _module(self, m, seg_a, idx_a, seg_b, idx_b, gb, tuc, dt, counter_rows, eps=None, out=None):

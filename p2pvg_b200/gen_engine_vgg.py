@@ -26,10 +26,10 @@ from __future__ import annotations
 
 import torch
 
-from ._lib import ACT_LRELU, ACT_TANH
-from .engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128
+from ._lib import ACT_LRELU
+from .engine_vgg import vgg_layers, vgg_tables
 from .gen_engine import GenerateEngine, _check_eval
-from .layouts import cast, pack_conv3, pack_conv4, pack_convt4, tile_bias
+from .layouts import pack_conv3
 
 
 class VggGenerateEngine(GenerateEngine):
@@ -61,22 +61,7 @@ class VggGenerateEngine(GenerateEngine):
                              "backbone (expected [B, nc, W, W])")
         return (nc, W, W)
 
-    # ------------------------------------------------------------------ layers and buffers
-    def _enc_layers(self):
-        """(stage i, index j, cin, cout, vgg_layer.main) of every 3x3 encoder layer, in order."""
-        enc = self.model.encoder
-        for i, stage in enumerate(self.ENC):
-            for j, (cin, cout) in enumerate(stage):
-                yield i, j, enc.nc if cin is None else cin, cout, getattr(enc, f"c{i + 1}")[j].main
-
-    def _dec_layers(self):
-        """(stage k, index j, cin, cout, vgg_layer.main) of every 3x3 decoder layer; cin of j = 0 counts both cat halves."""
-        dec = self.model.decoder
-        for k, stage in enumerate(self.DEC):
-            blk = getattr(dec, f"upc{k + 2}")
-            for j, (cin, cout) in enumerate(stage):
-                yield k, j, cin, cout, blk[j].main
-
+    # ------------------------------------------------------------------ buffers
     def _scratch(self, name, numel):
         """The first numel elements of scratch buffer `name` (activation dtype).  A buffer grows to the largest request of
         the signature's uncaptured warm-up run, so the captured run never allocates."""
@@ -109,53 +94,41 @@ class VggGenerateEngine(GenerateEngine):
     def _prepare_weights(self):
         K, G, model = self.K, self.G, self.model
         adt = G.cfg["adt"]
-        enc, dec, g = model.encoder, model.decoder, model.g_dim
-        self.ENC, self.DEC = (VGG_ENC_128, VGG_DEC_128) if enc.image_width == 128 else (VGG_ENC, VGG_DEC)
+        enc, dec = model.encoder, model.decoder
+        self.ENC, self.DEC = vgg_tables(enc.image_width)
+        enc_layers, dec_layers = vgg_layers(enc.image_width, enc.nc)
+        # (stage, index, cin, cout, vgg_layer.main) of every 3x3 layer; cin of a decoder stage's first layer counts both cat halves
+        self.enc_layers = [(i, j, cin, cout, enc.get_submodule(pre)) for i, j, cin, cout, pre in enc_layers]
+        self.dec_layers = [(k, j, cin, cout, dec.get_submodule(pre)) for k, j, cin, cout, pre in dec_layers]
         self.wp, self.bn = {}, {}
-
-        def coeffs(tag, bn):
-            C = bn.weight.numel()
-            sc, sh = self._buf(G, f"bn_{tag}_scale", C), self._buf(G, f"bn_{tag}_shift", C)
-            K.bn_eval_coeffs(bn.weight.data, bn.bias.data, bn.running_mean, bn.running_var, C, sc, sh, eps=bn.eps)
-            self.bn[tag] = (sc, sh)
 
         def pack3(tag, conv, c0, cin, cout):
             wp = self._buf(G, f"wp_{tag}", cout * 9 * cin, adt)
             pack_conv3(K, conv.weight.data, wp, c0, cin)
             self.wp[tag] = wp
 
-        for i, j, cin, cout, m in self._enc_layers():
+        for i, j, cin, cout, m in self.enc_layers:
             if i or j:   # the first layer reads its fp32 weight in place (p2pvg_vgg_first_eval)
                 pack3(f"enc{i}_{j}", m[0], 0, cin, cout)
-            coeffs(f"enc{i}_{j}", m[1])
-        top = getattr(enc, f"c{len(self.ENC) + 1}")
-        wp = self._buf(G, "wp_encf", g * 16 * 512, adt)
-        pack_conv4(K, top[0].weight.data, wp)
-        self.wp["encf"] = wp
-        coeffs("encf", top[1])
-        wp = self._buf(G, "wp_dec-1", g * 16 * 512, adt)
-        pack_convt4(K, dec.upc1[0].weight.data, wp)
-        b16 = self._buf(G, "bias16_dec-1", 16 * 512)
-        tile_bias(K, dec.upc1[0].bias.data, b16, 16)
-        self.wp["dec-1"], self.wp["dec-1.bias16"] = wp, b16
-        coeffs("dec-1", dec.upc1[1])
-        for k, j, cin, cout, m in self._dec_layers():
+            self._bn_coeffs(f"enc{i}_{j}", m[1])
+        self._prepare_latent(getattr(enc, f"c{len(self.ENC) + 1}"), dec.upc1)
+        for k, j, cin, cout, m in self.dec_layers:
             if j == 0:   # torch.cat([up(d), skip], 1): the two input-channel halves of the weight
                 pack3(f"dec{k}_0D", m[0], 0, cin // 2, cout)
                 pack3(f"dec{k}_0S", m[0], cin // 2, cin // 2, cout)
             else:
                 pack3(f"dec{k}_{j}", m[0], 0, cin, cout)
-            coeffs(f"dec{k}_{j}", m[1])
+            self._bn_coeffs(f"dec{k}_{j}", m[1])
 
     # ------------------------------------------------------------------ encoder / decoder
     def _encode(self, tag, frames, N, h_out):
         """frames: fp32 NCHW [N, nc, W, W] -> h_out fp32 [N, g]; returns the skip maps (NHWC, one per stage)."""
         K, G, model = self.K, self.G, self.model
         adt = G.cfg["adt"]
-        enc, g = model.encoder, model.g_dim
+        enc = model.encoder
         H = G.cfg["W"]
         skips, a, slot = [], None, None   # slot: the scratch buffer (0 / 1) holding `a`, None for a skip map
-        for i, j, cin, cout, m in self._enc_layers():
+        for i, j, cin, cout, m in self.enc_layers:
             if i and not j:
                 a, slot = self._pool(a, N, H, cin), 0
                 H //= 2
@@ -174,14 +147,7 @@ class VggGenerateEngine(GenerateEngine):
                 slot = None
             a = y
         p = self._pool(a, N, H, 512)
-        top = getattr(enc, f"c{len(self.ENC) + 1}")
-        sc, sh = self.bn["encf"]
-        raw = self._buf(G, f"{tag}_enc_rawf", N * g, adt)
-        y = h_out if adt == torch.float32 else self._buf(G, f"{tag}_enc_yf", N * g, adt)
-        K.gemm(p, self.wp["encf"], raw, N, g, 16 * 512, bias=top[0].bias.data)
-        K.bn_act(raw, y, sc, sh, 1, N, g, ACT_TANH)
-        if y is not h_out:
-            cast(K, y, h_out, N * g)
+        self._encode_top(tag, p, N, h_out, getattr(enc, f"c{len(self.ENC) + 1}")[0].bias)
         return skips
 
     def _pool(self, a, N, H, C):
@@ -194,7 +160,7 @@ class VggGenerateEngine(GenerateEngine):
         the c0 = cin half of its weight).  Returns per stage (tensor, nsrc) for the decodes."""
         K, G = self.K, self.G
         n, out = len(self.DEC), []
-        for k, j, cin, cout, _ in self._dec_layers():
+        for k, j, cin, cout, _ in self.dec_layers:
             if j:
                 continue
             C, H = cin // 2, 8 << k
@@ -211,20 +177,11 @@ class VggGenerateEngine(GenerateEngine):
 
     def _decode(self, h_pred, halves, frame_out, rows):
         """h_pred fp32 [rows, g] -> frame_out fp32 NCHW [rows, nc, W, W] (sigmoid applied), on the first rows rows."""
-        K, G, model = self.K, self.G, self.model
-        adt = G.cfg["adt"]
-        dec, g = model.decoder, model.g_dim
-        if adt == torch.float32:
-            hp = h_pred
-        else:
-            hp = self._buf(G, "dec_hp", rows * g, adt)
-            cast(K, h_pred, hp, rows * g)
-        raw, d = self._scratch("raw", rows * 16 * 512), self._scratch(0, rows * 16 * 512)
-        K.gemm(hp, self.wp["dec-1"], raw, rows, 16 * 512, g, b_mn=True, bias=self.wp["dec-1.bias16"])
-        sc, sh = self.bn["dec-1"]
-        K.bn_act(raw, d, sc, sh, 1, rows * 16, 512, ACT_LRELU)
+        K, dec = self.K, self.model.decoder
+        d = self._scratch(0, rows * 16 * 512)
+        self._decode_head(h_pred, rows, self._scratch("raw", rows * 16 * 512), d)
         slot, H = 0, 4
-        for k, j, cin, cout, m in self._dec_layers():
+        for k, j, cin, cout, m in self.dec_layers:
             if j == 0:
                 C = cin // 2
                 slot = 1 - slot

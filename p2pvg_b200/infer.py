@@ -103,18 +103,54 @@ def encoder_forward(mod, x):
         nchw._p2pvg_nhwc = y  # decoder_forward reuses the NHWC copy when it gets this very tensor back
         skips.append(nchw)
         a, H, cin = y, Ho, cout
-    fin = getattr(mod, f"c{n + 1}")
-    conv, bn = fin[0], fin[1]
-    g = mod.dim
-    wp = torch.empty(g * 16 * cin, device=dev, dtype=adt)
+    return _encode_top(K, getattr(mod, f"c{n + 1}"), a, B, mod.dim, adt), skips
+
+
+def _encode_top(K, top, a, B, g, adt):
+    """The encoder's top layer ``top`` = Conv2d(512, g, 4, 1, 0) + BatchNorm + Tanh on the 4x4x512 maps a [B, 4, 4, 512] (NHWC):
+    h [B, g] fp32."""
+    conv, bn = top[0], top[1]
+    dev = a.device
+    wp = torch.empty(g * 16 * 512, device=dev, dtype=adt)
     pack_conv4(K, conv.weight.data, wp)
     raw = torch.empty(B * g, device=dev, dtype=adt)
     y = torch.empty(B * g, device=dev, dtype=adt)
-    K.gemm(a, wp, raw, B, g, 16 * cin, bias=conv.bias.data)
+    K.gemm(a, wp, raw, B, g, 16 * 512, bias=conv.bias.data)
     _bn(K, bn, raw, y, 1, B, g, ACT_TANH, dev)
     h = torch.empty(B, g, device=dev)
     cast(K, y, h, B * g)
-    return h, skips
+    return h
+
+
+def _decode_head(K, upc1, vec, g, adt):
+    """The decoder's head ``upc1`` = ConvTranspose2d(g, 512, 4, 1, 0) + BatchNorm + LeakyReLU on the latents vec (any shape
+    with B * g elements): (d [B, 4, 4, 512] NHWC, B)."""
+    dev = vec.device
+    vec = vec.reshape(-1, g).float().contiguous()
+    B = int(vec.shape[0])
+    hp = torch.empty(B * g, device=dev, dtype=adt)
+    cast(K, vec, hp, B * g)
+    convt, bn = upc1[0], upc1[1]
+    wp = torch.empty(g * 16 * 512, device=dev, dtype=adt)
+    pack_convt4(K, convt.weight.data, wp)
+    b16 = torch.empty(16 * 512, device=dev)
+    tile_bias(K, convt.bias.data, b16, 16)
+    raw = torch.empty(B * 16 * 512, device=dev, dtype=adt)
+    d = torch.empty_like(raw)
+    K.gemm(hp, wp, raw, B, 16 * 512, g, b_mn=True, bias=b16)
+    _bn(K, bn, raw, d, 1, B * 16, 512, ACT_LRELU, dev)
+    return d, B
+
+
+def _frames_out(K, raw, B, W, nc):
+    """Decoder output raw [B, W, W, nc] (NHWC, activation dtype) -> Sigmoid, as fp32 NCHW frames."""
+    dev = raw.device
+    out32 = torch.empty(B * W * W * nc, device=dev)
+    cast(K, raw, out32, B * W * W * nc)
+    K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
+    out = torch.empty(B, nc, W, W, device=dev)
+    nhwc_to_nchw(K, out32, out, B, W * W, nc)
+    return out
 
 
 def _to_nhwc(K, t, adt):
@@ -132,21 +168,8 @@ def decoder_forward(mod, vec, skip):
     K = kernels_for(vec.device)
     dev, adt = vec.device, _act_dtype()
     chans = _stages(mod)
-    n, g = len(chans), mod.dim
-    vec = vec.reshape(-1, g).float().contiguous()
-    B = int(vec.shape[0])
-    hp = torch.empty(B * g, device=dev, dtype=adt)
-    cast(K, vec, hp, B * g)
-    ctop = chans[-1]
-    convt, bn = mod.upc1[0], mod.upc1[1]
-    wp = torch.empty(g * 16 * ctop, device=dev, dtype=adt)
-    pack_convt4(K, convt.weight.data, wp)
-    b16 = torch.empty(16 * ctop, device=dev)
-    tile_bias(K, convt.bias.data, b16, 16)
-    raw = torch.empty(B * 16 * ctop, device=dev, dtype=adt)
-    d = torch.empty_like(raw)
-    K.gemm(hp, wp, raw, B, 16 * ctop, g, b_mn=True, bias=b16)
-    _bn(K, bn, raw, d, 1, B * 16, ctop, ACT_LRELU, dev)
+    n = len(chans)
+    d, B = _decode_head(K, mod.upc1, vec, mod.dim, adt)
     Hi = 4
     src = torch.zeros(1, dtype=torch.int32, device=dev)
     for k in range(n):
@@ -170,13 +193,7 @@ def decoder_forward(mod, vec, skip):
             _bn(K, blk.main[1], raw, dn, 1, B * 4 * Hi * Hi, cout, ACT_LRELU, dev)
             d = dn
         Hi *= 2
-    W = Hi
-    out32 = torch.empty(B * W * W * mod.nc, device=dev)
-    cast(K, raw, out32, B * W * W * mod.nc)
-    K.act_fwd(out32, out32.numel(), ACT_SIGMOID)
-    out = torch.empty(B, mod.nc, W, W, device=dev)
-    nhwc_to_nchw(K, out32, out, B, W * W, mod.nc)
-    return out
+    return _frames_out(K, raw, B, Hi, mod.nc)
 
 
 def _lstm_cells(K, mod, inp):

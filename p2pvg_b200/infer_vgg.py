@@ -3,9 +3,9 @@
 p2pvg_b200/infer.py: NCHW fp32 in / out, BatchNorm honours ``module.training``."""
 import torch
 
-from ._lib import ACT_LRELU, ACT_SIGMOID, ACT_TANH
-from .infer import _act_dtype, _bn, _to_nhwc, kernels_for
-from .layouts import cast, implicit_shape, nchw_to_nhwc, nhwc_to_nchw, pack_conv3, pack_conv4, pack_convt4, tile_bias, up8
+from ._lib import ACT_LRELU
+from .infer import _act_dtype, _bn, _decode_head, _encode_top, _frames_out, _to_nhwc, kernels_for
+from .layouts import implicit_shape, nchw_to_nhwc, nhwc_to_nchw, pack_conv3, up8
 
 
 def _conv3(K, a, conv, c0, cin, out, N, H, adt, dev, bias=True, accumulate_from=None):
@@ -65,38 +65,15 @@ def vgg_encoder_forward(mod, x):
         skips.append(nchw)
     p = torch.empty(B * 16 * C, device=dev, dtype=adt)
     K.maxpool2_fwd(a, p, B, H, H, C)
-    top = getattr(mod, f"c{nst + 1}")
-    conv, bn = top[0], top[1]
-    g = mod.dim
-    wp = torch.empty(g * 16 * C, device=dev, dtype=adt)
-    pack_conv4(K, conv.weight.data, wp)
-    raw = torch.empty(B * g, device=dev, dtype=adt)
-    y = torch.empty(B * g, device=dev, dtype=adt)
-    K.gemm(p, wp, raw, B, g, 16 * C, bias=conv.bias.data)
-    _bn(K, bn, raw, y, 1, B, g, ACT_TANH, dev)
-    h = torch.empty(B, g, device=dev)
-    cast(K, y, h, B * g)
-    return h, skips
+    return _encode_top(K, getattr(mod, f"c{nst + 1}"), p, B, mod.dim, adt), skips
 
 
 @torch.no_grad()
 def vgg_decoder_forward(mod, vec, skip):
     K = kernels_for(vec.device)
     dev, adt = vec.device, _act_dtype()
-    g, nc = mod.dim, mod.nc
-    vec = vec.reshape(-1, g).float().contiguous()
-    B = int(vec.shape[0])
-    hp = torch.empty(B * g, device=dev, dtype=adt)
-    cast(K, vec, hp, B * g)
-    convt, bn = mod.upc1[0], mod.upc1[1]
-    wp = torch.empty(g * 16 * 512, device=dev, dtype=adt)
-    pack_convt4(K, convt.weight.data, wp)
-    b16 = torch.empty(16 * 512, device=dev)
-    tile_bias(K, convt.bias.data, b16, 16)
-    raw = torch.empty(B * 16 * 512, device=dev, dtype=adt)
-    d = torch.empty_like(raw)
-    K.gemm(hp, wp, raw, B, 16 * 512, g, b_mn=True, bias=b16)
-    _bn(K, bn, raw, d, 1, B * 16, 512, ACT_LRELU, dev)
+    nc = mod.nc
+    d, B = _decode_head(K, mod.upc1, vec, mod.dim, adt)
     H, C = 4, 512
     nst, W0 = mod.nstage, mod.image_width
     for k in range(nst):
@@ -118,9 +95,4 @@ def vgg_decoder_forward(mod, vec, skip):
     K.gemm(d, wl, colT, M, ldl, 64, b_mn=True)
     raw = torch.empty(M * nc, device=dev, dtype=adt)
     K.col2im3(colT, raw, B, W0, W0, nc, ldl, bias=convt.bias.data)
-    out32 = torch.empty(M * nc, device=dev)
-    cast(K, raw, out32, M * nc)
-    K.act_fwd(out32, M * nc, ACT_SIGMOID)
-    out = torch.empty(B, nc, W0, W0, device=dev)
-    nhwc_to_nchw(K, out32, out, B, W0 * W0, nc)
-    return out
+    return _frames_out(K, raw, B, W0, nc)

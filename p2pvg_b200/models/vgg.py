@@ -9,7 +9,7 @@ BatchNorm buffers: arithmetic runs in the sm_90a kernels (engine_vgg.py for trai
 """
 import torch.nn as nn
 
-from ..engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128
+from ..engine_vgg import vgg_tables
 
 
 class vgg_layer(nn.Module):
@@ -29,7 +29,7 @@ class VggEncoder(nn.Module):
     def __init__(self, dim, nc=1):
         super().__init__()
         self.dim, self.nc = dim, nc
-        table = VGG_ENC_128 if self.image_width == 128 else VGG_ENC
+        table = vgg_tables(self.image_width)[0]
         self.nstage = len(table)
         for i, pairs in enumerate(table, 1):
             setattr(self, f"c{i}", _stage(pairs, nc))
@@ -48,7 +48,7 @@ class VggDecoder(nn.Module):
     def __init__(self, dim, nc=1):
         super().__init__()
         self.dim, self.nc = dim, nc
-        table = VGG_DEC_128 if self.image_width == 128 else VGG_DEC
+        table = vgg_tables(self.image_width)[1]
         self.nstage = len(table)
         self.upc1 = nn.Sequential(nn.ConvTranspose2d(dim, 512, 4, 1, 0), nn.BatchNorm2d(512), nn.LeakyReLU(0.2, inplace=True))
         for i, pairs in enumerate(table[:-1], 2):
