@@ -567,8 +567,10 @@ class GenerateEngine:
         return sum(t.numel() * t.element_size() for G in self._graphs.values() for t in G.bufs.values())
 
     def clear(self):
-        """Drop every cached graph and its buffers."""
+        """Drop every cached graph and its buffers.  The body keeps the graph it last ran in self.G (and its backend in
+        self.K) for the layer helpers; those references go too, or the last graph's buffers would outlive the call."""
         self._graphs.clear()
+        self.K = self.G = None
 
     # ------------------------------------------------------------------ buffers
     def _alloc_io(self, G):
