@@ -13,6 +13,11 @@ when it changes.  Each entry is a dict with `op`:
     weight gradient).
 `key(L)` is what a recording of the step is compared on.
 
+precision "fp32" derives the launches of the fp32 step instead (TrainEngine.implicit, bd, fuse_stats, fuse_last, bn_skip_sums,
+bn_wgrad_c1 off): im2col / col2im, the gemm_simt GEMMs with their pitches, the unfused BatchNorm passes, the group_sum of the
+decoder's dcol, add_indexed, colsum and sigmoid_mse, as launch_audit.gemm32 / op32 entries whose `key` is what
+launch_audit.fp32_call_key logs for the call (tests/test_dcgan_fp32_launches_gpu.py, tests/test_fp32_launch_lists_cpu.py).
+
 The float64 checkers work in image chunks (ref64.CHUNK elements) so that references of C2-sized tensors stay a few GiB.
 """
 import types
@@ -22,7 +27,9 @@ import torch.nn.functional as F
 
 from p2pvg_b200.engine import BN_FUSE_MIN, TrainEngine
 from p2pvg_b200.layouts import implicit_shape
-from tests.ref64 import A_STAT, CHUNK
+from tests.launch_audit import gemm32, op32
+from tests.lstm_schedule import gamma
+from tests.ref64 import A_STAT, CHUNK, bound_check
 from tests.tc_schedule import BETA, alpha_for, assert_within, box_for, cdiv, conv_ref64, rows_by_tile
 from tests.vgg_ref import row_cooperative
 
@@ -69,7 +76,9 @@ def _bn(op, name, G, R=None, C=None, act=None, F=None, dout=False):
 
 
 def key(L):
-    """What a recorded call is compared on."""
+    """What a recorded call is compared on (an fp32 entry: launch_audit.fp32_call_key of the call)."""
+    if "key" in L:
+        return L["key"]
     if L["op"] == "conv_gemm":
         return ("conv_gemm", L["kind"], L["N"], L["H"], L["Ck"], L["Cn"], L["Cm"], L["bias"], L["addend"], L["ipg"],
                 L["stat"] is not None)
@@ -94,8 +103,11 @@ def _stack(nc, W0):
     return ch, n, (16 * nc) % 64 != 0
 
 
-def forward_launches(T, B, S, nskip, nc, W0):
-    """encode (engine.py:761-800) then decode (engine.py:944-1004), in engine order."""
+def forward_launches(T, B, S, nskip, nc, W0, precision="bf16"):
+    """encode (engine.py:761-800) then decode (engine.py:944-1004), in engine order.  precision "fp32": the fp32 step's
+    launches (_forward32), entries with op32 / gemm32 keys."""
+    if precision == "fp32":
+        return _forward32(T, B, S, nskip, nc, W0)
     ch, n, bd = _stack(nc, W0)
     out = []
     N = T * B
@@ -197,9 +209,11 @@ def _decoder_backward(out, g0, g1, B, nskip, nc, W0, want_wgrad, want_skip, tag)
     out.append(_gemm(f"{tag}dec-1 dgrad", N, G_DIM, 16 * ctop))
 
 
-def backward_launches(T, B, S, nskip, nc, W0, has_cpc=True):
+def backward_launches(T, B, S, nskip, nc, W0, has_cpc=True, precision="bf16"):
     """backward_decoder (engine.py:1236), the CPC chain of backward_prior (:1355) and encoder_backward (:1286-1344), in the
-    order the step enqueues them (engine.py:679-696, mode A)."""
+    order the step enqueues them (engine.py:679-696, mode A).  precision "fp32": _backward32."""
+    if precision == "fp32":
+        return _backward32(T, B, S, nskip, nc, W0, has_cpc)
     ch, n, bd = _stack(nc, W0)
     out = []
     _decoder_backward(out, 0, S, B, nskip, nc, W0, True, True, "")
@@ -234,8 +248,177 @@ def backward_launches(T, B, S, nskip, nc, W0, has_cpc=True):
     return out
 
 
-def step_launches(T, B, S, nskip, nc, W0, has_cpc=True):
-    return forward_launches(T, B, S, nskip, nc, W0) + backward_launches(T, B, S, nskip, nc, W0, has_cpc)
+def step_launches(T, B, S, nskip, nc, W0, has_cpc=True, precision="bf16"):
+    return forward_launches(T, B, S, nskip, nc, W0, precision) + backward_launches(T, B, S, nskip, nc, W0, has_cpc, precision)
+
+
+# ------------------------------------------------------------------ the fp32 step's launches
+
+def _bn_forward32(out, name, G, R, C, act):
+    """TrainEngine.bn_forward (engine.py:838-840) without fused statistics."""
+    out += [op32("bn_fwd_stats", name, G, R, C), op32("bn_act", name, G, R, C, act)]
+
+
+def _forward32(T, B, S, nskip, nc, W0):
+    """encode (engine.py:750-784) and decode (:941-1011) with TrainEngine.implicit, bd and fuse_last off (act_dtype fp32,
+    engine.py:207-215): every 4x4 convolution is im2col -> gemm_simt, every transposed one gemm_simt -> col2im."""
+    ch, n = chans(W0), len(chans(W0))
+    out = []
+    N, H = T * B, W0
+    for l in range(n):
+        cin, cout = (nc if l == 0 else ch[l - 1]), ch[l]
+        Ho = H // 2
+        out.append(op32("im2col", f"enc{l}", N, H, cin))                                       # :774
+        out.append(gemm32(f"enc{l}", N * Ho * Ho, cout, 16 * cin, bias=True))                   # :778
+        _bn_forward32(out, f"enc{l}", T, B * Ho * Ho, cout, ACT_LRELU)                          # :779
+        H = Ho
+    out.append(gemm32("enc_top", N, G_DIM, 16 * ch[-1], bias=True))                             # encode_top :793
+    _bn_forward32(out, "enc_top", T, B, G_DIM, ACT_TANH)
+    G = S + 1
+    N = G * B
+    out.append(gemm32("dec-1", N, 16 * ch[-1], G_DIM, b_mn=True, bias=True))                    # decode_head :1008
+    _bn_forward32(out, "dec-1", G, B * 16, ch[-1], ACT_LRELU)
+    Hi = 4
+    for k in range(n):
+        cd, cout = ch[n - 1 - k], (ch[n - 2 - k] if k < n - 1 else nc)
+        out.append(gemm32(f"dec{k}.D", N * Hi * Hi, 16 * cout, cd, b_mn=True))                  # :977
+        out.append(gemm32(f"dec{k}.S", nskip * B * Hi * Hi, 16 * cout, cd, b_mn=True))          # :978
+        out.append(op32("col2im", f"dec{k}", N, Hi, cout, True, True, B))                       # :983
+        if k < n - 1:
+            _bn_forward32(out, f"dec{k}", G, B * 4 * Hi * Hi, cout, ACT_LRELU)                 # :987
+        Hi *= 2
+    out.append(op32("sigmoid_mse", "loss", G, B * nc * W0 * W0))                                # losses_fwd :1026
+    return out
+
+
+def _decoder_backward32(out, Gn, B, nskip, nc, W0, want_wgrad, want_skip, tag):
+    """TrainEngine.decoder_backward (engine.py:1032-1128) on the explicit path (implicit, bn_skip_sums off), then
+    decode_head_backward (:1130-1154)."""
+    ch, n = chans(W0), len(chans(W0))
+    N = Gn * B
+    Hi = 4 << (n - 1)
+    for k in range(n - 1, -1, -1):
+        cd, cout = ch[n - 1 - k], (ch[n - 2 - k] if k < n - 1 else nc)
+        Md, Ms, Ho = N * Hi * Hi, nskip * B * Hi * Hi, 2 * Hi
+        nm = f"{tag}dec{k}"
+        if k < n - 1:
+            out.append(op32("bn_bwd", nm, Gn, B * Ho * Ho, cout, ACT_LRELU))                   # :1073
+            if want_wgrad:
+                out.append(op32("bn_param_grad", nm, Gn, cout))                                 # :1075
+        elif want_wgrad:
+            out.append(op32("colsum", f"{nm} bias grad", N * Ho * Ho, cout, cout))              # :1078
+        out.append(op32("im2col", f"{nm} dcol", N, Ho, cout))                                   # :1104
+        out.append(gemm32(f"{nm} dgrad D", Md, cd, 16 * cout))                                  # :1109
+        if want_wgrad:
+            out.append(gemm32(f"{nm} wgrad D", cd, 16 * cout, Md, a_mn=True, b_mn=True))        # :1111
+        if want_skip:
+            out.append(op32("group_sum", f"{nm} dcol skip sum", Gn, nskip, B * Hi * Hi * 16 * cout))   # :1114
+            out.append(gemm32(f"{nm} dgrad S", Ms, cd, 16 * cout))                              # :1119
+            if want_wgrad:
+                out.append(gemm32(f"{nm} wgrad S", cd, 16 * cout, Ms, a_mn=True, b_mn=True))    # :1122
+        Hi //= 2
+    ctop = ch[-1]
+    out.append(op32("bn_bwd", f"{tag}dec-1", Gn, B * 16, ctop, ACT_LRELU))                      # :1140
+    if want_wgrad:
+        out.append(op32("bn_param_grad", f"{tag}dec-1", Gn, ctop))                              # :1143
+        out.append(gemm32(f"{tag}dec-1 wgrad", G_DIM, 16 * ctop, N, a_mn=True, b_mn=True))      # :1146
+    out.append(gemm32(f"{tag}dec-1 dgrad", N, G_DIM, 16 * ctop))                                # :1150
+
+
+def encode_top_backward32(out, T, B, ctop=512):
+    """TrainEngine.encode_top_backward (engine.py:1337-1355), fp32: dy is dH itself."""
+    N = T * B
+    out.append(op32("bn_bwd", "enc_top", T, B, G_DIM, ACT_TANH))
+    out.append(op32("bn_param_grad", "enc_top", T, G_DIM))
+    out.append(gemm32("enc_top wgrad", G_DIM, 16 * ctop, N, a_mn=True, b_mn=True))
+    out.append(gemm32("enc_top dgrad", N, 16 * ctop, G_DIM, b_mn=True))
+
+
+def _backward32(T, B, S, nskip, nc, W0, has_cpc):
+    """backward_decoder's decoder_backward(0, S) (engine.py:1242), backward_prior's CPC decoder_backward(S, S + 1) (:1366) and
+    encoder_backward (:1292-1335) with bn_wgrad_c1 off, in the order the serial fp32 step enqueues them (:684-688)."""
+    ch, n = chans(W0), len(chans(W0))
+    out = []
+    _decoder_backward32(out, S, B, nskip, nc, W0, True, True, "")
+    if has_cpc:
+        _decoder_backward32(out, 1, B, nskip, nc, W0, False, False, "cpc ")
+    encode_top_backward32(out, T, B, ch[-1])
+    N = T * B
+    H = W0 >> (n - 1)
+    for l in range(n - 1, -1, -1):
+        cin, cout = (nc if l == 0 else ch[l - 1]), ch[l]
+        Ho = H // 2
+        M = N * Ho * Ho
+        out.append(op32("add_indexed", f"enc{l} skip grad", nskip, B * Ho * Ho * cout))         # :1307
+        out.append(op32("bn_bwd", f"enc{l}", T, B * Ho * Ho, cout, ACT_LRELU))                  # :1318
+        out.append(op32("bn_param_grad", f"enc{l}", T, cout))                                   # :1319
+        out.append(gemm32(f"enc{l} wgrad", cout, 16 * cin, M, a_mn=True, b_mn=True))           # :1325
+        if l > 0:
+            out.append(gemm32(f"enc{l} dgrad", M, 16 * cin, cout, b_mn=True))                   # :1333
+            out.append(op32("col2im", f"enc{l} dx", N, Ho, cin, False, False, 0))               # :1334
+        H *= 2
+    return out
+
+
+# ------------------------------------------------------------------ the explicit lowering (conv_lower.cu)
+
+def im2col_ref(x, N, H, C):
+    """col[(n, oy, ox), (kh, kw, c)] = x[n, 2 oy - 1 + kh, 2 ox - 1 + kw, c], zero outside the map (conv_lower.cu:32)."""
+    Ho = H // 2
+    xp = F.pad(x.reshape(N, H, H, C), (0, 0, 1, 1, 1, 1))
+    taps = [xp[:, kh:kh + 2 * Ho:2, kw:kw + 2 * Ho:2] for kh in range(4) for kw in range(4)]
+    return torch.stack(taps, 3).reshape(N * Ho * Ho, 16 * C)
+
+
+def check_im2col(x, col, N, H, C, name=""):
+    """im2col bit-exact against the gather reference, image chunk by image chunk."""
+    Ho = H // 2
+    rows = Ho * Ho
+    x = x.reshape(-1)[:N * H * H * C].view(N, H * H * C)
+    col = col.reshape(-1)[:N * rows * 16 * C].view(N, rows * 16 * C)
+    per = max(1, CHUNK // (rows * 16 * C))
+    for n0 in range(0, N, per):
+        n = min(per, N - n0)
+        assert torch.equal(col[n0:n0 + n].reshape(n * rows, 16 * C), im2col_ref(x[n0:n0 + n], n, H, C)), \
+            f"{name}: im2col N={N} {H}x{H}x{C} differs from the gather in images [{n0}, {n0 + n})"
+
+
+def check_col2im(y, col, N, Hi, C, bias=None, col2=None, grp_src=None, ipg=0, name=""):
+    """col2im (conv_lower.cu:107-177): y[n, oy, ox] = bias + the (up to) four taps (kh, kw) with oy = 2 iy - 1 + kh,
+    ox = 2 ix - 1 + kw of col[n, iy, ix] and, with col2, of col2 at image grp_src[n // ipg] * ipg + n % ipg; an fp32 chain
+    from the bias, one rounding per tap add (at most 8), stored as it is.  Against float64, image chunk by image chunk.
+    Returns the worst ratio."""
+    from tests.launch_audit import addend_index
+    Ho = 2 * Hi
+    cv = col.reshape(-1)[:N * Hi * Hi * 16 * C].view(N, Hi, Hi, 4, 4, C)
+    yv = y.reshape(-1)[:N * Ho * Ho * C].view(N, Ho, Ho, C)
+    idx = None
+    if col2 is not None:
+        idx = addend_index(grp_src.tolist()[:cdiv(N, ipg)], ipg, N, col.device)
+        c2v = col2.reshape(-1)[:(int(idx.max()) + 1) * Hi * Hi * 16 * C].view(-1, Hi, Hi, 4, 4, C)
+    per = max(1, CHUNK // (Hi * Hi * 16 * C))
+    worst = 0.0
+    for n0 in range(0, N, per):
+        n1 = min(N, n0 + per)
+        c = cv[n0:n1].double()
+        m = c.abs()
+        if idx is not None:
+            c2 = c2v[idx[n0:n1]].double()
+            c, m = c + c2, m + c2.abs()
+            del c2
+        ref = torch.zeros(n1 - n0, Ho + 2, Ho + 2, C, dtype=torch.float64, device=col.device)
+        mag = torch.zeros_like(ref)
+        for kh in range(4):
+            for kw in range(4):
+                ref[:, kh:kh + Ho:2, kw:kw + Ho:2] += c[:, :, :, kh, kw]
+                mag[:, kh:kh + Ho:2, kw:kw + Ho:2] += m[:, :, :, kh, kw]
+        ref, mag = ref[:, 1:-1, 1:-1], mag[:, 1:-1, 1:-1]
+        if bias is not None:
+            ref = ref + bias.double()
+            mag = mag + bias.double().abs()
+        worst = max(worst, bound_check(yv[n0:n1], ref, gamma(8) * mag, f"{name}: col2im images [{n0}, {n1})"))
+        del c, m, ref, mag
+    return worst
 
 
 # ------------------------------------------------------------------ kinds 0 / 2: per-(image, channel) sums

@@ -15,9 +15,9 @@ import contextlib
 import torch
 
 from tests.dcgan_ref import check_conv4_sums, conv4_ref64_elem
+from tests.launch_audit import kernel_for, simt_alpha
 from tests.loss_ref import ACT_LRELU, ACT_TANH, TINY, act_fwd_ref
 from tests.lstm_schedule import U, gamma
-from tests.mlp_ref import kernel_for, simt_alpha
 from tests.ref64 import bound_check
 from tests.tc_schedule import BETA, alpha_for, assert_within, cdiv, gemm_tc_tiles
 from tests.vgg_ref import VggAudit, check_conv3_sums, conv3_ref64_elem

@@ -31,10 +31,10 @@ from p2pvg_b200.engine import StepPlan, TrainEngine
 from tests.dcgan_ref import (ACT_LRELU, ACT_TANH, check_conv4_sums, check_stat_rows, check_wgrad_c1, conv4_ref64_elem, conv_variant,
                              forward_launches, key, step_launches, wgrad4_ref64, wgrad_c1_ref64)
 from tests.launch_audit import K, memory_per_test, sms  # noqa: F401  (fixtures)
-from tests.launch_audit import (ALPHA_BN, BENCH_OPT, NAN, SKIP_OPT, AuditKernels, RecordingKernels, addend_index, audit_step,
-                                bn_inputs, bn_stats, randn, slices_with_boundary)
-from tests.ref64 import (EPS, assert_exact, binary01, bn_group_ref64, bound_check, check_finalize_vs_output, finalize_ref,
-                         gemm_ref64)
+from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, RecordingKernels, addend_index, audit_step, bn_inputs,
+                                bn_stats, randn, slices_with_boundary)
+from tests.launch_audit import bn_bwd_refs as _refs, check_bn_bwd as _check_bwd, check_bn_stats as _check_stats
+from tests.ref64 import EPS, assert_exact, binary01, bound_check, check_finalize_vs_output, gemm_ref64
 from tests.tc_schedule import BETA, assert_within, cdiv, conv_tiles, gemm_tc_tiles, sm_count
 
 pytestmark = pytest.mark.gpu
@@ -320,19 +320,6 @@ def test_weight_gradient_gemm(K, sms, cfg, L):
 
 # ------------------------------------------------------------------ D. BatchNorm at the launch shapes
 
-def _check_stats(st, raw, G, R, C, gamma, beta, name):
-    """bn_fwd_stats against float64 group by group (finalize_ref's bounds with sums known within ALPHA_BN)."""
-    x = raw.view(G, R, C)
-    s1 = torch.stack([x[g].double().sum(0) for g in range(G)])
-    s2 = torch.stack([(x[g].double() ** 2).sum(0) for g in range(G)])
-    m1 = torch.stack([x[g].double().abs().sum(0) for g in range(G)])
-    w = 0.0
-    for got, (ref, bnd), nm in zip((st["mean"], st["invstd"], st["varu"], st["scale"], st["shift"]),
-                                   finalize_ref(s1, s2, m1, R, gamma, beta, EPS, ALPHA_BN), ("mean", "invstd", "varu", "scale", "shift")):
-        w = max(w, bound_check(got.view(G, C), ref, bnd, f"{name} {nm}"))
-    return w
-
-
 def _unfused_fwd_shapes():
     out = []
     for n in CONFIGS:
@@ -382,37 +369,6 @@ def _bwd_shapes():
 
 
 BWD = _bwd_shapes()
-
-
-def _side(raw, st, G, R, C):
-    return raw.view(G, R, C).double() * st["scale"].view(G, 1, C).double() + st["shift"].view(G, 1, C).double() > 0
-
-
-def _check_bwd(res, refs, G, C, name):
-    """dx (bf16), sum dz, sum dz*xhat per group, and dgamma / dbeta, against the per-group float64 references."""
-    w = 0.0
-    for g, r in enumerate(refs):
-        w = max(w, assert_within(res["dx"][g], r["dx"], r["dx_mag"], 0, torch.bfloat16, alpha=ALPHA_BN, quiet=True, name=f"{name} dx group {g}"))
-        w = max(w, assert_within(res["sdz"].view(G, C)[g], r["sdz"], r["sdz_mag"], 0, torch.float32, alpha=ALPHA_BN, quiet=True,
-                                 name=f"{name} sum_dz group {g}"))
-        w = max(w, assert_within(res["sdzx"].view(G, C)[g], r["sdzx"], r["sdzx_mag"], 0, torch.float32, alpha=ALPHA_BN, quiet=True,
-                                 name=f"{name} sum_dzx group {g}"))
-    if "dgamma" in res:
-        dg, db = sum(r["sdzx"] for r in refs), sum(r["sdz"] for r in refs)
-        w = max(w, assert_within(res["dgamma"], dg, sum(r["sdzx_mag"] for r in refs), 0, torch.float32, alpha=ALPHA_BN, name=f"{name} dgamma"))
-        w = max(w, assert_within(res["dbeta"], db, sum(r["sdz_mag"] for r in refs), 0, torch.float32, alpha=ALPHA_BN, name=f"{name} dbeta"))
-    return w
-
-
-def _refs(raw, dy, st, gamma, beta, G, R, C, act, y=None):
-    x, d = raw.view(G, R, C), dy.view(G, R, C)
-    side = _side(raw, st, G, R, C) if act == ACT_LRELU else None
-    refs = []
-    for g in range(G):
-        r = bn_group_ref64(x[g], d[g], gamma, beta, act, side=side[g] if side is not None else None,
-                           y=y.view(G, R, C)[g] if y is not None else None)
-        refs.append({k: r[k] for k in ("dx", "dx_mag", "sdz", "sdz_mag", "sdzx", "sdzx_mag")})
-    return refs
 
 
 @pytest.mark.parametrize("case", BWD, ids=[f"{c[0]}-{c[5]}-G{c[1]}_R{c[2]}_C{c[3]}" for c in BWD])

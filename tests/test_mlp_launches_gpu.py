@@ -31,13 +31,13 @@ from p2pvg_b200._lib import CudaKernels, KernelError
 from p2pvg_b200.engine import StepPlan
 from p2pvg_b200.engine_mlp import TrainEngineMLP
 from tests.launch_audit import K, memory_per_test  # noqa: F401  (fixtures)
-from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, RecordingKernels, assert_concurrent, assert_equal_steps,
-                                audit_step, release, run_step, skip_seed, step_inputs)
+from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, TF32_FLAG, TF32_REQUIRE, AuditKernels, RecordingKernels, assert_concurrent,
+                                assert_equal_steps, audit_step, entry_kernel, gemm_alpha, kernel_for, release, run_step, simt_alpha,
+                                skip_seed, step_inputs, watch_backbone)
 from tests.loss_ref import (ACT_RELU, ACT_TANH, TINY, act_bwd_ref, act_fwd_ref, build_concat_ref, check_gather_add_cols,
                             check_layernorm_bwd, check_layernorm_fwd)
 from tests.lstm_schedule import U
-from tests.mlp_ref import (POSE, TF32_FLAG, TF32_REQUIRE, backbone_launches, entry_kernel, gemm_alpha, gemm_variant, kernel_for,
-                           key, simt_alpha)
+from tests.mlp_ref import POSE, backbone_launches, gemm_variant, key
 from tests.ref64 import assert_exact, bound_check, gemm_ref64
 from tests.tc_schedule import alpha_for, assert_within, gemm_tc_tiles
 
@@ -48,25 +48,8 @@ CFG = dict(g_dim=128, z_dim=10, rnn_size=512, backbone="mlp", predictor_rnn_laye
 H = 128                      # h_dim = g_dim (engine_mlp.py:130)
 LD = 2 * H + 2               # pitch of the skip matrix (engine_mlp.py:167)
 SENTINEL = -777.0
-BACKBONE = ("encode", "decode", "losses_fwd", "decoder_backward", "encoder_backward")
-
-
 def _np_seed(T, optkw):
     return skip_seed(T) if optkw.get("skip_prob") else 0
-
-
-def _watch(eng):
-    """Sets eng.K.on while the engine runs a backbone method (everything outside the recurrent phase)."""
-    for nm in BACKBONE:
-        f = getattr(eng, nm)
-
-        def w(*a, _f=f, **kw):
-            eng.K.on = True
-            try:
-                return _f(*a, **kw)
-            finally:
-                eng.K.on = False
-        setattr(eng, nm, w)
 
 
 # ------------------------------------------------------------------ A. the launch lists
@@ -153,7 +136,7 @@ def _recorded_step(T, B, optkw, adt, rerun=False):
     rec = MlpRecording("cuda", rerun=rerun)
 
     def prepare(eng, x):   # eng.K is the engine's view of rec (CudaKernels.with_mode): same logs, its own flags
-        _watch(eng)
+        watch_backbone(eng)
         eng.K.loc = _Locator(eng, x)
     plan, (losses, _, _) = run_step(TrainEngineMLP, CFG, optkw, rec, T, B, _np_seed(T, optkw), act_dtype=adt, prepare=prepare)
     assert np.all(np.isfinite(losses))
@@ -555,7 +538,7 @@ def test_audit_mlp_step(case):
 
     def watched(eng, x):
         eng.K.eng = eng
-        _watch(eng)
+        watch_backbone(eng)
     audit_step(TrainEngineMLP, CFG, optkw, C5["T"], B, audit, expect, name, prepare=watched)
     rec = {v for v in audit.seen if v[0] == "gemm-recurrent"}
     assert ("gemm-recurrent", torch.float32, "tf32") in rec and ("gemm-recurrent", torch.bfloat16, "tc") in rec, rec

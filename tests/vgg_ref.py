@@ -6,6 +6,9 @@ checks and the audited step both files run.
 VGG_DEC_128 for 128x128) the way TrainEngineVGG.encode / decode / decoder_backward / encoder_backward do and ask the engine's
 own rules (implicit_shape, TrainEngine.stat_buf with BN_FUSE_MIN) which launches take the implicit GEMM,
 which get fused BatchNorm statistics and which carry the skip addend, so the list follows the engine when it changes.
+precision "fp32" derives every launch of the fp32 step's backbone methods that launch_audit.FP32_OPS names instead: im2col3
+(both tap signs), the gemm_simt GEMMs with their pitches, gather_add of the fp32 skip half, col2im3, group_sum, add_indexed,
+the unfused BatchNorm passes, colsum and sigmoid_mse (tests/test_vgg_fp32_launches_gpu.py, test_fp32_launch_lists_cpu.py).
 
 The checkers work in image chunks so that float64 references of C3-sized tensors (up to 10^9 elements) stay a few GiB:
   * conv3_sums64: per-(image, channel) sums of a kind-3 / kind-5 output from per-tap window sums of the input, O(N H W Ck);
@@ -21,8 +24,8 @@ import torch.nn.functional as F
 
 from p2pvg_b200.engine import TrainEngine
 from p2pvg_b200.engine_vgg import VGG_DEC, VGG_DEC_128, VGG_ENC, VGG_ENC_128, TrainEngineVGG
-from p2pvg_b200.layouts import implicit_shape
-from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, addend_index, audit_step, randn, release,
+from p2pvg_b200.layouts import implicit_shape, up8
+from tests.launch_audit import (BENCH_OPT, NAN, SKIP_OPT, AuditKernels, addend_index, audit_step, gemm32, op32, randn, release,
                                 slices_with_boundary)
 from tests.ref64 import (A_STAT, CHUNK, assert_exact, binary01, bound_check, check_finalize_vs_output, finalize_ref,
                          gemm_ref64)
@@ -44,8 +47,11 @@ def vgg_tables(W0):
     return (VGG_ENC_128, VGG_DEC_128) if W0 == 128 else (VGG_ENC, VGG_DEC)
 
 
-def forward_launches(T, B, S, nskip, W0=64):
-    """Every implicit-GEMM forward convolution of one bf16 vgg step (encode, then decode), in engine order."""
+def forward_launches(T, B, S, nskip, W0=64, precision="bf16", nc=3):
+    """Every implicit-GEMM forward convolution of one bf16 vgg step (encode, then decode), in engine order.  precision "fp32":
+    every launch of the fp32 step's encode and decode that launch_audit.FP32_OPS names (_forward32), with op32 / gemm32 keys."""
+    if precision == "fp32":
+        return _forward32(T, B, S, nskip, W0, nc)
     ENC, DEC = vgg_tables(W0)
     out = []
     N, H, C = T * B, W0, None
@@ -107,12 +113,14 @@ def _decoder_backward(out, DEC, N, B, nskip, want_wgrad, want_skip, tag):
                     out.append(_wgrad(f"{tag}dec{k}.{j}", N, H, cout, cin))
 
 
-def backward_launches(T, B, S, nskip, W0=64, has_cpc=True):
+def backward_launches(T, B, S, nskip, W0=64, has_cpc=True, precision="bf16", nc=3):
     """The data-gradient (kind 5) and weight-gradient (kind 4) launches of one bf16 vgg step, in the order the step enqueues
     them (engine.py TrainEngine.phases, mode A): backward_decoder's decoder_backward(0, S) with weight and skip gradients over
     the S B reconstruction images (engine.py:1236), the CPC decode's decoder_backward(S, S + 1) with data gradients only over
     B images (backward_prior, :1355), then encoder_backward over all T B frames, where the first layer (3 input channels) has
-    an explicit weight gradient and no data gradient."""
+    an explicit weight gradient and no data gradient.  precision "fp32": _backward32."""
+    if precision == "fp32":
+        return _backward32(T, B, S, nskip, W0, nc, has_cpc)
     ENC, DEC = vgg_tables(W0)
     out = []
     _decoder_backward(out, DEC, S * B, B, nskip, True, True, "")
@@ -129,6 +137,129 @@ def backward_launches(T, B, S, nskip, W0=64, has_cpc=True):
                 out.append(_wgrad(f"enc{i}.{j}", N, H, cout, cin))
             if implicit_shape(cout, cin):
                 out.append(_dgrad(f"enc{i}.{j}", N, H, cout, cin, B))
+    return out
+
+
+# ------------------------------------------------------------------ the fp32 step's launches
+
+def _conv3_fwd32(out, name, N, H, cin, cout, bias=True, add_groups=0):
+    """TrainEngineVGG.conv3_fwd on the explicit path (engine_vgg.py:104-109): im2col3 into rows of pitch up8(9 cin), gemm_simt,
+    and the fp32 skip addend gathered into the output (add_groups groups of N / add_groups images)."""
+    ld = up8(9 * cin)
+    out.append(op32("im2col3", name, N, H, cin, ld, 1))
+    out.append(gemm32(name, N * H * H, cout, ld, bias=bias))
+    if add_groups:
+        out.append(op32("gather_add", f"{name} skip addend", add_groups, N // add_groups * H * H * cout))
+
+
+def _conv3_dgrad32(out, name, N, H, cout, cin):
+    """conv3_dgrad (engine_vgg.py:116-118): im2col3 of dy with the taps mirrored (sgn -1), pitch 9 cout."""
+    out.append(op32("im2col3", f"{name} dgrad", N, H, cout, 9 * cout, -1))
+    out.append(gemm32(f"{name} dgrad", N * H * H, cin, 9 * cout))
+
+
+def _conv3_wgrad32(out, name, N, H, cout, cin):
+    """conv3_wgrad (engine_vgg.py:126-129): im2col3 of the layer input, dy^T col over every pixel."""
+    ld = up8(9 * cin)
+    out.append(op32("im2col3", f"{name} wgrad", N, H, cin, ld, 1))
+    out.append(gemm32(f"{name} wgrad", cout, ld, N * H * H, a_mn=True, b_mn=True, lda=cout, ldb=ld))
+
+
+def _forward32(T, B, S, nskip, W0, nc):
+    """TrainEngineVGG.encode (engine_vgg.py:132-156) and decode (:159-204) with TrainEngine.implicit off (act_dtype fp32)."""
+    ENC, DEC = vgg_tables(W0)
+    out = []
+    N, H = T * B, W0
+    for i, stage in enumerate(ENC):
+        for j, (cin, cout) in enumerate(stage):
+            if j == 0 and i > 0:
+                H //= 2
+            _conv3_fwd32(out, f"enc{i}.{j}", N, H, nc if cin is None else cin, cout)                    # :148
+            out += [op32("bn_fwd_stats", f"enc{i}.{j}", T, B * H * H, cout), op32("bn_act", f"enc{i}.{j}", T, B * H * H, cout, 1)]
+    out.append(gemm32("enc_top", N, 128, 16 * 512, bias=True))                                        # encode_top (engine.py:793)
+    out += [op32("bn_fwd_stats", "enc_top", T, B, 128), op32("bn_act", "enc_top", T, B, 128, 2)]
+    G = S + 1
+    N, H = G * B, 4
+    out.append(gemm32("dec-1", N, 16 * 512, 128, b_mn=True, bias=True))                              # decode_head (engine.py:1008)
+    out += [op32("bn_fwd_stats", "dec-1", G, B * 16, 512), op32("bn_act", "dec-1", G, B * 16, 512, 1)]
+    for k, stage in enumerate(DEC):
+        for j, (cin, cout) in enumerate(stage):
+            if j == 0:
+                H *= 2
+                C = cin // 2
+                _conv3_fwd32(out, f"dec{k}.0.S", nskip * B, H, C, cout)                                 # :183
+                _conv3_fwd32(out, f"dec{k}.0.D", N, H, C, cout, bias=False, add_groups=G)             # :185
+            else:
+                _conv3_fwd32(out, f"dec{k}.{j}", N, H, cin, cout)                                       # :189
+            out += [op32("bn_fwd_stats", f"dec{k}.{j}", G, B * H * H, cout), op32("bn_act", f"dec{k}.{j}", G, B * H * H, cout, 1)]
+    ldl = up8(9 * nc)
+    out.append(gemm32("dec_last", N * W0 * W0, ldl, 64, b_mn=True))                                    # :198
+    out.append(op32("col2im3", "dec_last", N, W0, nc, ldl, True))                                      # :200
+    out.append(op32("sigmoid_mse", "loss", G, B * nc * W0 * W0))                                       # losses_fwd (engine.py:1026)
+    return out
+
+
+def _decoder_backward32(out, DEC, Gn, B, nskip, W0, nc, want_wgrad, want_skip, tag):
+    """TrainEngineVGG.decoder_backward (engine_vgg.py:207-272) on the explicit path, then decode_head_backward (engine.py:1130)."""
+    N = Gn * B
+    ldl = up8(9 * nc)
+    M = N * W0 * W0
+    out.append(op32("im2col3", f"{tag}dec_last dcol", N, W0, nc, ldl, 1))                              # :220
+    out.append(gemm32(f"{tag}dec_last dgrad", M, 64, ldl))                                              # :223
+    if want_wgrad:
+        out.append(op32("colsum", f"{tag}dec_last bias grad", M, nc, nc))                              # :225
+        out.append(gemm32(f"{tag}dec_last wgrad", 64, ldl, M, a_mn=True, b_mn=True, lda=64, ldb=ldl))  # :227
+    for k in range(len(DEC) - 1, -1, -1):
+        H = 8 << k
+        for j in range(len(DEC[k]) - 1, -1, -1):
+            cin, cout = DEC[k][j]
+            nm = f"{tag}dec{k}.{j}"
+            out.append(op32("bn_bwd", nm, Gn, B * H * H, cout, 1))                                     # :237
+            if want_wgrad:
+                out.append(op32("bn_param_grad", nm, Gn, cout))                                        # :239
+            if j == 0:
+                C = cin // 2
+                _conv3_dgrad32(out, f"{nm}.D", N, H, cout, C)                                           # :245
+                if want_wgrad:
+                    _conv3_wgrad32(out, f"{nm}.D", N, H, cout, C)                                       # :248
+                if want_skip:
+                    out.append(op32("group_sum", f"{nm} skip sum", Gn, nskip, B * H * H * cout))       # :251
+                    _conv3_dgrad32(out, f"{nm}.S", nskip * B, H, cout, C)                               # :253
+                    if want_wgrad:
+                        _conv3_wgrad32(out, f"{nm}.S", nskip * B, H, cout, C)                           # :256
+            else:
+                _conv3_dgrad32(out, nm, N, H, cout, cin)                                                # :266
+                if want_wgrad:
+                    _conv3_wgrad32(out, nm, N, H, cout, cin)                                            # :269
+    out.append(op32("bn_bwd", f"{tag}dec-1", Gn, B * 16, 512, 1))                                      # engine.py:1140
+    if want_wgrad:
+        out.append(op32("bn_param_grad", f"{tag}dec-1", Gn, 512))
+        out.append(gemm32(f"{tag}dec-1 wgrad", 128, 16 * 512, N, a_mn=True, b_mn=True))
+    out.append(gemm32(f"{tag}dec-1 dgrad", N, 128, 16 * 512))
+
+
+def _backward32(T, B, S, nskip, W0, nc, has_cpc):
+    """decoder_backward(0, S), the CPC decoder_backward(S, S + 1) and encoder_backward (engine_vgg.py:274-305), in the order the
+    serial fp32 step enqueues them (engine.py:684-688)."""
+    ENC, DEC = vgg_tables(W0)
+    out = []
+    _decoder_backward32(out, DEC, S, B, nskip, W0, nc, True, True, "")
+    if has_cpc:
+        _decoder_backward32(out, DEC, 1, B, nskip, W0, nc, False, False, "cpc ")
+    N = T * B
+    out += [op32("bn_bwd", "enc_top", T, B, 128, 2), op32("bn_param_grad", "enc_top", T, 128),        # encode_top_backward
+            gemm32("enc_top wgrad", 128, 16 * 512, N, a_mn=True, b_mn=True), gemm32("enc_top dgrad", N, 16 * 512, 128, b_mn=True)]
+    for i in range(len(ENC) - 1, -1, -1):
+        H = W0 >> i
+        out.append(op32("add_indexed", f"enc{i} skip grad", nskip, B * H * H * ENC[i][-1][1]))          # :290
+        for j in range(len(ENC[i]) - 1, -1, -1):
+            cin, cout = ENC[i][j]
+            cin = nc if cin is None else cin
+            nm = f"enc{i}.{j}"
+            out += [op32("bn_bwd", nm, T, B * H * H, cout, 1), op32("bn_param_grad", nm, T, cout)]   # :296-297
+            _conv3_wgrad32(out, nm, N, H, cout, cin)                                                    # :300
+            if i > 0 or j > 0:
+                _conv3_dgrad32(out, nm, N, H, cout, cin)                                                # :304
     return out
 
 
@@ -390,6 +521,19 @@ def check_col2im3(col, y, N, H, W, C, ld, bias, name):
             ref += t
             mag += t.abs()
         worst = max(worst, bound_check(y[n0:n0 + n], ref, 9 * 2.0 ** -24 * mag + BETA[y.dtype] * ref.abs(), f"{name} col2im3 images [{n0}, ..)"))
+    return worst
+
+
+def check_gather_add(dst, dst0, src, grp_src, G, n, name=""):
+    """gather_add: dst[g] = dst0[g] + src[grp_src[g]] with one rounding to dst's dtype (a bf16 destination rounds twice: one
+    bf16 ulp), group by group against float64.  Returns the worst ratio."""
+    srcl = grp_src.tolist()[:G]
+    rel = 2.0 ** -7 if dst.dtype == torch.bfloat16 else 2.0 ** -24
+    dv, d0, sv = dst.reshape(-1)[:G * n].view(G, n), dst0.reshape(-1)[:G * n].view(G, n), src.reshape(-1)
+    worst = 0.0
+    for g in range(G):
+        ref = d0[g].double() + sv[srcl[g] * n:(srcl[g] + 1) * n].double()
+        worst = max(worst, bound_check(dv[g], ref, rel * ref.abs(), f"{name}: gather_add group {g}"))
     return worst
 
 
